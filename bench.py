@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Headline benchmark: image-text pairs/sec of one CLIP ViT-B/16 contrastive pre-training step (forward + loss +
-backward + gradient all-reduce + AdamW), bs=1024 per GPU, bf16 tensor-core math, synthetic 224x224x3 / 77-token data.
+backward + gradient all-reduce + AdamW), bs=512 per GPU (what fits an 80 GB H100), bf16 tensor-core math, synthetic 224x224x3 / 77-token data.
 
     python bench.py --gpus 1 --steps 5 --warmup 3                  # ours, one GPU
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -25,12 +25,12 @@ sys.path.insert(0, ROOT)
 # Algorithmic FLOPs per pair, CLIP ViT-B/16 (SURVEY.md §8d / BASELINE.md §5): forward 41.01 GF, step = 3x forward.
 F_FWD_B16 = 35.127e9 + 5.887e9
 F_STEP_B16 = 3.0 * F_FWD_B16
-METRIC = "image-text pairs/sec (CLIP ViT-B/16 contrastive pretrain step, bs=1024/GPU)"
+METRIC = "image-text pairs/sec (CLIP ViT-B/16 contrastive pretrain step, bs=512/GPU)"
 # BASELINE.json configs[3] (a parity / capability case, not the headline line): CLIP ViT-L/14, 4096 pairs per GPU
 # (global 32 768 on 8 GPUs), two-pass activation recompute in micro-batches.  SURVEY.md §8d: 175.22 GF forward per pair.
 F_STEP_L14 = 3.0 * (162.03e9 + 13.19e9)
 CONFIGS = {
-    "b16": {"builder": "clip_vit_b16", "f_step": F_STEP_B16, "batch": 1024, "micro_batch": None, "metric": METRIC,
+    "b16": {"builder": "clip_vit_b16", "f_step": F_STEP_B16, "batch": 512, "micro_batch": None, "metric": METRIC,
             "workload": "CLIP ViT-B/16 contrastive pretrain step (fwd+loss+bwd+grad-allreduce+AdamW)"},
     "l14": {"builder": "clip_vit_l14", "f_step": F_STEP_L14, "batch": 4096, "micro_batch": 256,
             "metric": "image-text pairs/sec (CLIP ViT-L/14 contrastive pretrain step, bs=4096/GPU, global 32768 on 8 GPUs)",
@@ -53,6 +53,9 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true",
                     help="skip the info-only same-box torch eager bf16-autocast leg of the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (loss, logit scale, seeded "
+                         "samples of the updated weights and Adam moments) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -61,7 +64,7 @@ def measured_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return float(d["bf16_tflops_sustained"]), float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json, sustained cuBLAS bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md: 1.4 PFLOP/s sustained)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16 989 TFLOP/s, HBM3 3.35 TB/s at 700 W), not measured"
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -138,7 +141,7 @@ def run_reference(args):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# Info-only leg: "what PyTorch gives today" on the same B200 (BASELINE.md §4, SURVEY.md §8d) — stock torch modules
+# Info-only leg: "what PyTorch gives today" on the same GPU (BASELINE.md §4, SURVEY.md §8d) — stock torch modules
 # (torch.nn.TransformerEncoder fast path, flash SDPA, cuBLAS), bf16 autocast, torch's fused AdamW, same batch.
 # None of this repo's kernels run here; it is context for the kernels' numbers, not an arm the driver scores.
 # ----------------------------------------------------------------------------------------------------------------
@@ -220,12 +223,12 @@ def run_torch_eager(args):
         return
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
-    r = torch_eager_gpu_run(args.batch or 1024, args.steps, args.warmup, dev)
+    r = torch_eager_gpu_run(args.batch or CONFIGS["b16"]["batch"], args.steps, args.warmup, dev)
     print(json.dumps({"impl": "torch-eager-gpu", "metric": METRIC, "value": r["value"], "unit": "pairs/s", "n_gpus": 1,
                       "steps": args.steps, "warmup": args.warmup, "ms_per_step": r["ms_per_step"], "higher_is_better": True,
                       "dtype": "bf16 autocast", "data": "synthetic",
-                      "config": {"workload": "CLIP ViT-B/16 contrastive pretrain step, stock PyTorch eager on the same B200",
-                                 "per_gpu_batch": r["per_gpu_batch"], "requested_batch": args.batch or 1024}, "detail": r}))
+                      "config": {"workload": "CLIP ViT-B/16 contrastive pretrain step, stock PyTorch eager on the same GPU",
+                                 "per_gpu_batch": r["per_gpu_batch"], "requested_batch": args.batch or CONFIGS["b16"]["batch"]}, "detail": r}))
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -279,6 +282,31 @@ class ClockSampler:
 # ----------------------------------------------------------------------------------------------------------------
 # our arm
 # ----------------------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 20   # elements per sampled array: 4 arrays x 4 MB, far below the 64 MB budget
+
+
+def dump_outputs(dirname, trainer, loss):
+    """What the timed step hands its caller: the loss, and the model / optimizer state it updated in place (the
+    logit scale in full; the flat fp32 master weights and Adam first moments of each tower as a fixed, seeded sample
+    of DUMP_SAMPLE positions).  Two builds run with the same arguments see identical inputs and weights, so their
+    dumps compare array for array."""
+    import numpy as np
+    import torch
+
+    os.makedirs(dirname, exist_ok=True)
+    torch.cuda.synchronize()
+    g = torch.Generator(device="cpu").manual_seed(0)
+    arrays = {"loss": loss.detach().double().reshape(1).cpu(), "logit_scale": trainer.ls.detach().double().reshape(-1).cpu()}
+    for tower, rt, opt in (("image", trainer.img, trainer.opt_img), ("text", trainer.txt, trainer.opt_txt)):
+        n = rt.store.master.numel()
+        idx = torch.randint(0, n, (min(DUMP_SAMPLE, n),), generator=g).sort().values.to(rt.store.master.device)
+        arrays[f"{tower}_weights_sample"] = rt.store.master.detach().view(-1)[idx].float().cpu()
+        arrays[f"{tower}_adam_m_sample"] = opt.m.detach().view(-1)[idx].float().cpu()
+        arrays[f"{tower}_sample_index"] = idx.double().cpu()
+    for name, t in arrays.items():
+        np.save(os.path.join(dirname, f"{name}.npy"), t.numpy())
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -358,6 +386,8 @@ def run_ours(args):
     ms_dev = max_over_ranks(e0.elapsed_time(e1) / args.steps)
     launches = (_lib.LAUNCHES - launches0) // args.steps
     final_loss = float(loss.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, loss)
 
     # ---- per-kernel-family breakdown: INSTR_STEPS more steps with every GEMM / attention / LayerNorm launch bracketed
     # by CUDA events on the launching stream (kept out of the region above: ~1000 event records per step) ----
@@ -448,23 +478,14 @@ def run_ours(args):
         burst_tf = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"])
     except Exception:  # noqa: BLE001
         pass
-    # DRAM traffic of the dominant kernel's benchmarked launch, from the committed `ncu --set full` capture
-    traffic, traffic_src = None, "no committed capture found (profiles/r2_ncu_kernels.json)"
-    try:
-        cap = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_kernels.json")))
-        k = cap["kernels"]["gemm_qkv_fwd"]
-        traffic = k["dram_bytes_read"] + k["dram_bytes_write"]
-        traffic_src = (f"{k['name']} {k['shape']}: dram__bytes_read.sum + dram__bytes_write.sum of ONE launch, "
-                       f"{cap['source']}; algorithmic bytes of that launch {k['algorithmic_bytes']:.4g}")
-    except Exception:  # noqa: BLE001
-        pass
+    traffic, traffic_src = None, "not measured"
     out = {
         "metric": cfg["metric"], "value": value, "unit": "pairs/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
         "data": "synthetic",
         "config": {"workload": cfg["workload"], "name": args.config, "micro_batch": MB,
                    "per_gpu_batch": B, "global_batch": B * world, "image": "224x224x3 fp32", "text_len": 77,
-                   "parallelism": f"dp{world}", "l2": "activations (~84 GB/step) and inputs (616 MB) exceed the 126 MB L2; no flush needed",
+                   "parallelism": f"dp{world}", "l2": "activations and inputs (308 MB at bs 512) exceed the 50 MB L2; no flush needed",
                    "final_loss": final_loss},
         "e2e": {"value": e2e_val, "unit": "pairs/s", "h2d_bytes_per_step": img_h.numel() * 4 + txt_h.numel() * 8,
                 "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e,
@@ -483,7 +504,7 @@ def run_ours(args):
                                    "recompute pass is NOT counted as useful work) / measured sustained bf16 peak",
                      "peak_source": peak_src,
                      "traffic": traffic, "traffic_launch": traffic_src,
-                     "dominant_kernel": "mmb::gemm_kernel (tcgen05, all instantiations)",
+                     "dominant_kernel": "mmb::gemm_kernel (wgmma, all instantiations)",
                      "by_kernel": by_kernel,
                      "by_kernel_note": f"CUDA events around every launch during {INSTR_STEPS} extra instrumented steps "
                                        f"({ms_instr:.1f} ms/step with the events) right after the timed region",

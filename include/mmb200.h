@@ -1,4 +1,4 @@
-/* libmmb200 — C ABI of the B200-native dual-encoder + contrastive-loss hot path.
+/* libmmb200 — C ABI of the H100-native (sm_90a) dual-encoder + contrastive-loss hot path.
  *
  * The reference (facebookresearch/multimodal) has no FFI: its hot path is Python calling
  * torch.nn.functional.  These entry points are what a maintainer would bind (ctypes; see
@@ -24,13 +24,13 @@ extern "C" {
 #define MMB_EPI_BF16 0      /* D0 = bf16(alpha*acc + bias)                                   */
 #define MMB_EPI_BF16_ACT 1  /* D0 = bf16(pre = alpha*acc + bias), D1 = bf16(act(D0))         */
 #define MMB_EPI_BF16_DACT 2 /* D0 = bf16(alpha*acc * act'(aux))                              */
-#define MMB_EPI_F32 3       /* D0 = fp32(alpha*acc + bias); reduce-add when split-K/accumulate */
+#define MMB_EPI_F32 3       /* D0 = fp32(alpha*acc + bias) (+ D0 when accumulate); split-K summed in a fixed order */
 #define MMB_ACT_QUICK_GELU 0 /* torchmultimodal/modules/layers/activation.py:12-25 ("SiLU")  */
 #define MMB_ACT_GELU_ERF 1   /* nn.GELU(), torchmultimodal/modules/layers/mlp.py             */
 
 int mmb_version(void);
 
-/* D[M,N] = alpha * A (x) B (+ bias[N]), bf16 operands, fp32 accumulation on tcgen05 tensor cores.
+/* D[M,N] = alpha * A (x) B (+ bias[N]), bf16 operands, fp32 accumulation on Hopper tensor cores (wgmma).
  *   a_mn_major = 0: A is [M,K] row-major (lda >= K);  1: A is stored [K,M] row-major (lda >= M)
  *   b_mn_major = 0: B is [N,K] row-major (ldb >= K);  1: B is stored [K,N] row-major (ldb >= N)
  * Replaces: F.linear in torch/nn/functional.py:6478 (in-proj), :6690 (out-proj),
@@ -46,15 +46,16 @@ int mmb_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, l
                   float* colsum, void* stream);
 
 /* Test / A-B hook (process-wide): force the kernel variant mmb_gemm_bf16 dispatches to.
- *   cta2: -1 = automatic (size heuristic), 0 = 1-CTA 128x256 tiles, 1 = CTA pairs (cta_group::2, 256x256 tiles);
- *   epilogue_warps: 0 = default, 8 or 16 = warps of the activation epilogues.  Returns MMB_ERR_ARG on other values.
+ *   cta2: -1 = automatic (size heuristic), 0 = one CTA per 128x128 tile, 1 = 2-CTA clusters (256x128 tiles, the B tile
+ *   multicast to both CTAs); epilogue_warps: 0 or 8 (the two consumer warpgroups run every epilogue).  Returns
+ *   MMB_ERR_ARG on other values.
  * No reference counterpart: it exists so the parity tests can drive both kernels over every operand / epilogue case. */
 int mmb_gemm_set_mode(int cta2, int epilogue_warps);
 
 /* ---- fused similarity GEMM + temperature-scaled cross-entropy: the logits never reach HBM ---------------------------
  * Replaces `torch.matmul(a, b_all.T) * exp(logit_scale)` + `F.cross_entropy` of
  * modules/losses/contrastive_loss_with_temperature.py:90-107 (and serves any Linear -> CrossEntropy head).
- * A [M,K], B [N,K] bf16 row-major; logits[m,n] = exp(*log_scale) * sum_k A[m,k] B[n,k] live in TMEM / registers only.
+ * A [M,K], B [N,K] bf16 row-major; logits[m,n] = exp(*log_scale) * sum_k A[m,k] B[n,k] live in registers only.
  *
  * mmb_gemm_ce_stats: online-softmax statistics.  For every row m and every 128-column part of this launch it writes one
  *   float4 {max, sum e^(x-max), sum e^(x-max) x, sum x} into part[m * part_ld + part0 + ...] (mmb_gemm_ce_num_parts(N)
@@ -111,7 +112,7 @@ int mmb_vit_embed_ln_fwd(const void* patch_out_bf16, const float* cls, const flo
                          const float* beta, float* x0, float* mean, float* rstd, int B, int S, int d, float eps,
                          void* stream);
 
-/* LayerNorm backward (+ residual-gradient add): g_out = (g_in?) + dLN/dx; dgamma/dbeta accumulated with atomics.
+/* LayerNorm backward (+ residual-gradient add): g_out = (g_in?) + dLN/dx; dgamma/dbeta accumulated (+=) in a fixed order.
  * dy is bf16 or fp32 (exactly one non-NULL).  Gather mode as in the forward: x/dy/mean/rstd are compact [M,d],
  * g_out/g_bf16 are scattered to the physical rows of a zero-initialised [*,d] buffer.
  * gsum (optional, needs g_bf16): gsum[c] += sum over rows of the bf16-rounded g — the bias gradient of the Linear layer
@@ -164,14 +165,14 @@ int mmb_memset_async(void* p, int value, long long bytes, void* stream);
 int mmb_act_fwd(const float* x, float* y, long long n, int kind, void* stream);
 
 /* ---- attention --------------------------------------------------------------------------------------------- */
-/* O = softmax(Q K^T * scale [+ causal mask]) V per (batch, head), head_dim 64, S <= 384 (tcgen05 kernels; larger S
+/* O = softmax(Q K^T * scale [+ causal mask]) V per (batch, head), head_dim 64, S <= 384 (tensor-core kernels; larger S
  * returns MMB_ERR_UNSUPPORTED); qkv bf16 [B*S, 3*H*64] packed [q|k|v], out bf16 [B*S, H*64], lse fp32 [B,H,S].  Replaces F.scaled_dot_product_attention (torch/nn/functional.py:6682). */
 int mmb_attention_fwd(const void* qkv, void* out, float* lse, int B, int S, int H, int head_dim, int causal,
                       float scale, void* stream);
 int mmb_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, int B, int S,
                       int H, int head_dim, int causal, float scale, void* stream);
-/* Number of kernels one mmb_attention_bwd call launches at sequence length S (1: fused single-pass kernel, S <= 256;
- * 2: dQ pass + dK/dV pass) — for callers that count launches. */
+/* Number of kernels one mmb_attention_bwd call launches at sequence length S (always 1: one kernel computes dQ, dK
+ * and dV) — for callers that count launches. */
 int mmb_attention_bwd_launches(int S);
 
 /* Same with a key-padding mask [B,S] (1 = attend, 0 = masked_fill(-inf)): the BERT-style attention of the FLAVA text
@@ -208,7 +209,7 @@ int mmb_concat_tokens(const float* cls, const float* a, const float* b, float* o
 
 
 /* ---- FLAVA encoders, backward (config 3 as a training step; autograd of the files cited on the forward entries) -- */
-/* Backward of mmb_attention_fwd_kmask (fused single-pass tcgen05 kernel, S <= 256): masked keys get P = dS = 0. */
+/* Backward of mmb_attention_fwd_kmask (S <= 384): masked keys get P = dS = 0. */
 int mmb_attention_bwd_kmask(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                             const unsigned char* kmask, int B, int S, int H, int head_dim, int causal, float scale,
                             void* stream);

@@ -1,4 +1,4 @@
-"""multimodal_b200 — B200-native dual-encoder forward + contrastive-loss hot path of TorchMultimodal."""
+"""multimodal_b200 — H100-native dual-encoder forward + contrastive-loss hot path of TorchMultimodal."""
 __version__ = "0.1.0"
 
 

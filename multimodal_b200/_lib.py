@@ -1,4 +1,4 @@
-"""Loader / builder for libmmb200.so, the C-ABI shared library holding every sm_100a kernel.
+"""Loader / builder for libmmb200.so, the C-ABI shared library holding every sm_90a kernel.
 
 The library is built in-tree (``multimodal_b200/libmmb200.so``) with plain ``nvcc`` so that it travels
 with the repository snapshot to the GPU box.  There is NO fallback: if the library is missing, or a
@@ -16,7 +16,7 @@ _CSRC = _HERE / "csrc"
 LIB_PATH = _HERE / "libmmb200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

@@ -7,7 +7,7 @@
 // head_dim 96 for ViT-L/14), the text decoder's [causal x padding] mask with its CLS row (models/coca/text_decoder.py
 // :141-162) and the multimodal decoder's cross-attention (modules/layers/transformer.py:354-377), i.e. the
 // F.scaled_dot_product_attention calls of modules/layers/multi_head_attention.py:74-76,171-173.  These are ~3 % of
-// CoCa's FLOPs; the ViT and causal self-attention layers stay on the tcgen05 kernels (attention_tc.cu).
+// CoCa's FLOPs; the ViT and causal self-attention layers stay on the head_dim-64 kernels (attention.cu).
 //
 // Math: softmax(Q K^T * scale + mask) V with fp32 statistics, P rounded to bf16 for the PV product.  A fully masked
 // query row yields zeros (SDPA would yield NaN; no caller on this path produces such a row).

@@ -1,4 +1,4 @@
-// Device-side PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
+// Device-side PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor, cluster multicast), wgmma, mma.sync.
 // Everything here is hand-written inline PTX; there is no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
@@ -85,6 +85,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// Same watchdog without the printf: a function call inside a wgmma pipeline makes ptxas serialise the wgmmas.
+__device__ __forceinline__ void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  uint32_t polls = 0;
+  uint64_t t0 = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++polls & 1023u) == 0) {
+      const uint64_t now = global_timer_ns();
+      if (t0 == 0) t0 = now;
+      else if (now - t0 > MMB_WATCHDOG_NS) __trap();
+    }
+  }
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA
 // ----------------------------------------------------------------------------------------------
@@ -102,14 +116,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-// Same, for CTA pairs: the smem destination is local, the barrier is the LEADER CTA's (peer bit cleared).
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint64_t* bar, void* smem, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(const CUtensorMap* m, uint64_t* bar, void* smem, int c0, int c1,
@@ -148,118 +154,90 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// Clusters
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// One elected lane of a converged warp.  Together with a warp index obtained through __shfl_sync (uniform_warp_idx)
-// this lets ptxas keep tcgen05.mma / TMA operands in uniform registers: code under `if (threadIdx-derived)` is treated
-// as divergent and every UTCHMMA / UTMALDG gets an ELECT + R2UR "waterfall" loop (~80 clocks per issue, measured in
-// round 1 and again in the round-2 phase traces), which starved the N = 64 attention MMAs (32 clocks each).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// 2-D tiled load global -> the same smem offset in every CTA of `cta_mask`; each destination's same-offset barrier
+// receives the complete_tx of the bytes that landed there.
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* m, uint64_t* bar, void* smem, int c0, int c1,
+                                                      uint16_t cta_mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
+      "%4}], [%2], %5;" ::"r"(smem_u32(smem)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// CTA-pair version: arrive on the same-offset barrier in every CTA of `cta_mask`.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread `lane` of the warp gets row (32*(warp%4)+lane), columns [c, c+32).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor")
+// wgmma (sm_90a warpgroup MMA): D[regs] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, SWIZZLE_128B, version 1 (sm_100).
+// Shared-memory matrix descriptor, SWIZZLE_128B (PTX ISA "Matrix Descriptor Format" for wgmma):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version = 1   [61,64) layout type (2 = SWIZZLE_128B)
+//   [32,46) stride-dim byte offset>>4 [62,64) layout type (1 = SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16: bf16 x bf16 -> fp32.
-//   [4,6) D format (1 = F32)  [7,10) A format (1 = BF16)  [10,13) B format (1 = BF16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// m64n128k16: the warpgroup's 64 x 128 fp32 accumulator, 64 registers per thread.  Thread (warp w, lane l) holds rows
+// 16w + l/4 (+8) and columns 8j + 2(l%4) (+1), j = 0..15: d[4j + 0..1] row 16w + l/4, d[4j + 2..3] row 16w + l/4 + 8.
+// TA / TB = 1: the operand is MN-major in shared memory.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+// ----------------------------------------------------------------------------------------------
+// mma.sync (warp-level tensor-core MMA) + ldmatrix
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -284,35 +262,6 @@ __device__ __forceinline__ float rcp_approx(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// ---- packed fp32 pairs (sm_100: FFMA2 / FADD2 / FMUL2 take one issue slot for two lanes' worth of FMA-pipe work; the
-// FMA-pipe time is unchanged — scripts/probes/tmem_probe.cu: 123 fma/clk/SM either way) and 3-input max (FMNMX3) ----
-__device__ __forceinline__ uint64_t pk2(float a, float b) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void upk2(uint64_t r, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(r)); }
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t fmul2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-
 // branch-free (no IEEE slow paths): the epilogue must keep 8+ independent elements in flight to hide MUFU latency
 __device__ __forceinline__ float fast_sigmoid(float z) {
   return rcp_approx(1.f + ex2_approx(-1.4426950408889634f * z));
@@ -333,25 +282,6 @@ __device__ __forceinline__ float quick_gelu_grad(float x) {
   const float u = 0.851f * x;
   const float t = tanh_approx(u);
   return fmaf(0.5f, fmaf(u, fmaf(-t, t, 1.f), t), 0.5f);
-}
-// Packed versions (two elements per FMA-pipe instruction): same formulas, same tanh.approx per element.
-__device__ __forceinline__ uint64_t tanh2(uint64_t u) {
-  float a, b;
-  upk2(u, a, b);
-  return pk2(tanh_approx(a), tanh_approx(b));
-}
-__device__ __forceinline__ uint64_t quick_gelu2(uint64_t x) {
-  const uint64_t t = tanh2(fmul2(x, pk2(0.851f, 0.851f))), h = fmul2(x, pk2(0.5f, 0.5f));
-  return ffma2(h, t, h);
-}
-__device__ __forceinline__ uint64_t quick_gelu_grad2(uint64_t x) {
-  const uint64_t u = fmul2(x, pk2(0.851f, 0.851f));
-  float t0, t1;
-  upk2(u, t0, t1);
-  t0 = tanh_approx(t0); t1 = tanh_approx(t1);
-  const uint64_t t = pk2(t0, t1);
-  const uint64_t w = ffma2(pk2(-t0, -t1), t, pk2(1.f, 1.f));           // 1 - t^2
-  return ffma2(pk2(0.5f, 0.5f), ffma2(u, w, t), pk2(0.5f, 0.5f));       // 0.5 (1 + t + u (1 - t^2))
 }
 // Exact (erf) GELU, as nn.GELU() in the FLAVA / CoCa MLPs (torchmultimodal/modules/layers/mlp.py:35)
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }

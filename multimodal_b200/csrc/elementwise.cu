@@ -4,13 +4,65 @@
 // for the grid-stride ones.
 #include "common.cuh"
 #include "mmb200_internal.h"
+#include <mutex>
 
 namespace mmb {
 
-__device__ __forceinline__ void red_add_v4(float* dst, const float4& v) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-               : "memory");
+// ---------------------------------------------------------------------------------------------
+// Deterministic reductions (mmb200_internal.h)
+// ---------------------------------------------------------------------------------------------
+struct ScratchEntry { int dev; cudaStream_t stream; int slot; void* ptr; size_t cap; };
+static ScratchEntry g_scratch[256];
+static int g_scratch_n = 0;
+static std::mutex g_scratch_mu;
+
+void* scratch(int slot, size_t bytes, cudaStream_t stream) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lk(g_scratch_mu);
+  ScratchEntry* e = nullptr;
+  for (int i = 0; i < g_scratch_n; ++i)
+    if (g_scratch[i].dev == dev && g_scratch[i].stream == stream && g_scratch[i].slot == slot) { e = &g_scratch[i]; break; }
+  if (!e) {
+    if (g_scratch_n == 256) return nullptr;
+    e = &g_scratch[g_scratch_n++];
+    *e = ScratchEntry{dev, stream, slot, nullptr, 0};
+  }
+  if (bytes > e->cap) {
+    if (e->ptr) cudaFree(e->ptr);
+    e->ptr = nullptr; e->cap = 0;
+    if (cudaMalloc(&e->ptr, bytes) != cudaSuccess) { e->ptr = nullptr; return nullptr; }
+    e->cap = bytes;
+  }
+  return e->ptr;
 }
+
+// block = 8 row groups x 32 columns; row group r sums rows r, r+8, r+16, ... in order, then the 8 group sums are added
+// in order: a fixed summation tree for every (P, N)
+__global__ void __launch_bounds__(256) reduce_partials_kernel(const float* __restrict__ part, int P, int N, long long ldp,
+                                                              float* __restrict__ out, int accumulate) {
+  const int col = threadIdx.x & 31, rg = threadIdx.x >> 5;
+  const int n = blockIdx.x * 32 + col;
+  float acc = 0.f;
+  if (n < N)
+    for (int p = rg; p < P; p += 8) acc += part[(long long)p * ldp + n];
+  __shared__ float s[8][33];
+  s[rg][col] = acc;
+  __syncthreads();
+  if (rg == 0 && n < N) {
+    float t = 0.f;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) t += s[r][col];
+    out[n] = accumulate ? out[n] + t : t;
+  }
+}
+
+int reduce_partials(const float* part, int P, int N, long long ldp, float* out, int accumulate, cudaStream_t stream) {
+  if (P <= 0 || N <= 0) return MMB_OK;
+  reduce_partials_kernel<<<(N + 31) / 32, 256, 0, stream>>>(part, P, N, ldp, out, accumulate);
+  return (int)cudaGetLastError();
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -310,17 +362,21 @@ __global__ void coca_text_embed_fwd_kernel(const long long* __restrict__ ids, co
 }
 
 // Cross-entropy over rows of fp32 logits [M, V] against int64 labels with ignore_index (nn.CrossEntropyLoss(
-// ignore_index=pad) of models/coca/coca_model.py:425,447-450): accum[0] += sum of row losses, accum[1] += #valid rows.
+// ignore_index=pad) of models/coca/coca_model.py:425,447-450): accum[0] += sum of row losses, accum[1] += #valid rows
+// (row i writes (loss, 1) or (0, 0) to part2[2i..]; the host wrapper sums them in row order).
 __global__ void __launch_bounds__(256) ce_labels_kernel(const float* __restrict__ logits, long long ld,
                                                         const long long* __restrict__ labels, long long label_stride,
                                                         long long ignore_index, int M, int V,
-                                                        float* __restrict__ row_loss, float* __restrict__ accum) {
+                                                        float* __restrict__ row_loss, float* __restrict__ part2) {
   __shared__ float red[8];
   const int i = blockIdx.x;
   if (i >= M) return;
   const long long lab = labels[(long long)i * label_stride];
   if (lab == ignore_index) {
-    if (threadIdx.x == 0 && row_loss) row_loss[i] = 0.f;
+    if (threadIdx.x == 0) {
+      if (row_loss) row_loss[i] = 0.f;
+      part2[2 * i] = 0.f; part2[2 * i + 1] = 0.f;
+    }
     return;
   }
   if (lab < 0 || lab >= V) __trap();
@@ -345,8 +401,7 @@ __global__ void __launch_bounds__(256) ce_labels_kernel(const float* __restrict_
     for (int w = 0; w < 8; ++w) t += red[w];
     const float loss = mx + logf(t) - row[lab];
     if (row_loss) row_loss[i] = loss;
-    atomicAdd(accum, loss);
-    atomicAdd(accum + 1, 1.f);
+    part2[2 * i] = loss; part2[2 * i + 1] = 1.f;
   }
 }
 
@@ -433,13 +488,14 @@ struct LnBwdArgs {
   const float* g_in; float* g_out; __nv_bfloat16* g_bf16;
   float* dgamma; float* dbeta;
   float* gsum;  // optional: gsum[c] += sum_rows bf16(g_out[row, c]) — the bias gradient of the Linear that consumes g_bf16
+  float* part;  // [3][gridDim.x][d] per-CTA column partials of dgamma / dbeta / gsum (reduced in a fixed order)
   const int* row_idx; int rows_per_group;
   int M, d;
 };
 
 // One CTA of NV warps per row (one float4 of the row per thread): ~20 live registers per thread, so 10-16 CTAs are
-// resident per SM and 60+ warps hide the HBM latency (the earlier warp-per-row version kept the whole row plus three
-// per-lane column accumulators in ~170 registers and ran at 12 warps per SM, latency-bound at ~65 % of HBM peak).
+// resident per SM and 60+ warps hide the HBM latency (a warp-per-row layout would keep the whole row plus three
+// per-lane column accumulators in ~170 registers and leave only 12 warps per SM to hide it).
 // The two row reductions cross the NV warps through a double-buffered smem slot: one __syncthreads per row.
 template <bool VIT, int NV>
 __global__ void __launch_bounds__(NV * 32, (1536 / (NV * 32) > 32 ? 32 : 1536 / (NV * 32))) ln_bwd_kernel(const LnBwdArgs a) {
@@ -515,36 +571,48 @@ __global__ void __launch_bounds__(NV * 32, (1536 / (NV * 32) > 32 ? 32 : 1536 / 
       }
     }
   }
-  // every thread owns 4 distinct columns: one vector reduction per output per CTA
-  if (a.dgamma) red_add_v4(a.dgamma + c, accg);
-  if (a.dbeta) red_add_v4(a.dbeta + c, accb);
-  if (want_gsum) red_add_v4(a.gsum + c, accs);
+  // every thread owns 4 distinct columns: this CTA's partial sums, reduced across CTAs in a fixed order afterwards
+  const long long plane = (long long)gridDim.x * d;
+  float* pp = a.part + (long long)blockIdx.x * d + c;
+  if (a.dgamma) *reinterpret_cast<float4*>(pp) = accg;
+  if (a.dbeta) *reinterpret_cast<float4*>(pp + plane) = accb;
+  if (want_gsum) *reinterpret_cast<float4*>(pp + 2 * plane) = accs;
 }
 
 template <bool VIT>
-static int launch_ln_bwd(const LnBwdArgs& a, cudaStream_t st) {
+static int launch_ln_bwd(LnBwdArgs a, cudaStream_t st) {
   const int nv = a.d >> 7;
   const int threads = nv * 32;
   int per_sm = 1536 / threads;   // matches the kernel's __launch_bounds__ (<= 42 registers per thread)
   if (per_sm > 24) per_sm = 24;
   int grid = num_sms() * per_sm;
   if (grid > a.M) grid = a.M;
-  if ((reinterpret_cast<uintptr_t>(a.dgamma) | reinterpret_cast<uintptr_t>(a.dbeta) | reinterpret_cast<uintptr_t>(a.gsum)) & 15)
-    return MMB_ERR_ARG;  // vector reductions
+  if (grid < 1) return MMB_ERR_ARG;
+  const bool any_col = a.dgamma || a.dbeta || a.gsum;
+  if (any_col) {
+    a.part = static_cast<float*>(scratch(SCR_LN_BWD, 3ull * grid * a.d * sizeof(float), st));
+    if (!a.part) return (int)cudaErrorMemoryAllocation;
+  }
   switch (nv) {
 #define LNB(NVV) case NVV: ln_bwd_kernel<VIT, NVV><<<grid, threads, 0, st>>>(a); break;
     LNB(1) LNB(2) LNB(3) LNB(4) LNB(5) LNB(6) LNB(7) LNB(8)
 #undef LNB
     default: return MMB_ERR_UNSUPPORTED;
   }
-  return (int)cudaGetLastError();
+  int rc = (int)cudaGetLastError();
+  const long long plane = (long long)grid * a.d;
+  float* outs[3] = {a.dgamma, a.dbeta, a.gsum};
+  for (int i = 0; i < 3 && rc == 0; ++i)
+    if (outs[i]) rc = reduce_partials(a.part + i * plane, grid, a.d, a.d, outs[i], 1, st);
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------
 // out[j] += sum_b in[b, j]   (positional-embedding / cls-token gradients: sum over the batch)
 //   in fp32 [Bn, n] with row stride ld; columns [0,n) ; optional row subset via (row0, row_step)
 // ---------------------------------------------------------------------------------------------
-__global__ void batch_sum_kernel(const float* __restrict__ in, float* __restrict__ out, int Bn, long long ld, int n,
+// Each blockIdx.y writes its chunk's sums to part[blockIdx.y][n]; reduce_partials adds the chunks in order.
+__global__ void batch_sum_kernel(const float* __restrict__ in, float* __restrict__ part, int Bn, long long ld, int n,
                                  int b_chunk) {
   const int j = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (j >= n) return;
@@ -554,13 +622,14 @@ __global__ void batch_sum_kernel(const float* __restrict__ in, float* __restrict
     const float4 v = *reinterpret_cast<const float4*>(in + (long long)b * ld + j);
     acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
   }
-  atomicAdd(out + j, acc.x); atomicAdd(out + j + 1, acc.y); atomicAdd(out + j + 2, acc.z); atomicAdd(out + j + 3, acc.w);
+  *reinterpret_cast<float4*>(part + (long long)blockIdx.y * n + j) = acc;
 }
 
 // ---------------------------------------------------------------------------------------------
 // out[n] += sum_m x[m, n]   (bias gradients), x bf16 [M, N] row-major with leading dim ld
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out,
+// Each blockIdx.y writes its row chunk's sums to part[blockIdx.y][N]; reduce_partials adds the chunks in order.
+__global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ part,
                                                           int M, int N, long long ld, int rows_per_block) {
   // block = 256 threads: 32 column-octets (256 columns) x 8 row lanes; 4 independent 16 B loads in flight per thread
   const int co = threadIdx.x & 31, rl = threadIdx.x >> 5;
@@ -595,7 +664,7 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* _
       float t = 0.f;
 #pragma unroll
       for (int r = 0; r < 8; ++r) t += s[r][co][e];
-      atomicAdd(out + n + e, t);
+      part[(long long)blockIdx.y * N + n + e] = t;
     }
   }
 }
@@ -621,20 +690,39 @@ __global__ void text_embed_fwd_kernel(const long long* __restrict__ tokens, cons
     reinterpret_cast<float4*>(x)[i] = make_float4(e.x + p.x, e.y + p.y, e.z + p.z, e.w + p.w);
   }
 }
-// demb[token[b,s],:] += g[b,s,:]  (fp32 atomics; dpos is produced by batch_sum)
-__global__ void text_embed_bwd_kernel(const long long* __restrict__ tokens, const float* __restrict__ g,
-                                      float* __restrict__ demb, int B, int S, int d) {
+// demb[token[b,s],:] += g[b,s,:]  (dpos is produced by batch_sum).  Deterministic without atomics: CTA k owns the
+// token ids t with t % gridDim.x == k, walks all B*S rows in order (a ballot per 32 rows finds its own) and adds
+// each of its rows into the table with plain read-modify-writes, so every table row is summed in row order by one CTA.
+__global__ void __launch_bounds__(256) text_embed_bwd_kernel(const long long* __restrict__ tokens, const float* __restrict__ g,
+                                                             float* __restrict__ demb, int rows, int d) {
+  __shared__ long long tok[256];
+  __shared__ unsigned mask[8];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int d4 = d >> 2;
-  const long long total = (long long)B * S * d4;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % d4);
-    const long long row = i / d4;
-    const long long tok = tokens[row];
-    const float4 v = reinterpret_cast<const float4*>(g)[i];
-    float* dst = demb + tok * d + c * 4;
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                 : "memory");
+  for (int r0 = 0; r0 < rows; r0 += 256) {
+    const int r = r0 + threadIdx.x;
+    const long long t = r < rows ? tokens[r] : -1;
+    const bool mine = r < rows && (int)((unsigned long long)t % gridDim.x) == (int)blockIdx.x;
+    tok[threadIdx.x] = t;
+    const unsigned m = __ballot_sync(0xffffffffu, mine);
+    if (lane == 0) mask[w] = m;
+    __syncthreads();
+    for (int ww = 0; ww < 8; ++ww) {
+      unsigned mm = mask[ww];
+      while (mm) {
+        const int i = ww * 32 + __ffs(mm) - 1;
+        mm &= mm - 1;
+        const float4* src = reinterpret_cast<const float4*>(g + (long long)(r0 + i) * d);
+        float4* dst = reinterpret_cast<float4*>(demb + tok[i] * d);
+        for (int c = threadIdx.x; c < d4; c += blockDim.x) {
+          const float4 v = src[c];
+          float4 o = dst[c];
+          o.x += v.x; o.y += v.y; o.z += v.z; o.w += v.w;
+          dst[c] = o;
+        }
+      }
+    }
+    __syncthreads();
   }
 }
 // idx[b] = argmax_s tokens[b,s] (first maximum, like torch.argmax)  (models/clip/text_encoder.py:130-132)
@@ -883,8 +971,11 @@ extern "C" int mmb_batch_sum(const float* in, float* out, int Bn, long long ld, 
   if (chunks < 1) chunks = 1;
   const int b_chunk = (Bn + chunks - 1) / chunks;
   dim3 grid(bx, (Bn + b_chunk - 1) / b_chunk);
-  batch_sum_kernel<<<grid, 128, 0, ST(stream)>>>(in, out, Bn, ld, n, b_chunk);
-  return LAUNCH_RC();
+  float* part = static_cast<float*>(scratch(SCR_BATCH_SUM, (size_t)grid.y * n * sizeof(float), ST(stream)));
+  if (!part) return (int)cudaErrorMemoryAllocation;
+  batch_sum_kernel<<<grid, 128, 0, ST(stream)>>>(in, part, Bn, ld, n, b_chunk);
+  const int rc = LAUNCH_RC();
+  return rc ? rc : reduce_partials(part, (int)grid.y, n, n, out, 1, ST(stream));
 }
 
 extern "C" int mmb_colsum_bf16(const void* x, float* out, int M, int N, long long ld, void* stream) {
@@ -894,8 +985,11 @@ extern "C" int mmb_colsum_bf16(const void* x, float* out, int M, int N, long lon
   int rows_per_block = (M + chunks - 1) / chunks;
   rows_per_block = ((rows_per_block + 7) / 8) * 8;
   dim3 grid(bx, (M + rows_per_block - 1) / rows_per_block);
-  colsum_bf16_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, M, N, ld, rows_per_block);
-  return LAUNCH_RC();
+  float* part = static_cast<float*>(scratch(SCR_COLSUM, (size_t)grid.y * N * sizeof(float), ST(stream)));
+  if (!part) return (int)cudaErrorMemoryAllocation;
+  colsum_bf16_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)x, part, M, N, ld, rows_per_block);
+  const int rc = LAUNCH_RC();
+  return rc ? rc : reduce_partials(part, (int)grid.y, N, N, out, 1, ST(stream));
 }
 
 extern "C" int mmb_text_embed_fwd(const long long* tokens, const float* emb, const float* pos, float* x, int B, int S,
@@ -907,7 +1001,7 @@ extern "C" int mmb_text_embed_fwd(const long long* tokens, const float* emb, con
 extern "C" int mmb_text_embed_bwd(const long long* tokens, const float* g, float* demb, int B, int S, int d,
                                   void* stream) {
   if (d & 3) return MMB_ERR_ARG;
-  text_embed_bwd_kernel<<<grid_for((long long)B * S * d / 4, 256), 256, 0, ST(stream)>>>(tokens, g, demb, B, S, d);
+  text_embed_bwd_kernel<<<num_sms() * 4, 256, 0, ST(stream)>>>(tokens, g, demb, B * S, d);
   return LAUNCH_RC();
 }
 extern "C" int mmb_argmax_tokens(const long long* tokens, int* idx, int B, int S, void* stream) {
@@ -964,8 +1058,11 @@ extern "C" int mmb_coca_text_embed_fwd(const long long* ids, const float* emb, c
 extern "C" int mmb_ce_labels(const float* logits, long long ld, const long long* labels, long long label_stride,
                              long long ignore_index, int M, int V, float* row_loss, float* accum, void* stream) {
   if (M <= 0 || V <= 0 || !accum) return MMB_ERR_ARG;
-  ce_labels_kernel<<<M, 256, 0, ST(stream)>>>(logits, ld, labels, label_stride, ignore_index, M, V, row_loss, accum);
-  return LAUNCH_RC();
+  float* part2 = static_cast<float*>(scratch(SCR_LOSS, 2ull * M * sizeof(float), ST(stream)));
+  if (!part2) return (int)cudaErrorMemoryAllocation;
+  ce_labels_kernel<<<M, 256, 0, ST(stream)>>>(logits, ld, labels, label_stride, ignore_index, M, V, row_loss, part2);
+  const int rc = LAUNCH_RC();
+  return rc ? rc : reduce_partials(part2, M, 2, 2, accum, 1, ST(stream));
 }
 extern "C" int mmb_gather_rows_cast(const float* x, void* out_bf16, int B, int rows_per_group, int row, int d,
                                     void* stream) {

@@ -1,5 +1,5 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a: TMA -> smem ring -> tcgen05.mma (TMEM accumulators)
-// -> epilogue warps (tcgen05.ld -> registers -> swizzled smem slab -> TMA store / TMA reduce-add).
+// Persistent warp-specialised bf16 GEMM for sm_90a: TMA -> smem ring -> wgmma (register accumulators) -> fused epilogue
+// straight from the accumulator registers.
 //
 // One kernel covers every dense contraction on the dual-encoder path:
 //   forward linears   y = x W^T      A K-major [M,K],  B K-major [N,K]      (torch/nn/functional.py:6478,6690;
@@ -8,9 +8,12 @@
 //   wgrad             dW = dy^T x    A MN-major [tokens,N'], B MN-major [tokens,K']   (split-K, fp32 reduce-add)
 //   logits            a b^T * T      (modules/losses/contrastive_loss_with_temperature.py:90-95)
 //
-// Tile: BLOCK_M=128 x BLOCK_N=256 x BLOCK_K=64, 4-stage smem ring (48 KB/stage), 2 TMEM accumulator stages
-// (2 x 256 fp32 columns = all 512 TMEM columns) so the epilogue of tile i overlaps the MMAs of tile i+1.
-// Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc), warps 2..9 = epilogue (two column halves).
+// Tile: BLOCK_M=128 x BLOCK_N=128 x BLOCK_K=64 per CTA, 6-stage smem ring (32 KB/stage).  Warp roles: warpgroup 0 =
+// TMA producer (one elected thread), warpgroups 1 and 2 = consumers, each owning 64 rows of the tile (wgmma m64n128k16,
+// 64 fp32 accumulator registers per thread) and running the epilogue of its rows.  While the consumers run an epilogue
+// the producer is already filling the ring with the next tile's k-blocks.
+// Cluster mode (CLU): two CTAs of a cluster compute a 256 x 128 tile; each loads its own 128 rows of A and HALF of
+// the B tile, multicast into both CTAs' shared memory, which halves the L2 -> SM traffic for B.
 #include "common.cuh"
 #include "mmb200_internal.h"
 #include <stdlib.h>
@@ -19,27 +22,15 @@
 namespace mmb {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = 256;
+constexpr int BLOCK_N = 128;
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int ACC_STAGES = 2;
-constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB per CTA
-// 1-CTA mode: each CTA loads the whole 256-row B tile (32 KB), 4 stages.  CTA-pair mode (cta_group::2, 256x256 tile
-// per pair): each CTA loads its 128 rows of A and HALF of B (16 KB), 6 stages; the pair's MMA reads B from both CTAs'
-// shared memory, which halves the per-SM shared-memory and L2->SM traffic per flop.
-template <bool CTA2, int EPI> struct Cfg {
-  static constexpr int LOAD_N = CTA2 ? 128 : 256;
-  static constexpr int B_BYTES = LOAD_N * BLOCK_K * 2;
-  // The activation epilogues give one ring stage (32 / 48 KB) to two more 16 KB slabs: EPI_BF16_DACT TMA-prefetches
-  // the act'(aux) operand into them while the tile's MMAs are still running; EPI_BF16_ACT alternates two
-  // (pre-activation, activation) slab pairs so that one named barrier per 64-column group suffices.
-  static constexpr int STAGES = (CTA2 ? 6 : 4) - ((EPI == EPI_BF16_DACT || EPI == EPI_BF16_ACT) ? 1 : 0);
-  static constexpr int TILE_M = CTA2 ? 256 : 128;
-};
-constexpr int SLAB_BYTES = 128 * 128;           // 128 rows x 128 B
-constexpr int NUM_SLABS = 2;
-constexpr int BIAS_BYTES = BLOCK_N * 4;          // the tile's bias slice, staged once per tile (bf16 epilogues)
-constexpr int GEMM_SMEM_BYTES = 1024 /*align slack*/ + 4 * (A_BYTES + 32768) + NUM_SLABS * SLAB_BYTES + BIAS_BYTES + 256;  // == 6 * (16K + 16K) + ...
+constexpr int WG_K = 16;
+constexpr int STAGES = 6;
+constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
+constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;   // 16 KB
+constexpr int GEMM_THREADS = 384;
+constexpr int COLSUM_SMEM = 8 * BLOCK_N * 4;    // per-warp column sums of the tile (bf16 epilogues with colsum)
+constexpr int GEMM_SMEM_BYTES = 1024 /*align slack*/ + STAGES * (A_BYTES + B_BYTES) + 256 + COLSUM_SMEM;
 
 struct GemmArgs {
   int M, N, K;
@@ -48,10 +39,12 @@ struct GemmArgs {
   const float* bias;          // [N] fp32 or nullptr
   const __nv_bfloat16* aux;   // EPI_DACT: pre-activation [M, ld_aux]
   long long ld_aux;
-  void* d0; void* d1;         // bf16 epilogues write with plain coalesced stores
+  void* d0; void* d1;
   long long ldd0, ldd1;
-  float* colsum;              // bf16 epilogues (not ACT): colsum[n] += sum_m bf16(D0[m,n]) (bias gradient), or nullptr
-  int reduce_add;             // fp32 epilogue: TMA reduce-add instead of store
+  float* colsum_part;         // bf16 epilogues (not ACT), or nullptr: [ceil(M/128)][N] column sums of bf16(D0) per
+                              // 128-row block; the host adds them into colsum[n] in block order (bias gradient)
+  float* splitk_ws;           // fp32 epilogue with split-K: [splits][M][N] partial products, reduced in split order
+  int accumulate;             // fp32 epilogue without split-K: D0 += result (one writer per element)
   // ---- temperature-scaled cross-entropy epilogues (EPI_CE_STATS / EPI_CE_GRAD): logits = exp(*ce_log_scale) * acc
   // are consumed in registers and never written to HBM (contrastive_loss_with_temperature.py:90-107)
   const float* ce_log_scale;  // device scalar (logit_scale parameter)
@@ -71,80 +64,44 @@ struct GemmArgs {
   float* ce_xlabel;           // CE_STATS: [M] logit at the label column
 };
 
-template <int NT> __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
-__device__ __forceinline__ void half_bar_sync(int h) { asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory"); }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+__device__ __forceinline__ void store_bf16x2(void* base, long long ld, int m, int n, float a, float b) {
+  *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(base) + (long long)m * ld + n) = pack_bf16x2(a, b);
 }
 
-// EW = epilogue warps: 8 (thread == row x column half) or, for the activation epilogues whose per-element math
-// (MUFU + ~8 FP32 ops) two warps per scheduler cannot hide, 16 (thread == row x column quarter).
-template <bool A_MN, bool B_MN, int EPI, int ACT, bool CTA2, int EW>
-__global__ void __launch_bounds__(64 + EW * 32, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmD0, const __grid_constant__ CUtensorMap tmD1, const GemmArgs p) {
+template <bool A_MN, bool B_MN, int EPI, int ACT, bool CLU>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024 B alignment for the 128B-swizzle atoms; pointer arithmetic on the __shared__ array keeps the address
-  // space known to the compiler (LDS/STS instead of generic LD/ST).
+  // 1024 B alignment for the 128B-swizzle atoms (identical offset in both CTAs of a cluster: the multicast target)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr int STAGES = Cfg<CTA2, EPI>::STAGES, B_BYTES = Cfg<CTA2, EPI>::B_BYTES, LOAD_N = Cfg<CTA2, EPI>::LOAD_N;
-  constexpr int TILE_M = Cfg<CTA2, EPI>::TILE_M;
-  const uint32_t rank = CTA2 ? cluster_ctarank() : 0u;   // 0 = leader of the CTA pair (issues the MMAs)
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint8_t* sSlab = smem + STAGES * (A_BYTES + B_BYTES);
-  uint8_t* sAux = sSlab + NUM_SLABS * SLAB_BYTES;   // 2 more slabs: EPI_BF16_DACT (aux prefetch) / EPI_BF16_ACT (2nd pair)
-  constexpr bool FOUR_SLABS = (EPI == EPI_BF16_DACT || EPI == EPI_BF16_ACT);
-  float* sBias = reinterpret_cast<float*>(sSlab + (FOUR_SLABS ? 2 : 1) * NUM_SLABS * SLAB_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sBias) + BIAS_BYTES);
-  uint64_t* full_bar = bars;                   // [STAGES]
-  uint64_t* empty_bar = bars + STAGES;         // [STAGES]
-  uint64_t* tfull_bar = bars + 2 * STAGES;     // [ACC_STAGES]
-  uint64_t* tempty_bar = bars + 2 * STAGES + ACC_STAGES;  // [ACC_STAGES]
-  uint64_t* aux_bar = bars + 2 * STAGES + 2 * ACC_STAGES;  // [2] aux slab landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * ACC_STAGES + 2);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));   // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                                  // [STAGES]
+  float* sCol = reinterpret_cast<float*>(smem + STAGES * (A_BYTES + B_BYTES) + 256);        // [8 warps][BLOCK_N]
+  constexpr int TILE_M = CLU ? 2 * BLOCK_M : BLOCK_M;
+  const uint32_t rank = CLU ? cluster_ctarank() : 0u;
+  const int wg = threadIdx.x >> 7;
 
-  const int warp = uniform_warp_idx();   // warp-uniform for ptxas: the issue loops below keep their operands in URs
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmD0);
-    if (EPI == EPI_BF16_ACT) tma_prefetch_desc(&tmD1);
-    if (EPI == EPI_BF16_DACT) { tma_prefetch_desc(&tmD1); mbar_init(&aux_bar[0], 1); mbar_init(&aux_bar[1], 1); }
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < ACC_STAGES; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], CTA2 ? 2 * EW : EW);  // one arrive per epilogue warp (of both CTAs of a pair)
+      mbar_init(&empty_bar[i], CLU ? 4 : 2);   // one arrive per consumer warpgroup (of both CTAs of a cluster)
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if (CTA2) tmem_alloc_2sm(tmem_slot, ACC_STAGES * BLOCK_N);
-    else      tmem_alloc(tmem_slot, ACC_STAGES * BLOCK_N);
-  }
-  tc_fence_before();
-  if (CTA2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CLU) cluster_sync_all(); else __syncthreads();
 
   const int tiles_mn = p.m_tiles * p.n_tiles;
   const int total_tiles = tiles_mn * p.splits;
-  const int tile_first = CTA2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = CTA2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int tile_first = CLU ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+  const int tile_step = CLU ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = tile_first; t < total_tiles; t += tile_step) {
@@ -153,386 +110,252 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int m_blk = rem / p.n_tiles, n_blk = rem - m_blk * p.n_tiles;
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
+        const int m_row = m_blk * TILE_M + (int)rank * BLOCK_M;
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          // CTA pair: only the leader arms its full barrier, with the bytes of BOTH CTAs; the peer's TMA loads
-          // complete_tx on the leader's barrier (cta_group::2 form).
-          if (!CTA2) mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
-          else if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * (A_BYTES + B_BYTES));
+          mbar_wait_quiet(&empty_bar[stage], phase ^ 1);
+          // the B bytes of both CTAs' multicast halves land here too
+          mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
           uint8_t* a_dst = sA + stage * A_BYTES;
           uint8_t* b_dst = sB + stage * B_BYTES;
-          const int m_row = m_blk * TILE_M + (int)rank * BLOCK_M;
-          const int n_row = n_blk * BLOCK_N + (int)rank * LOAD_N;
-          auto ld = [&](const CUtensorMap* m, void* dst, int c0, int c1) {
-            if (CTA2) tma_load_2d_2sm(m, &full_bar[stage], dst, c0, c1);
-            else      tma_load_2d(m, &full_bar[stage], dst, c0, c1);
-          };
           if (!A_MN) {
-            ld(&tmA, a_dst, kb * BLOCK_K, m_row);
+            tma_load_2d(&tmA, &full_bar[stage], a_dst, kb * BLOCK_K, m_row);
           } else {
 #pragma unroll
-            for (int j = 0; j < BLOCK_M / 64; ++j) ld(&tmA, a_dst + j * (64 * BLOCK_K * 2), m_row + j * 64, kb * BLOCK_K);
+            for (int j = 0; j < BLOCK_M / 64; ++j)
+              tma_load_2d(&tmA, &full_bar[stage], a_dst + j * (64 * BLOCK_K * 2), m_row + j * 64, kb * BLOCK_K);
           }
-          if (!B_MN) {
-            ld(&tmB, b_dst, kb * BLOCK_K, n_row);
+          // B: K-major -> rows [n0, n0 + 128) of [N][K]; MN-major -> two 64-column boxes of [K][N], 8 KB apart.
+          // Either way one 8 KB half is box / row block `h` at byte offset h * 8192.
+          const int n0 = n_blk * BLOCK_N;
+          if (CLU) {
+            const int h = (int)rank;
+            if (!B_MN) tma_load_2d_multicast(&tmB, &full_bar[stage], b_dst + h * 8192, kb * BLOCK_K, n0 + h * 64, 3);
+            else       tma_load_2d_multicast(&tmB, &full_bar[stage], b_dst + h * 8192, n0 + h * 64, kb * BLOCK_K, 3);
           } else {
-#pragma unroll
-            for (int j = 0; j < LOAD_N / 64; ++j) ld(&tmB, b_dst + j * (64 * BLOCK_K * 2), n_row + j * 64, kb * BLOCK_K);
+            if (!B_MN) {
+              tma_load_2d(&tmB, &full_bar[stage], b_dst, kb * BLOCK_K, n0);
+            } else {
+              tma_load_2d(&tmB, &full_bar[stage], b_dst, n0, kb * BLOCK_K);
+              tma_load_2d(&tmB, &full_bar[stage], b_dst + 8192, n0 + 64, kb * BLOCK_K);
+            }
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(TILE_M, BLOCK_N, A_MN, B_MN);
-      // K-major SW128: 8-row groups 1024 B apart (SBO); LBO unused. MN-major SW128: 64-element MN blocks
-      // (one TMA box, BLOCK_K rows x 128 B) 8192 B apart (LBO); 8-row k groups 1024 B apart (SBO).
-      constexpr uint32_t A_LBO = A_MN ? 64 * BLOCK_K * 2 : 16, B_LBO = B_MN ? 64 * BLOCK_K * 2 : 16;
-      constexpr uint32_t A_KSTEP = A_MN ? (UMMA_K / 8) * 1024 : UMMA_K * 2;  // bytes per UMMA_K step
-      constexpr uint32_t B_KSTEP = B_MN ? (UMMA_K / 8) * 1024 : UMMA_K * 2;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int t = tile_first; t < total_tiles; t += tile_step) {
-        const int split = t / tiles_mn;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = make_smem_desc_sw128(smem_u32(sA + stage * A_BYTES), A_LBO, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES), B_LBO, 1024);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            if (CTA2)
-              umma_bf16_2sm(d_tmem, adesc + (uint64_t)((k * A_KSTEP) >> 4), bdesc + (uint64_t)((k * B_KSTEP) >> 4),
-                            idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else
-              umma_bf16(d_tmem, adesc + (uint64_t)((k * A_KSTEP) >> 4), bdesc + (uint64_t)((k * B_KSTEP) >> 4), idesc,
-                        (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // frees this smem stage (in both CTAs of a pair) once the MMAs above have read it
-          if (CTA2) umma_commit_2sm(&empty_bar[stage], 3); else umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        // accumulator complete -> epilogue (of both CTAs of a pair)
-        if (CTA2) umma_commit_2sm(&tfull_bar[acc], 3); else umma_commit(&tfull_bar[acc]);
-        if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
       }
     }
   } else {
-    // ===================== Epilogue (warps 2..9) =====================
-    // Thread == tile row (TMEM lane); the two warpgroups ("halves") split the columns so that every SM sub-partition
-    // has two epilogue warps to interleave (MUFU / tcgen05.ld latency hiding).
-    static_assert(EW == 8 || (EW == 16 && EPI != EPI_F32), "the fp32 epilogue is written for two column halves");
-    constexpr int NP = EW / 4;                // column parts per 64-column group
-    constexpr int CWE = 64 / NP;              // columns per thread per group (32 | 16)
-    constexpr int ENT = EW * 32;              // epilogue threads
-    const int q = warp & 3;                   // TMEM lane quadrant this warp may access
-    const int half = (warp - 2) >> 2;         // column part: 0: warps 2..5, 1: warps 6..9, (2, 3: warps 10..17)
-    const int row = q * 32 + lane;            // row of the tile owned by this thread
-    const int epi_tid = threadIdx.x - 64;     // 0..ENT-1
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int slab = 0;
-    uint32_t aux_phase = 0;  // bit b = parity of aux slab b
+    // ===================== Consumers: wgmma main loop + epilogue =====================
+    const int cw = wg - 1;                       // 64-row half of the CTA's tile
+    const int wq = (threadIdx.x >> 5) & 3;       // warp within the warpgroup: 16-row slice
+    const int lane = threadIdx.x & 31;
+    const int tq = lane & 3;
+    // K-major SW128: 8-row groups 1024 B apart (SBO), LBO unused.  MN-major SW128: 64-element MN blocks (one TMA box,
+    // BLOCK_K rows x 128 B) 8192 B apart (LBO); 8-row k groups 1024 B apart (SBO).
+    constexpr uint32_t A_KSTEP = A_MN ? (WG_K / 8) * 1024 : WG_K * 2;   // bytes per k16 step
+    constexpr uint32_t B_KSTEP = B_MN ? (WG_K / 8) * 1024 : WG_K * 2;
+    constexpr uint32_t B_LBO = B_MN ? 64 * BLOCK_K * 2 : 16;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[64];
     for (int t = tile_first; t < total_tiles; t += tile_step) {
       const int split = t / tiles_mn;
       const int rem = t - split * tiles_mn;
       const int m_blk = rem / p.n_tiles, n_blk = rem - m_blk * p.n_tiles;
-      const int m0 = m_blk * TILE_M + (int)rank * BLOCK_M, n0 = n_blk * BLOCK_N;
-      const bool add_bias = (p.bias != nullptr) && (split == 0);
-      if (EPI == EPI_BF16_DACT && epi_tid == 0) {
-        // prefetch the act' operand of the first two 64-column groups while this tile's MMAs are still in flight
+      const int kb0 = split * p.kb_per_split;
+      const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
+      int prev_stage = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait_quiet(&full_bar[stage], phase);
+        // this warpgroup's 64 rows of A: 64 K-major rows or one 64-wide MN box -- 8192 B in from the stage base either way
+        const uint64_t adesc = make_smem_desc_sw128(smem_u32(sA + stage * A_BYTES + cw * 8192), 16, 1024);
+        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sB + stage * B_BYTES), B_LBO, 1024);
+        wgmma_fence();
 #pragma unroll
-        for (int g = 0; g < 2; ++g)
-          if (n0 + g * 64 < p.N) {
-            mbar_arrive_expect_tx(&aux_bar[g], SLAB_BYTES);
-            tma_load_2d(&tmD1, &aux_bar[g], sAux + g * SLAB_BYTES, n0 + g * 64, m0);
-          }
-      }
-      constexpr bool IS_CE = (EPI == EPI_CE_STATS || EPI == EPI_CE_GRAD);
-      if (EPI != EPI_F32 && !IS_CE && p.bias != nullptr) {
-        // stage the tile's bias slice in shared memory (every reader of the previous tile's slice has passed that
-        // tile's last group barrier); global-load latency is taken here, under the MMAs, instead of in every group
-        if (epi_tid < BLOCK_N) sBias[epi_tid] = (add_bias && n0 + epi_tid < p.N) ? __ldg(p.bias + n0 + epi_tid) : 0.f;
-      }
-      if (EPI == EPI_CE_GRAD && p.ce_lse_col != nullptr) {   // column LSEs (log2 units) of the transposed term
-        if (epi_tid < BLOCK_N)
-          sBias[epi_tid] = (n0 + epi_tid < p.N) ? __ldg(p.ce_lse_col + n0 + epi_tid) * 1.4426950408889634f : 0.f;
-      }
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      if ((EPI != EPI_F32 && !IS_CE && p.bias != nullptr) || (EPI == EPI_CE_GRAD && p.ce_lse_col != nullptr))
-        epi_bar_sync<ENT>();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BLOCK_N;
-      // All TMEM reads of this accumulator stage are complete (tcgen05.wait::ld) -> hand it back to the MMA warp.
-      auto release_acc = [&]() {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (CTA2 && rank != 0) mbar_arrive_cluster(&tempty_bar[acc], 0);  // the leader's MMA warp owns the wait
-          else mbar_arrive(&tempty_bar[acc]);
+        for (int k = 0; k < BLOCK_K / WG_K; ++k)
+          wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + (uint64_t)((k * A_KSTEP) >> 4),
+                                                      bdesc + (uint64_t)((k * B_KSTEP) >> 4), (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        // keep one k-block of MMAs in flight; the one before it has read its stage -> release that stage
+        wgmma_wait<1>();
+        if (prev_stage >= 0 && threadIdx.x % 128 == 0) {
+          mbar_arrive(&empty_bar[prev_stage]);
+          if (CLU) mbar_arrive_cluster(&empty_bar[prev_stage], rank ^ 1u);
         }
-      };
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev_stage >= 0 && threadIdx.x % 128 == 0) {
+        mbar_arrive(&empty_bar[prev_stage]);
+        if (CLU) mbar_arrive_cluster(&empty_bar[prev_stage], rank ^ 1u);
+      }
 
+      // ---------------- epilogue: rows r[0], r[1] of this thread, columns n0 + 8j + 2tq (+1) ----------------
+      const int m0 = m_blk * TILE_M + (int)rank * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2);
+      const int r[2] = {m0, m0 + 8};
+      const int n0 = n_blk * BLOCK_N + 2 * tq;
+      const bool add_bias = (p.bias != nullptr) && (split == 0);
       if (EPI == EPI_CE_STATS) {
-        // Online softmax statistics of this thread's row over its columns of the tile; nothing but 16 B per
-        // (row, 128-column part) leaves the SM.  x = T * acc (natural-log logits); exponentials in base 2.
         const float T = __expf(__ldg(p.ce_log_scale));
         const float T2 = T * 1.4426950408889634f;
-        const int lab = p.ce_labels ? __ldg(p.ce_labels + min(m0 + row, p.M - 1)) : p.ce_label0 + m0 + row;
-        float m2 = -INFINITY, se = 0.f, sex = 0.f, sx = 0.f;
-        uint32_t vbuf[2][CWE];
-        auto ld_group = [&](int g, uint32_t (&v)[CWE]) {
-          if (CWE == 32) tmem_ld32(t_addr + g * 64 + half * 32, reinterpret_cast<uint32_t(&)[32]>(v));
-          else           tmem_ld16(t_addr + g * 64 + half * 16, reinterpret_cast<uint32_t(&)[16]>(v));
-        };
-        ld_group(0, vbuf[0]);
 #pragma unroll
-        for (int g = 0; g < BLOCK_N / 64; ++g) {
-          if (n0 + g * 64 >= p.N) break;
-          uint32_t (&v)[CWE] = vbuf[g & 1];
-          const int nb = n0 + g * 64 + half * CWE;
-          tmem_ld_wait();
-          if (g + 1 < BLOCK_N / 64 && n0 + (g + 1) * 64 < p.N) ld_group(g + 1, vbuf[(g + 1) & 1]);
-          else release_acc();
+        for (int i = 0; i < 2; ++i) {
+          const int lab = p.ce_labels ? __ldg(p.ce_labels + min(r[i], p.M - 1)) : p.ce_label0 + r[i];
           float gm = -INFINITY;
 #pragma unroll
-          for (int e = 0; e < CWE; ++e)
-            if (nb + e < p.N) gm = fmaxf(gm, __uint_as_float(v[e]));
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (n0 + 8 * j + e < p.N) gm = fmaxf(gm, acc[4 * j + 2 * i + e]);
+          float m2 = gm * T2, se = 0.f, sex = 0.f, sx = 0.f;
           if (gm > -INFINITY) {
-            const float gm2 = gm * T2;
-            if (gm2 > m2) {
-              const float rs = ex2_approx(m2 - gm2);   // m2 == -inf on the first group: 2^-inf = 0 (se, sex are 0 anyway)
-              se *= rs; sex *= rs; m2 = gm2;
-            }
 #pragma unroll
-            for (int e = 0; e < CWE; ++e) {
-              if (nb + e < p.N) {
-                const float a = __uint_as_float(v[e]);
-                const float x = a * T;
-                const float pe = ex2_approx(fmaf(a, T2, -m2));
-                se += pe; sex = fmaf(pe, x, sex); sx += x;
-                if (nb + e == lab && m0 + row < p.M) p.ce_xlabel[m0 + row] = x;
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * j + e;
+                if (n < p.N) {
+                  const float a = acc[4 * j + 2 * i + e];
+                  const float x = a * T;
+                  const float pe = ex2_approx(fmaf(a, T2, -m2));
+                  se += pe; sex = fmaf(pe, x, sex); sx += x;
+                  if (n == lab && r[i] < p.M) p.ce_xlabel[r[i]] = x;
+                }
               }
-            }
           }
-        }
-        if (m0 + row < p.M)
-          p.ce_part[(long long)(m0 + row) * p.ce_part_ld + p.ce_part0 + n_blk * NP + half] =
-              make_float4(m2 * 0.6931471805599453f, se, sex, sx);
-      } else if (EPI == EPI_F32) {
-        // fp32 output: a 32-column chunk is one 128 B x 128 row slab.  Half h owns chunks c == h (mod 2), slab h, named
-        // barrier 1+h and its own TMA bulk-group accounting (issued by its first thread).
-        const int htid = epi_tid & 127;
-        uint8_t* myslab = sSlab + half * SLAB_BYTES;
-        for (int c = half; c < BLOCK_N / 32; c += 2) {
-          if (n0 + c * 32 >= p.N) break;
-          uint32_t v[32];
-          tmem_ld32(t_addr + c * 32, v);
-          if (htid == 0) tma_store_wait_read<0>();
-          tmem_ld_wait();
-          half_bar_sync(half);
-          uint8_t* dst = myslab + row * 128;
+          // merge the four lanes of the quad (the row's 128 columns)
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 o;
-            const int n = n0 + c * 32 + j * 4;
-            float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (add_bias && n < p.N) bb = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-            o.x = __uint_as_float(v[j * 4 + 0]) * p.alpha + bb.x;
-            o.y = __uint_as_float(v[j * 4 + 1]) * p.alpha + bb.y;
-            o.z = __uint_as_float(v[j * 4 + 2]) * p.alpha + bb.z;
-            o.w = __uint_as_float(v[j * 4 + 3]) * p.alpha + bb.w;
-            *reinterpret_cast<float4*>(dst + ((j ^ (row & 7)) << 4)) = o;
+          for (int o = 1; o <= 2; o <<= 1) {
+            const float mo = __shfl_xor_sync(0xffffffffu, m2, o);
+            const float seo = __shfl_xor_sync(0xffffffffu, se, o);
+            const float sexo = __shfl_xor_sync(0xffffffffu, sex, o);
+            const float sxo = __shfl_xor_sync(0xffffffffu, sx, o);
+            const float mn = fmaxf(m2, mo);
+            const float f = (m2 == -INFINITY) ? 0.f : ex2_approx(m2 - mn);
+            const float fo = (mo == -INFINITY) ? 0.f : ex2_approx(mo - mn);
+            se = se * f + seo * fo; sex = sex * f + sexo * fo; sx += sxo; m2 = mn;
           }
-          fence_proxy_async_smem();
-          half_bar_sync(half);
-          if (htid == 0) {
-            if (p.reduce_add) tma_reduce_add_2d(&tmD0, myslab, n0 + c * 32, m0);
-            else              tma_store_2d(&tmD0, myslab, n0 + c * 32, m0);
-            tma_store_commit();
+          if (tq == 0 && r[i] < p.M)
+            p.ce_part[(long long)r[i] * p.ce_part_ld + p.ce_part0 + n_blk] = make_float4(m2 * 0.6931471805599453f, se, sex, sx);
+        }
+      } else if (EPI == EPI_F32) {
+        float* D = reinterpret_cast<float*>(p.d0);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int n = n0 + 8 * j;
+          if (n >= p.N) continue;
+          float b0 = 0.f, b1 = 0.f;
+          if (add_bias) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            if (r[i] >= p.M) continue;
+            const float v0 = fmaf(acc[4 * j + 2 * i], p.alpha, b0), v1 = fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1);
+            if (p.splitk_ws) {
+              float* dst = p.splitk_ws + ((long long)split * p.M + r[i]) * p.N + n;
+              dst[0] = v0; dst[1] = v1;
+            } else {
+              float* dst = D + (long long)r[i] * p.ldd0 + n;
+              if (p.accumulate) { dst[0] += v0; dst[1] += v1; }
+              else              { dst[0] = v0; dst[1] = v1; }
+            }
           }
         }
       } else {
-        // bf16 outputs.  Per 64-column group: each column part converts its columns (TMEM -> registers -> bias /
-        // activation / act' -> bf16) into a 128B-swizzled smem slab (thread == row); one named barrier; then ONE thread
-        // hands the slab to the TMA store engine (cp.async.bulk.tensor clips the M / N edges).  No LDS/STG copy-out: the
-        // epilogue warps only convert.  Slabs alternate (EPI_BF16_ACT: two (pre-activation, activation) pairs), the
-        // issuing thread drains its bulk-group reads before each barrier, so a slab is free again two groups later.
-        // The tcgen05.ld of group g+1 is issued before the math of group g, and the accumulator stage is handed back
-        // to the MMA warp as soon as the last load has landed in registers.
-        constexpr bool DUAL = (EPI == EPI_BF16_ACT);
-        constexpr int NG4 = BLOCK_N / 64;
-        uint32_t vbuf[2][CWE];
-        auto ld_group = [&](int g, uint32_t (&v)[CWE]) {
-          if (CWE == 32) tmem_ld32(t_addr + g * 64 + half * 32, reinterpret_cast<uint32_t(&)[32]>(v));
-          else           tmem_ld16(t_addr + g * 64 + half * 16, reinterpret_cast<uint32_t(&)[16]>(v));
-        };
-        // EPI_CE_GRAD: per-row constants of this thread's row
-        float ce_T = 0.f, ce_T2 = 0.f, ce_lse2 = 0.f, ce_gsT = 0.f, ce_gcT = 0.f, ce_eps_n = 0.f;
-        int ce_lab = -1;
+        // bf16 outputs.  EPI_CE_GRAD: per-row constants of this thread's two rows.
+        float ce_T = 0.f, ce_T2 = 0.f, ce_eps_n = 0.f, ce_gcT = 0.f;
+        float ce_lse2[2] = {0.f, 0.f}, ce_gsT[2] = {0.f, 0.f};
         if (EPI == EPI_CE_GRAD) {
-          const int gr = min(m0 + row, p.M - 1);
           ce_T = __expf(__ldg(p.ce_log_scale));
           ce_T2 = ce_T * 1.4426950408889634f;
-          ce_lse2 = __ldg(p.ce_lse_row + gr) * 1.4426950408889634f;
-          ce_gsT = ce_T * (p.ce_row_w ? p.ce_loss_weight * __ldg(p.ce_row_w + gr) : p.ce_gs);
           ce_gcT = ce_T * p.ce_gs;
           ce_eps_n = p.ce_smoothing / (float)p.ce_n_total;
-          ce_lab = p.ce_label0 + m0 + row;
-        }
-        ld_group(0, vbuf[0]);
 #pragma unroll
-        for (int g = 0; g < NG4; ++g) {
-          if (n0 + g * 64 >= p.N) break;
-          uint32_t (&v)[CWE] = vbuf[g & 1];
-          const int sl = DUAL ? 2 * slab : slab;              // slab (pair) of this group
-          uint8_t* slab0 = sSlab + sl * SLAB_BYTES;
-          uint8_t* dst0 = slab0 + row * 128;
-          uint8_t* dst1 = dst0 + SLAB_BYTES;
-          const int h = half;
-          const int nb = n0 + g * 64 + h * CWE;
-          uint4 auxv[CWE / 8];
-          if (EPI == EPI_BF16_DACT) {
-            mbar_wait(&aux_bar[g & 1], (aux_phase >> (g & 1)) & 1);
-            const uint8_t* arow = sAux + (g & 1) * SLAB_BYTES + row * 128;
-#pragma unroll
-            for (int j = 0; j < CWE / 8; ++j)
-              auxv[j] = *reinterpret_cast<const uint4*>(arow + (((h * (CWE / 8) + j) ^ (row & 7)) << 4));
+          for (int i = 0; i < 2; ++i) {
+            const int gr = min(r[i], p.M - 1);
+            ce_lse2[i] = __ldg(p.ce_lse_row + gr) * 1.4426950408889634f;
+            ce_gsT[i] = ce_T * (p.ce_row_w ? p.ce_loss_weight * __ldg(p.ce_row_w + gr) : p.ce_gs);
           }
-          tmem_ld_wait();
-          if (g + 1 < NG4 && n0 + (g + 1) * 64 < p.N) ld_group(g + 1, vbuf[(g + 1) & 1]);
-          else release_acc();                                 // every TMEM read of this stage is in registers
+        }
+        const bool do_colsum = (EPI == EPI_BF16 || EPI == EPI_BF16_DACT) && p.colsum_part != nullptr;
 #pragma unroll
-          for (int j = 0; j < CWE / 8; ++j) {  // 8 columns -> one 16 B chunk
-            float f[8];
+        for (int j = 0; j < 16; ++j) {
+          const int n = n0 + 8 * j;
+          const bool col_ok = n < p.N;
+          float b0 = 0.f, b1 = 0.f;
+          if (add_bias && col_ok) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+          float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const bool ok = col_ok && r[i] < p.M;
+            float f0, f1;
             if (EPI == EPI_CE_GRAD) {
               // d(loss_weight * mean CE) / d sims of this row block, plus (columns [col_lo, col_hi)) the transposed
-              // other-direction term rebuilt from the column LSEs — see contrastive_ce_grad_kernel (loss.cu)
+              // other-direction term rebuilt from the column LSEs -- see contrastive_ce_grad_kernel (loss.cu)
+              float f[2];
 #pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const int n = nb + j * 8 + e;
-                const float a = __uint_as_float(v[j * 8 + e]);
-                const float tt = ((n == ce_lab) ? (1.f - p.ce_smoothing) : 0.f) + ce_eps_n;
-                float gsum = ce_gsT * (ex2_approx(fmaf(a, ce_T2, -ce_lse2)) - tt);
-                if (p.ce_lse_col != nullptr && n >= p.ce_col_lo && n < p.ce_col_hi) {
-                  const float wc = p.ce_col_w ? p.ce_loss_weight * ce_T * __ldg(p.ce_col_w + min(n, p.N - 1)) : ce_gcT;
-                  if (wc != 0.f) gsum += wc * (ex2_approx(fmaf(a, ce_T2, -sBias[g * 64 + h * CWE + j * 8 + e])) - tt);
+              for (int e = 0; e < 2; ++e) {
+                const int c = n + e;
+                const float a = acc[4 * j + 2 * i + e];
+                const float tt = ((c == p.ce_label0 + r[i]) ? (1.f - p.ce_smoothing) : 0.f) + ce_eps_n;
+                float gsum = ce_gsT[i] * (ex2_approx(fmaf(a, ce_T2, -ce_lse2[i])) - tt);
+                if (p.ce_lse_col != nullptr && c >= p.ce_col_lo && c < p.ce_col_hi && c < p.N) {
+                  const float wc = p.ce_col_w ? p.ce_loss_weight * ce_T * __ldg(p.ce_col_w + c) : ce_gcT;
+                  if (wc != 0.f) gsum += wc * (ex2_approx(fmaf(a, ce_T2, -__ldg(p.ce_lse_col + c) * 1.4426950408889634f)) - tt);
                 }
                 f[e] = gsum;
               }
-            } else if (add_bias) {
-              const float4 b0 = *reinterpret_cast<const float4*>(sBias + g * 64 + h * CWE + j * 8);
-              const float4 b1 = *reinterpret_cast<const float4*>(sBias + g * 64 + h * CWE + j * 8 + 4);
-              const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = fmaf(__uint_as_float(v[j * 8 + e]), p.alpha, bb[e]);
+              f0 = f[0]; f1 = f[1];
             } else {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[j * 8 + e]) * p.alpha;
+              f0 = fmaf(acc[4 * j + 2 * i], p.alpha, b0);
+              f1 = fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1);
             }
-            if (EPI == EPI_BF16_DACT) {
-              const uint32_t a[4] = {auxv[j].x, auxv[j].y, auxv[j].z, auxv[j].w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                f[2 * e] *= act_grad<ACT>(bf16_lo(a[e]));
-                f[2 * e + 1] *= act_grad<ACT>(bf16_hi(a[e]));
+            if (EPI == EPI_BF16_DACT && ok) {
+              const uint32_t av = *reinterpret_cast<const uint32_t*>(p.aux + (long long)r[i] * p.ld_aux + n);
+              f0 *= act_grad<ACT>(bf16_lo(av));
+              f1 *= act_grad<ACT>(bf16_hi(av));
+            }
+            if (ok) {
+              const uint32_t o = pack_bf16x2(f0, f1);
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.d0) + (long long)r[i] * p.ldd0 + n) = o;
+              if (EPI == EPI_BF16_ACT) {
+                // the activation is applied to the bf16-ROUNDED pre-activation: exactly what the backward (which only
+                // sees the stored bf16 pre-activation) differentiates
+                store_bf16x2(p.d1, p.ldd1, r[i], n, act_fn<ACT>(bf16_lo(o)), act_fn<ACT>(bf16_hi(o)));
               }
+              if (do_colsum) { cs0 += bf16_lo(o); cs1 += bf16_hi(o); }
             }
-            uint4 o;
-            o.x = pack_bf16x2(f[0], f[1]);
-            o.y = pack_bf16x2(f[2], f[3]);
-            o.z = pack_bf16x2(f[4], f[5]);
-            o.w = pack_bf16x2(f[6], f[7]);
-            const int off = ((h * (CWE / 8) + j) ^ (row & 7)) << 4;
-            *reinterpret_cast<uint4*>(dst0 + off) = o;
-            if (DUAL) {
-              // The activation is applied to the bf16-ROUNDED pre-activation: exactly what the backward (which
-              // only sees the stored bf16 pre-activation) differentiates.
-              const uint32_t pr[4] = {o.x, o.y, o.z, o.w};
-              float a[8];
+          }
+          if (do_colsum) {
+            // column sums of the rounded output over the warp's 16 rows (lanes sharing tq) -> this warp's smem row
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                a[2 * e] = act_fn<ACT>(bf16_lo(pr[e]));
-                a[2 * e + 1] = act_fn<ACT>(bf16_hi(pr[e]));
-              }
-              uint4 oa;
-              oa.x = pack_bf16x2(a[0], a[1]);
-              oa.y = pack_bf16x2(a[2], a[3]);
-              oa.z = pack_bf16x2(a[4], a[5]);
-              oa.w = pack_bf16x2(a[6], a[7]);
-              *reinterpret_cast<uint4*>(dst1 + off) = oa;
+            for (int o = 4; o <= 16; o <<= 1) {
+              cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
+              cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
+            }
+            if (lane < 4) {
+              sCol[(cw * 4 + wq) * BLOCK_N + 8 * j + 2 * tq] = cs0;
+              sCol[(cw * 4 + wq) * BLOCK_N + 8 * j + 2 * tq + 1] = cs1;
             }
           }
-          fence_proxy_async_smem();                       // generic-proxy slab writes -> visible to the TMA engine
-          if (epi_tid == 0) tma_store_wait_read<0>();     // stores of the previous group have left their slab
-          epi_bar_sync<ENT>();
-          if (epi_tid == 0) {
-            tma_store_2d(&tmD0, slab0, n0 + g * 64, m0);
-            if (DUAL) tma_store_2d(&tmD1, slab0 + SLAB_BYTES, n0 + g * 64, m0);
-            tma_store_commit();
-          }
-          if (EPI == EPI_BF16_DACT) {
-            aux_phase ^= 1u << (g & 1);
-            if (epi_tid == 0 && g + 2 < NG4 && n0 + (g + 2) * 64 < p.N) {  // aux slab (g & 1) is free again
-              mbar_arrive_expect_tx(&aux_bar[g & 1], SLAB_BYTES);
-              tma_load_2d(&tmD1, &aux_bar[g & 1], sAux + (g & 1) * SLAB_BYTES, n0 + (g + 2) * 64, m0);
-            }
-          }
-          if (!DUAL && p.colsum != nullptr) {   // uniform
-            // Column sums of the tile's rounded output (the bias gradient of the layer whose dgrad this is), read back
-            // from the slab: thread -> (16 B chunk ch, rows r = it*(ENT/8) + tid/8); the 4 lanes of a warp that share
-            // a chunk fold with two shuffles, then lanes 0..7 fire two vector reds each.
-            const int ch = epi_tid & 7;
-            const int ncol = n0 + g * 64 + ch * 8;
-            float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        }
+        if (do_colsum) {
+          // the 8 consumer warps' sums in warp order -> one partial row per 128-row block (no atomics: the host reduces
+          // the blocks in order, so the result does not depend on which CTA finishes first)
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+          const int ct = threadIdx.x - 128, blk_row = m_blk * TILE_M + (int)rank * BLOCK_M;
+          if (ct < BLOCK_N && blk_row < p.M && n_blk * BLOCK_N + ct < p.N) {
+            float t = 0.f;
 #pragma unroll
-            for (int it = 0; it < 1024 / ENT; ++it) {
-              const int r = it * (ENT / 8) + (epi_tid >> 3);
-              const uint4 val = *reinterpret_cast<const uint4*>(slab0 + r * 128 + ((ch ^ (r & 7)) << 4));
-              if (m0 + r < p.M) {
-                cs[0] += bf16_lo(val.x); cs[1] += bf16_hi(val.x); cs[2] += bf16_lo(val.y); cs[3] += bf16_hi(val.y);
-                cs[4] += bf16_lo(val.z); cs[5] += bf16_hi(val.z); cs[6] += bf16_lo(val.w); cs[7] += bf16_hi(val.w);
-              }
-            }
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              cs[e] += __shfl_xor_sync(0xffffffffu, cs[e], 8);
-              cs[e] += __shfl_xor_sync(0xffffffffu, cs[e], 16);
-            }
-            if (lane < 8 && ncol < p.N) {
-              float* dst = p.colsum + ncol;
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(cs[0]), "f"(cs[1]), "f"(cs[2]),
-                           "f"(cs[3]) : "memory");
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4), "f"(cs[4]), "f"(cs[5]),
-                           "f"(cs[6]), "f"(cs[7]) : "memory");
-            }
+            for (int w = 0; w < 8; ++w) t += sCol[w * BLOCK_N + ct];
+            p.colsum_part[(long long)(blk_row / BLOCK_M) * p.N + n_blk * BLOCK_N + ct] = t;
           }
-          slab ^= 1;
+          asm volatile("bar.sync 1, 256;" ::: "memory");
         }
       }
-      if (EPI == EPI_F32) release_acc();   // fp32 path: after its last tcgen05.wait::ld
-      if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
     }
-    if ((epi_tid & 127) == 0) tma_store_wait_all<0>();
   }
-
-  __syncwarp();
-  tc_fence_before();
-  if (CTA2) cluster_sync_all(); else __syncthreads();  // pair: nobody exits / frees while the peer still signals it
-  if (warp == 1) {
-    tc_fence_after();
-    if (CTA2) tmem_dealloc_2sm(tmem_base, ACC_STAGES * BLOCK_N);
-    else      tmem_dealloc(tmem_base, ACC_STAGES * BLOCK_N);
-  }
+  // cluster: nobody exits while the peer may still multicast into it or arrive on its barriers
+  if (CLU) cluster_sync_all();
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -632,10 +455,9 @@ int num_sms() {
   return g_num_sms;
 }
 
-template <bool A_MN, bool B_MN, int EPI, int ACT, bool CTA2, int EW>
-static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tD0, const CUtensorMap& tD1,
-                       const GemmArgs& args, cudaStream_t stream) {
-  auto kfn = gemm_kernel<A_MN, B_MN, EPI, ACT, CTA2, EW>;
+template <bool A_MN, bool B_MN, int EPI, int ACT, bool CLU>
+static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const GemmArgs& args, cudaStream_t stream) {
+  auto kfn = gemm_kernel<A_MN, B_MN, EPI, ACT, CLU>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_BYTES);
@@ -645,7 +467,7 @@ static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
   const int total = args.m_tiles * args.n_tiles * args.splits;
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute attr[1];
-  if (CTA2) {
+  if (CLU) {
     const int clusters = total < num_sms() / 2 ? total : num_sms() / 2;
     cfg.gridDim = dim3(2 * clusters);
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -654,10 +476,10 @@ static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
   } else {
     cfg.gridDim = dim3(total < num_sms() ? total : num_sms());
   }
-  cfg.blockDim = dim3(64 + EW * 32);
+  cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = GEMM_SMEM_BYTES;
   cfg.stream = stream;
-  return (int)cudaLaunchKernelEx(&cfg, kfn, tA, tB, tD0, tD1, args);
+  return (int)cudaLaunchKernelEx(&cfg, kfn, tA, tB, args);
 }
 
 }  // namespace mmb
@@ -665,15 +487,33 @@ static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
 using namespace mmb;
 
 // Test / A-B hook: force the kernel variant mmb_gemm_bf16 dispatches to (process-wide).
-//   cta2: -1 = automatic (size heuristic / MMB_GEMM_CTA2), 0 = 1-CTA 128x256 tiles, 1 = CTA pairs (256x256 tiles)
-//   epilogue_warps: 0 = default (8 / MMB_GEMM_EW), 8 or 16 = activation-epilogue warps
-static int g_force_cta2 = -1, g_force_ew = 0;
+//   cta2: -1 = automatic (size heuristic), 0 = one CTA per 128x128 tile, 1 = 2-CTA clusters (256x128 tiles, B multicast)
+//   epilogue_warps: 0 or 8 (the two consumer warpgroups run the epilogue; kept for ABI compatibility)
+static int g_force_cta2 = -1;
 extern "C" int mmb_gemm_set_mode(int cta2, int epilogue_warps) {
-  if (cta2 < -1 || cta2 > 1 || (epilogue_warps != 0 && epilogue_warps != 8 && epilogue_warps != 16)) return MMB_ERR_ARG;
+  if (cta2 < -1 || cta2 > 1 || (epilogue_warps != 0 && epilogue_warps != 8)) return MMB_ERR_ARG;
   g_force_cta2 = cta2;
-  g_force_ew = epilogue_warps;
   return MMB_OK;
 }
+
+// D[m, n] = (accumulate ? D[m, n] : 0) + sum_{s = 0..S-1} ws[s][m][n], splits added in order (N % 4 == 0)
+__global__ void splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int N, float* __restrict__ D, long long ldd,
+                                     int accumulate) {
+  const int n = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (n >= N) return;
+  for (int m = blockIdx.y; m < M; m += gridDim.y) {
+    float* dst = D + (long long)m * ldd + n;
+    float4 acc = accumulate ? make_float4(dst[0], dst[1], dst[2], dst[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int s = 0; s < S; ++s) {
+      const float4 v = *reinterpret_cast<const float4*>(ws + ((long long)s * M + m) * N + n);
+      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+    dst[0] = acc.x; dst[1] = acc.y; dst[2] = acc.z; dst[3] = acc.w;
+  }
+}
+
+static int gemm_launch(int a_mn_major, int b_mn_major, int epilogue, int act, bool cta2, const CUtensorMap& tA,
+                       const CUtensorMap& tB, const GemmArgs& g, cudaStream_t stream);
 
 static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const void* B, long long ldb, int b_mn_major,
                          void* D0, long long ldd0, void* D1, long long ldd1, int M, int N, int K, int epilogue, int act,
@@ -684,20 +524,14 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
   if ((epilogue == EPI_CE_STATS || epilogue == EPI_CE_GRAD) && (!ce || a_mn_major || b_mn_major)) return MMB_ERR_ARG;
   if ((lda & 7) || (ldb & 7)) return MMB_ERR_ARG;
   if (epilogue != EPI_CE_STATS && (epilogue == EPI_F32 ? (N & 3) : (N & 7))) return MMB_ERR_ARG;   // CE_STATS writes no tensor
-  // CTA-pair mode (cta_group::2, 256x256 tiles) for everything large enough to fill the 74 SM pairs at least once;
-  // MMB_GEMM_CTA2=0 forces the 1-CTA kernel (A/B testing), =1 forces pairs.
-  static int cta2_env0 = -2;
-  if (cta2_env0 == -2) {
-    const char* e = getenv("MMB_GEMM_CTA2");
-    cta2_env0 = e ? atoi(e) : -1;
-  }
-  const int cta2_env = g_force_cta2 >= 0 ? g_force_cta2 : cta2_env0;   // mmb_gemm_set_mode() wins over the env var
-  const long long big_tiles = (long long)((M + 255) / 256) * ((N + BLOCK_N - 1) / BLOCK_N);
-  const bool cta2 = cta2_env == 1 || (cta2_env == -1 && M >= 512 && big_tiles * (splits < 1 ? 1 : splits) >= 37);
+  // 2-CTA clusters (256x128 tiles, B multicast) for everything large enough to fill the SM pairs at least once
+  const long long big_tiles = (long long)((M + 2 * BLOCK_M - 1) / (2 * BLOCK_M)) * ((N + BLOCK_N - 1) / BLOCK_N);
+  const bool cta2 = g_force_cta2 == 1 ||
+                    (g_force_cta2 == -1 && M >= 512 && big_tiles * (splits < 1 ? 1 : splits) >= num_sms() / 2);
   GemmArgs g{};
   if (ce) g = *ce;   // cross-entropy epilogue parameters (the geometry fields below are overwritten)
   g.M = M; g.N = N; g.K = K;
-  g.m_tiles = cta2 ? (M + 255) / 256 : (M + BLOCK_M - 1) / BLOCK_M;
+  g.m_tiles = cta2 ? (M + 2 * BLOCK_M - 1) / (2 * BLOCK_M) : (M + BLOCK_M - 1) / BLOCK_M;
   g.n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
   g.kb_total = (K + BLOCK_K - 1) / BLOCK_K;
   if (splits < 1) splits = 1;
@@ -710,75 +544,61 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
   g.aux = reinterpret_cast<const __nv_bfloat16*>(aux);
   g.ld_aux = ld_aux;
   g.d0 = D0; g.d1 = D1; g.ldd0 = ldd0; g.ldd1 = ldd1;
-  g.reduce_add = (accumulate || g.splits > 1) ? 1 : 0;
-  if (colsum && (epilogue == EPI_F32 || epilogue == EPI_BF16_ACT || (reinterpret_cast<uintptr_t>(colsum) & 15)))
-    return MMB_ERR_ARG;
-  g.colsum = colsum;
+  g.accumulate = accumulate ? 1 : 0;
+  if (colsum && (epilogue == EPI_F32 || epilogue == EPI_BF16_ACT)) return MMB_ERR_ARG;
+  const int col_blocks = (M + BLOCK_M - 1) / BLOCK_M;
+  if (colsum) {
+    g.colsum_part = static_cast<float*>(scratch(SCR_GEMM_COLSUM, (size_t)col_blocks * N * sizeof(float), stream));
+    if (!g.colsum_part) return (int)cudaErrorMemoryAllocation;
+  }
+  if (epilogue == EPI_F32 && g.splits > 1) {
+    g.splitk_ws = static_cast<float*>(scratch(SCR_GEMM_SPLITK, (size_t)g.splits * M * N * sizeof(float), stream));
+    if (!g.splitk_ws) return (int)cudaErrorMemoryAllocation;
+  }
 
-  CUtensorMap tA, tB, tD0, tD1;
+  CUtensorMap tA, tB;
   int rc;
   // A: K-major -> global [M rows][K inner]; MN-major -> global [K rows][M inner]
   if (!a_mn_major) rc = make_tmap_2d(&tA, A, 2, false, K, M, lda * 2, 64, BLOCK_M);
   else             rc = make_tmap_2d(&tA, A, 2, false, M, K, lda * 2, 64, BLOCK_K);
   if (rc) return rc;
-  if (!b_mn_major) rc = make_tmap_2d(&tB, B, 2, false, K, N, ldb * 2, 64, cta2 ? 128 : BLOCK_N);
+  // B: a cluster CTA loads (and multicasts) half of the 128-row tile
+  if (!b_mn_major) rc = make_tmap_2d(&tB, B, 2, false, K, N, ldb * 2, 64, cta2 ? BLOCK_N / 2 : BLOCK_N);
   else             rc = make_tmap_2d(&tB, B, 2, false, N, K, ldb * 2, 64, BLOCK_K);
   if (rc) return rc;
-  if (epilogue == EPI_CE_STATS) {
-    tD0 = tA; tD1 = tA;   // no tensor output: 16 B of statistics per (row, 128-column part)
-  } else if (epilogue == EPI_F32) {
+  if (epilogue == EPI_F32) {
     if (ldd0 & 3) return MMB_ERR_ARG;
-    rc = make_tmap_2d(&tD0, D0, 4, true, N, M, ldd0 * 4, 32, 128);
-    if (rc) return rc;
-    tD1 = tD0;
-    if (g.splits > 1 && !accumulate) {
-      cudaError_t e = cudaMemset2DAsync(D0, ldd0 * 4, 0, (size_t)N * 4, M, stream);
-      if (e != cudaSuccess) return (int)e;
-    }
-  } else {
+  } else if (epilogue != EPI_CE_STATS) {
     if ((ldd0 & 7) || (reinterpret_cast<uintptr_t>(D0) & 15)) return MMB_ERR_ARG;
     if (epilogue == EPI_BF16_ACT && (!D1 || (ldd1 & 7) || (reinterpret_cast<uintptr_t>(D1) & 15))) return MMB_ERR_ARG;
     if (epilogue == EPI_BF16_DACT && (!aux || (ld_aux & 7) || (reinterpret_cast<uintptr_t>(aux) & 15))) return MMB_ERR_ARG;
-    // bf16 outputs leave through TMA stores of 128-row x 64-column (128 B) swizzled slabs; the tensor map clips M / N
-    rc = make_tmap_2d(&tD0, D0, 2, false, N, M, ldd0 * 2, 64, 128);
-    if (rc) return rc;
-    tD1 = tD0;
-    if (epilogue == EPI_BF16_ACT) {
-      rc = make_tmap_2d(&tD1, D1, 2, false, N, M, ldd1 * 2, 64, 128);
-      if (rc) return rc;
-    }
-    if (epilogue == EPI_BF16_DACT) {  // act' operand, TMA-prefetched in 128-row x 64-column slabs
-      rc = make_tmap_2d(&tD1, aux, 2, false, N, M, ld_aux * 2, 64, 128);
-      if (rc) return rc;
-    }
   }
 
+  int rc_launch = gemm_launch(a_mn_major, b_mn_major, epilogue, act, cta2, tA, tB, g, stream);
+  if (rc_launch) return rc_launch;
+  if (g.splitk_ws) {
+    splitk_reduce_kernel<<<dim3((N / 4 + 127) / 128, M < 65535 ? M : 65535), 128, 0, stream>>>(g.splitk_ws, g.splits, M, N,
+                                                                         reinterpret_cast<float*>(D0), ldd0, g.accumulate);
+    rc_launch = (int)cudaGetLastError();
+    if (rc_launch) return rc_launch;
+  }
+  if (colsum) return reduce_partials(g.colsum_part, col_blocks, N, N, colsum, 1, stream);
+  return MMB_OK;
+}
+
+static int gemm_launch(int a_mn_major, int b_mn_major, int epilogue, int act, bool cta2, const CUtensorMap& tA,
+                       const CUtensorMap& tB, const GemmArgs& g, cudaStream_t stream) {
   const int am = a_mn_major ? 1 : 0, bm = b_mn_major ? 1 : 0;
-  // activation epilogues: 8 epilogue warps; MMB_GEMM_EW=16 selects the experimental 16-warp variant (FC2-dgrad x act'
-  // 871 -> 996 TFLOP/s in isolation, FC1+act unchanged; not yet validated inside the full training step)
-  static int ew_env0 = -1;
-  if (ew_env0 < 0) {
-    const char* e = getenv("MMB_GEMM_EW");
-    ew_env0 = (e && e[0] == '1' && e[1] == '6') ? 16 : 8;
-  }
-  const int ew_env = g_force_ew > 0 ? g_force_ew : ew_env0;
-  const bool act_epi = epilogue == EPI_BF16_ACT || epilogue == EPI_BF16_DACT;
-  if (epilogue == EPI_CE_STATS || epilogue == EPI_CE_GRAD) {
-    if (epilogue == EPI_CE_STATS)
-      return cta2 ? launch_impl<false, false, EPI_CE_STATS, 0, true, 8>(tA, tB, tD0, tD1, g, stream)
-                  : launch_impl<false, false, EPI_CE_STATS, 0, false, 8>(tA, tB, tD0, tD1, g, stream);
-    return cta2 ? launch_impl<false, false, EPI_CE_GRAD, 0, true, 8>(tA, tB, tD0, tD1, g, stream)
-                : launch_impl<false, false, EPI_CE_GRAD, 0, false, 8>(tA, tB, tD0, tD1, g, stream);
-  }
-#define MMB_CASE(AM, BM, E, AC)                                                                                     \
-  if (am == AM && bm == BM && epilogue == E && (AC < 0 || act == AC)) {                                             \
-    constexpr int EWX = (E == EPI_BF16_ACT || E == EPI_BF16_DACT) ? 16 : 8;                                         \
-    if (act_epi && ew_env == 16)                                                                                    \
-      return cta2 ? launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), true, EWX>(tA, tB, tD0, tD1, g, stream)  \
-                  : launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), false, EWX>(tA, tB, tD0, tD1, g, stream); \
-    return cta2 ? launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), true, 8>(tA, tB, tD0, tD1, g, stream)      \
-                : launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), false, 8>(tA, tB, tD0, tD1, g, stream);     \
-  }
+  if (epilogue == EPI_CE_STATS)
+    return cta2 ? launch_impl<false, false, EPI_CE_STATS, 0, true>(tA, tB, g, stream)
+                : launch_impl<false, false, EPI_CE_STATS, 0, false>(tA, tB, g, stream);
+  if (epilogue == EPI_CE_GRAD)
+    return cta2 ? launch_impl<false, false, EPI_CE_GRAD, 0, true>(tA, tB, g, stream)
+                : launch_impl<false, false, EPI_CE_GRAD, 0, false>(tA, tB, g, stream);
+#define MMB_CASE(AM, BM, E, AC)                                                                                   \
+  if (am == AM && bm == BM && epilogue == E && (AC < 0 || act == AC))                                             \
+    return cta2 ? launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), true>(tA, tB, g, stream)                \
+                : launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), false>(tA, tB, g, stream);
   MMB_CASE(0, 0, EPI_BF16, -1)
   MMB_CASE(0, 0, EPI_BF16_ACT, ACT_QUICK_GELU)
   MMB_CASE(0, 0, EPI_BF16_ACT, ACT_GELU_ERF)
@@ -792,7 +612,6 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
 #undef MMB_CASE
   return MMB_ERR_UNSUPPORTED;
 }
-
 extern "C" int mmb_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb,
                              int b_mn_major, void* D0, long long ldd0, void* D1, long long ldd1, int M, int N, int K,
                              int epilogue, int act, float alpha, const float* bias, const void* aux,
@@ -803,8 +622,8 @@ extern "C" int mmb_gemm_bf16(const void* A, long long lda, int a_mn_major, const
 }
 
 // ---- fused similarity GEMM + temperature-scaled cross-entropy (no logits in HBM) ------------------------------------
-// Number of float4 partials per row one mmb_gemm_ce_stats launch over N columns writes (two 128-column parts per tile).
-extern "C" int mmb_gemm_ce_num_parts(int N) { return N <= 0 ? 0 : 2 * ((N + BLOCK_N - 1) / BLOCK_N); }
+// Number of float4 partials per row one mmb_gemm_ce_stats launch over N columns writes (one per 128-column tile).
+extern "C" int mmb_gemm_ce_num_parts(int N) { return N <= 0 ? 0 : (N + BLOCK_N - 1) / BLOCK_N; }
 
 static int gemm_ce_stats_impl(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K,
                               const float* log_scale, int label0, const int* labels, void* part, int part_ld, int part0,

@@ -30,11 +30,12 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
 }
 
 // Pass 1 (per local row i): logits = T * sims; row LSE; loss_i (with label smoothing); optional logits output;
-// d loss / d logit_scale accumulated (atomic).  label(i) = label_offset + i.
+// row i's share of d loss / d logit_scale written to dscale_part[i] (summed in row order by the host wrapper).
+// label(i) = label_offset + i.
 __global__ void contrastive_ce_stats_kernel(const float* __restrict__ sims, long long ld,
                                             const float* __restrict__ logit_scale, int rows, int N, int label_offset,
                                             float smoothing, float loss_weight, float* __restrict__ row_loss,
-                                            float* __restrict__ lse_out, float* __restrict__ dscale_accum,
+                                            float* __restrict__ lse_out, float* __restrict__ dscale_part,
                                             float* __restrict__ logits_out, long long ld_l,
                                             const float* __restrict__ row_w) {
   __shared__ float red[32];
@@ -65,7 +66,7 @@ __global__ void contrastive_ce_stats_kernel(const float* __restrict__ sims, long
     if (row_loss) row_loss[i] = row_w ? loss * wrow * rows : loss;  // so that sum(row_loss) / rows is the masked mean
     if (lse_out) lse_out[i] = lse;
   }
-  if (dscale_accum) {
+  if (dscale_part) {
     // d loss_i / d logit_scale = sum_j (p_ij - (1-eps) y_ij - eps/N) * logit_ij   (d logit / d logit_scale = logit)
     float acc = 0.f;
     for (int j = threadIdx.x; j < N; j += blockDim.x) {
@@ -75,7 +76,7 @@ __global__ void contrastive_ce_stats_kernel(const float* __restrict__ sims, long
       acc += gl * l;
     }
     acc = block_reduce_sum(acc, red);
-    if (threadIdx.x == 0) atomicAdd(dscale_accum, acc * loss_weight * wrow);
+    if (threadIdx.x == 0) dscale_part[i] = acc * loss_weight * wrow;
   }
 }
 
@@ -121,7 +122,7 @@ __global__ void contrastive_ce_grad_kernel(const float* __restrict__ sims, long 
 __global__ void ce_stats_reduce_kernel(const float4* __restrict__ part, int part_ld, int n_parts,
                                        const float* __restrict__ xlabel, int rows, int n_total, float smoothing,
                                        float loss_weight, const float* __restrict__ row_w, float* __restrict__ row_loss,
-                                       float* __restrict__ lse_out, float* __restrict__ dscale_accum) {
+                                       float* __restrict__ lse_out, float* __restrict__ dscale_part) {
   const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (i >= rows) return;
@@ -156,8 +157,8 @@ __global__ void ce_stats_reduce_kernel(const float4* __restrict__ part, int part
     const float wrow = row_w ? row_w[i] : 1.f / rows;
     if (row_loss) row_loss[i] = row_w ? loss * wrow * rows : loss;
     if (lse_out) lse_out[i] = lse;
-    if (dscale_accum)
-      atomicAdd(dscale_accum, (sex / se - (1.f - smoothing) * l_label - smoothing * mean_logit) * loss_weight * wrow);
+    if (dscale_part)
+      dscale_part[i] = (sex / se - (1.f - smoothing) * l_label - smoothing * mean_logit) * loss_weight * wrow;
   }
 }
 
@@ -165,12 +166,15 @@ __global__ void ce_stats_reduce_kernel(const float4* __restrict__ part, int part
 // models/coca/coca_model.py:447-452): accum[0] += sum over kept rows of (lse - x_label), accum[1] += number of kept rows.
 __global__ void ce_labels_reduce_kernel(const float4* __restrict__ part, int part_ld, int n_parts,
                                         const float* __restrict__ xlabel, const int* __restrict__ labels, int ignore_index,
-                                        int rows, float* __restrict__ row_loss, float* __restrict__ accum) {
+                                        int rows, float* __restrict__ row_loss, float* __restrict__ part2) {
   const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (i >= rows) return;
   if (labels[i] == ignore_index) {
-    if (lane == 0 && row_loss) row_loss[i] = 0.f;
+    if (lane == 0) {
+      if (row_loss) row_loss[i] = 0.f;
+      part2[2 * i] = 0.f; part2[2 * i + 1] = 0.f;
+    }
     return;
   }
   const float4* pr = part + (long long)i * part_ld;
@@ -191,8 +195,7 @@ __global__ void ce_labels_reduce_kernel(const float4* __restrict__ part, int par
   if (lane == 0) {
     const float loss = mx + logf(se) - xlabel[i];
     if (row_loss) row_loss[i] = loss;
-    atomicAdd(accum, loss);
-    atomicAdd(accum + 1, 1.f);
+    part2[2 * i] = loss; part2[2 * i + 1] = 1.f;
   }
 }
 
@@ -248,10 +251,14 @@ extern "C" int mmb_contrastive_ce_stats(const float* sims, long long ld, const f
                                         float* lse_out, float* dscale_accum, float* logits_out, long long ld_l,
                                         const float* row_w, void* stream) {
   if (rows <= 0 || N <= 0 || label_offset < 0 || label_offset + rows > N) return MMB_ERR_ARG;
-  contrastive_ce_stats_kernel<<<rows, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      sims, ld, logit_scale, rows, N, label_offset, label_smoothing, loss_weight, row_loss, lse_out, dscale_accum,
-      logits_out, ld_l, row_w);
-  return (int)cudaGetLastError();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* dpart = nullptr;
+  if (dscale_accum && !(dpart = static_cast<float*>(scratch(SCR_LOSS, (size_t)rows * sizeof(float), st))))
+    return (int)cudaErrorMemoryAllocation;
+  contrastive_ce_stats_kernel<<<rows, 256, 0, st>>>(sims, ld, logit_scale, rows, N, label_offset, label_smoothing,
+                                                    loss_weight, row_loss, lse_out, dpart, logits_out, ld_l, row_w);
+  const int rc = (int)cudaGetLastError();
+  return (rc || !dscale_accum) ? rc : reduce_partials(dpart, rows, 1, 1, dscale_accum, 1, st);
 }
 
 extern "C" int mmb_contrastive_ce_grad(const float* sims, long long ld, const float* logit_scale, int rows, int N,
@@ -284,16 +291,25 @@ extern "C" int mmb_ce_stats_reduce(const void* part, int part_ld, int n_parts, c
                                    float label_smoothing, float loss_weight, const float* row_w, float* row_loss,
                                    float* lse_out, float* dscale_accum, void* stream) {
   if (!part || !xlabel || rows <= 0 || n_parts <= 0 || n_parts > part_ld || n_total <= 0) return MMB_ERR_ARG;
-  ce_stats_reduce_kernel<<<(rows + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const float4*>(part), part_ld, n_parts, xlabel, rows, n_total, label_smoothing, loss_weight, row_w,
-      row_loss, lse_out, dscale_accum);
-  return (int)cudaGetLastError();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* dpart = nullptr;
+  if (dscale_accum && !(dpart = static_cast<float*>(scratch(SCR_LOSS, (size_t)rows * sizeof(float), st))))
+    return (int)cudaErrorMemoryAllocation;
+  ce_stats_reduce_kernel<<<(rows + 7) / 8, 256, 0, st>>>(reinterpret_cast<const float4*>(part), part_ld, n_parts, xlabel,
+                                                         rows, n_total, label_smoothing, loss_weight, row_w, row_loss,
+                                                         lse_out, dpart);
+  const int rc = (int)cudaGetLastError();
+  return (rc || !dscale_accum) ? rc : reduce_partials(dpart, rows, 1, 1, dscale_accum, 1, st);
 }
 
 extern "C" int mmb_ce_labels_reduce(const void* part, int part_ld, int n_parts, const float* xlabel, const int* labels,
                                     int ignore_index, int rows, float* row_loss, float* accum, void* stream) {
   if (!part || !xlabel || !labels || !accum || rows <= 0 || n_parts <= 0 || n_parts > part_ld) return MMB_ERR_ARG;
-  ce_labels_reduce_kernel<<<(rows + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const float4*>(part), part_ld, n_parts, xlabel, labels, ignore_index, rows, row_loss, accum);
-  return (int)cudaGetLastError();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* part2 = static_cast<float*>(scratch(SCR_LOSS, 2ull * rows * sizeof(float), st));
+  if (!part2) return (int)cudaErrorMemoryAllocation;
+  ce_labels_reduce_kernel<<<(rows + 7) / 8, 256, 0, st>>>(reinterpret_cast<const float4*>(part), part_ld, n_parts, xlabel,
+                                                          labels, ignore_index, rows, row_loss, part2);
+  const int rc = (int)cudaGetLastError();
+  return rc ? rc : reduce_partials(part2, rows, 2, 2, accum, 1, st);
 }

@@ -27,3 +27,15 @@ int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_
                       uint64_t pitch2, uint32_t box_inner, uint32_t box1);
 int num_sms();
 }  // namespace mmb
+
+// Deterministic reductions: no floating-point atomics anywhere, so a run's results do not depend on the order in which
+// CTAs happen to finish.  Kernels write per-CTA (or per-row-slice) partials into scratch and a fixed-order reduction
+// adds them into the output.
+namespace mmb {
+// Device scratch of at least `bytes`, private to (device, stream, slot); grows on demand (cudaFree synchronises, so a
+// buffer an earlier launch still uses is never freed under it).  nullptr if the allocation fails.
+void* scratch(int slot, size_t bytes, cudaStream_t stream);
+enum ScratchSlot { SCR_GEMM_SPLITK = 0, SCR_GEMM_COLSUM, SCR_LN_BWD, SCR_COLSUM, SCR_BATCH_SUM, SCR_LOSS, SCR_COUNT };
+// out[n] (+)= sum_{p = 0..P-1} part[p * ldp + n] for n < N, summed in increasing p (accumulate = 0: out is overwritten).
+int reduce_partials(const float* part, int P, int N, long long ldp, float* out, int accumulate, cudaStream_t stream);
+}  // namespace mmb

@@ -1,5 +1,5 @@
 """Host-side runtime of the dual-encoder path: parameter shadows, activation workspaces and the explicit
-forward / backward schedules that drive the sm_100a kernels (multimodal_b200.ops).
+forward / backward schedules that drive the sm_90a kernels (multimodal_b200.ops).
 
 Nothing here computes: every tensor op is a C-ABI kernel launch on the current CUDA stream.  The schedules follow
 the reference call stack (SURVEY.md §3.1):

@@ -7,7 +7,7 @@ One generic pre-norm layer runner serves the TorchMultimodal `TransformerEncoder
     LN -> packed QKV GEMM -> attention -> out-proj GEMM -> (+residual, LN fused) -> [cross-attention] -> MLP (GELU fused
     into the first GEMM's epilogue) -> (+residual fused into the next LayerNorm kernel)
 
-Attention routing: unmasked / causal self-attention with head_dim 64 runs on the tcgen05 kernel (attention_tc.cu);
+Attention routing: unmasked / causal self-attention with head_dim 64 runs on the tensor-core attention kernel (attention.cu);
 anything else — cross-attention, the pooler's head_dim 96, the text decoder's [causal x padding] mask — on the general
 kernel (attention_generic.cu).  Reference call stacks: models/coca/coca_model.py:69-130, models/coca/text_decoder.py
 :141-203, models/coca/multimodal_decoder.py:86-108, modules/layers/attention_pooler.py:48-101,

@@ -4,12 +4,12 @@ forwards that keep what the backward needs + explicit backward schedules, behind
 398-454 under autograd).
 
 All layer stacks run on ``engine.TransformerStack`` (the CLIP towers' fused schedule and kernels):
-  vision encoder      : packed `input_proj` self-attention (tcgen05 fwd / bwd), erf-GELU MLP, optional final LayerNorm
+  vision encoder      : packed `input_proj` self-attention (tensor-core fwd / bwd), erf-GELU MLP, optional final LayerNorm
                         (modules/encoders/vision_transformer.py:56-89, patch_embedding.py:104-154)
   text decoder        : separate q / k / v projections presented as one packed operand, the [B, S, S] causal x padding
                         mask on the general attention kernels (fwd: mma.sync, bwd: SIMT), CLS row -> ln_final -> projection
                         (models/coca/text_decoder.py:141-203)
-  multimodal decoder  : causal self-attention (tcgen05) + cross-attention to the pooled image tokens (general kernels) +
+  multimodal decoder  : causal self-attention (tensor cores) + cross-attention to the pooled image tokens (general kernels) +
                         MLP per layer, final LayerNorm (models/coca/multimodal_decoder.py:86-108)
   attention pooler    : LayerNorm-ed keys / values, batch-shared learned queries (their gradient is summed over the batch
                         with fp32 atomics), ln_post (modules/layers/attention_pooler.py:48-72)

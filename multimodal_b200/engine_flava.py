@@ -254,7 +254,7 @@ class FlavaMMRuntime:
     def forward_projected(self, image_hidden: torch.Tensor, text_hidden: torch.Tensor, image_proj: nn.Linear,
                           text_proj: nn.Linear, want_attn: bool = False) -> TransformerOutput:
         """FLAVAModel.encode_mm (models/flava/model.py:283-298): project both token streams to the multimodal width
-        (two tcgen05 GEMMs, fp32 out + bias), then [cls | image | text] assembled by one kernel straight into X0."""
+        (two wgmma GEMMs, fp32 out + bias), then [cls | image | text] assembled by one kernel straight into X0."""
         st = self.stack
         ws, sh, d = st.ws, st.sh, st.d
         B, Si, di = image_hidden.shape

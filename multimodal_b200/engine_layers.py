@@ -6,8 +6,8 @@ exposes — and tests — on their own are callable outside an encoder:
   modules/layers/patch_embedding.py:25-157       PatchEmbeddings
   modules/layers/mlp.py:13-66                    MLP ([Linear, activation, Linear] form)
 
-They launch exactly the kernels the fused encoder schedules launch (tcgen05 GEMMs with bias / activation epilogues,
-tcgen05 attention, the add+LayerNorm kernel); nothing is computed by PyTorch.  Pre-norm `TransformerEncoderLayer` /
+They launch exactly the kernels the fused encoder schedules launch (wgmma GEMMs with bias / activation epilogues,
+tensor-core attention, the add+LayerNorm kernel); nothing is computed by PyTorch.  Pre-norm `TransformerEncoderLayer` /
 `TransformerEncoder` also train on their own (grad mode on: `engine_coca_train.LayersTrainRuntime`, the CLIP towers' fused
 forward / backward schedule); the other standalone modules compute forward values only, and asking them for an autograd
 graph raises instead of returning detached tensors.
@@ -230,7 +230,7 @@ def encoder_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask:
 
 def patch_embeddings_forward(mod: nn.Module, image: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None):
     """PatchEmbeddings.forward (patch_embedding.py:104-154) without random patch dropping: conv projection as
-    im2col + tcgen05 GEMM, [cls |] patches (mask-token substitution) + position embeddings in one assembly kernel."""
+    im2col + wgmma GEMM, [cls |] patches (mask-token substitution) + position embeddings in one assembly kernel."""
     from .modules.layers.patch_embedding import PatchEmbeddingsOutput
 
     forward_only_guard(mod, "PatchEmbeddings")

@@ -2,7 +2,7 @@
 
 Restates modules/losses/contrastive_loss_with_temperature.py:26-115 + utils/distributed.py:28-58:
 
-  sims_a = A_loc @ B_all^T, sims_b = B_loc @ A_all^T            (tcgen05 GEMMs, fp32 out; alpha applied in the CE kernel)
+  sims_a = A_loc @ B_all^T, sims_b = B_loc @ A_all^T            (wgmma GEMMs, fp32 out; alpha applied in the CE kernel)
   logits = exp(logit_scale) * sims ; CE against labels rank*B + i (+ label smoothing) ; loss = (loss_a + loss_b) / 2
   gradients w.r.t. A_loc, B_loc, logit_scale are produced in the same pass (dsims from the CE kernel, two GEMMs each).
 

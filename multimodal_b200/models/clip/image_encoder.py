@@ -3,7 +3,7 @@
 Same constructor signature, same state-dict keys/shapes, same initialisation (the parameter containers are created
 in the reference's order, so ``torch.manual_seed(s); CLIPViTEncoder(...)`` yields bit-identical weights), same
 ``ValueError``s.  The forward is NOT torch's layer stack: it is ``engine.ViTTower`` — im2col+GEMM patch embedding,
-fused LayerNorm / QKV / attention / MLP kernels on tcgen05 tensor cores (see DESIGN.md).
+fused LayerNorm / QKV / attention / MLP kernels on Hopper tensor cores (see DESIGN.md).
 """
 import torch
 from torch import nn, Tensor

@@ -1,5 +1,5 @@
 """CoCa multimodal decoder — drop-in for torchmultimodal/models/coca/multimodal_decoder.py:15-108.  Forward =
-`engine_coca.MultimodalDecoderRuntime`: causal self-attention on the tcgen05 kernel, cross-attention to the captioning
+`engine_coca.MultimodalDecoderRuntime`: causal self-attention on the tensor-core attention kernel, cross-attention to the captioning
 image tokens on the general kernel, final LayerNorm + vocabulary projection GEMM (fp32 logits)."""
 from typing import Callable, Optional
 

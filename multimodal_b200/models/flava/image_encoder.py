@@ -1,6 +1,6 @@
 """FLAVA image encoder — drop-in for torchmultimodal/models/flava/image_encoder.py:28-278 (`PatchEmbeddings`,
 `ImageEmbeddings`, `ImageTransformer`, `flava_image_encoder`).  Same constructors / state-dict keys / init; the forward
-is `engine_flava.FlavaImageRuntime` (im2col + tcgen05 GEMM patch embedding, fused token assembly, fused layer stack).
+is `engine_flava.FlavaImageRuntime` (im2col + wgmma GEMM patch embedding, fused token assembly, fused layer stack).
 Position-embedding interpolation (image_encoder.py:103-137) is out of scope (fixed 224x224 pre-training resolution)."""
 import warnings
 from functools import partial

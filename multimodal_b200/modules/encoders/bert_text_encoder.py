@@ -1,6 +1,6 @@
 """`BERTTextEncoder` — drop-in for torchmultimodal/modules/encoders/bert_text_encoder.py:17-176.  Same constructor,
 state-dict keys and argument meaning; the forward is `engine_flava.FlavaTextRuntime` (fused embedding-sum + LayerNorm,
-pad-derived key mask consumed by the tcgen05 attention kernel, fused layer stack, layernorm, pooler).
+pad-derived key mask consumed by the tensor-core attention kernel, fused layer stack, layernorm, pooler).
 
 On the accelerated path: `input_ids` (required), `attention_mask` of shape [batch, seq_len], `token_type_ids`.
 `position_ids` / `inputs_embeds` raise NotImplementedError; `return_attn_weights=True` returns the

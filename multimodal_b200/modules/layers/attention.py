@@ -1,6 +1,6 @@
 """Parameter containers mirroring torchmultimodal/modules/layers/attention.py:15-182 (`SelfAttention`,
 `MultiHeadAttention` with separate query/key/value/output Linears).  The FLAVA runtimes pack q/k/v into one [3d, d]
-operand and run the fused QKV GEMM + tcgen05 attention; attention probabilities are never materialised."""
+operand and run the fused QKV GEMM + tensor-core attention; attention probabilities are never materialised."""
 from typing import Any
 
 from torch import nn, Tensor

@@ -1,5 +1,5 @@
 """Parameter container mirroring torchmultimodal/modules/layers/mlp.py:13-66 (state-dict keys ``model.{i}.*``).
-Inside the FLAVA encoders the MLP runs as two tcgen05 GEMMs with the GELU fused into the first epilogue."""
+Inside the FLAVA encoders the MLP runs as two wgmma GEMMs with the GELU fused into the first epilogue."""
 from typing import Callable, List, Optional, Union
 
 import torch

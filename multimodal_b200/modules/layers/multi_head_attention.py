@@ -1,7 +1,7 @@
 """Parameter containers mirroring torchmultimodal/modules/layers/multi_head_attention.py:19-180
 (`MultiHeadSelfAttention` with the fused ``input_proj [3d, d]``; `MultiHeadAttentionWithCache` with separate
 ``q_proj / k_proj / v_proj / output_proj``).  They execute inside the owning encoder / decoder / pooler runtime
-(engine_coca.py): packed-QKV tcgen05 GEMM + attention kernel; F.scaled_dot_product_attention is never called."""
+(engine_coca.py): packed-QKV wgmma GEMM + attention kernel; F.scaled_dot_product_attention is never called."""
 from typing import Any, Optional
 
 from torch import nn, Tensor

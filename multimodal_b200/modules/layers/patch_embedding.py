@@ -1,6 +1,6 @@
 """`PatchEmbeddings` — parameter container mirroring torchmultimodal/modules/layers/patch_embedding.py:25-157
 (conv projection with truncated-normal init, optional CLS token, position embeddings, optional mask token).  Executed
-by `engine_coca.VisionRuntime` as im2col + tcgen05 GEMM + one token-assembly kernel.  Random patch dropping
+by `engine_coca.VisionRuntime` as im2col + wgmma GEMM + one token-assembly kernel.  Random patch dropping
 (`patch_drop_rate`, training-time augmentation) is not on the accelerated path."""
 import math
 from typing import Any, NamedTuple, Optional, Tuple, Union
@@ -57,7 +57,7 @@ class PatchEmbeddings(nn.Module):
         nn.init.zeros_(self.conv_projection.bias)
 
     def forward(self, image: Tensor, image_patches_mask: Optional[Tensor] = None) -> PatchEmbeddingsOutput:
-        """Standalone forward (values only): im2col + tcgen05 GEMM + token assembly, as inside VisionTransformer."""
+        """Standalone forward (values only): im2col + wgmma GEMM + token assembly, as inside VisionTransformer."""
         from ...engine_layers import patch_embeddings_forward
 
         return patch_embeddings_forward(self, image, image_patches_mask)

@@ -3,7 +3,7 @@ torchmultimodal/modules/losses/contrastive_loss_with_temperature.py:17-201.
 
 Same public surface (``ContrastiveLossOutput``, ``contrastive_loss_with_temperature``,
 ``ContrastiveLossWithTemperature``, ``DEFAULT_LOGIT_SCALE``), same ``ValueError`` / clamp quirks (:172-175, :193).
-The computation is ``engine_loss.ContrastiveRuntime``: similarity GEMMs on tcgen05 tensor cores, temperature scaling +
+The computation is ``engine_loss.ContrastiveRuntime``: similarity GEMMs on Hopper tensor cores, temperature scaling +
 cross-entropy + all gradients in one kernel pass; with torch.distributed initialised the peers' embeddings are pulled
 over NVLink inside the runtime (no NCCL all_gather on this path).
 """

@@ -1,6 +1,6 @@
 """Drop-in for torchmultimodal.modules.optimizers.anyprecision.AnyPrecisionAdamW (anyprecision.py:16-199): same
 constructor, same per-parameter state keys (`step`, `exp_avg`, `exp_avg_sq`, `compensation`) and dtypes, same update
-rule.  The step of every parameter is ONE fused sm_100a kernel (mmb_anyprecision_adamw_step) instead of the
+rule.  The step of every parameter is ONE fused sm_90a kernel (mmb_anyprecision_adamw_step) instead of the
 reference's ~12 elementwise passes; roundings to the state dtypes are reproduced one for one.
 
 Parameters and gradients must be fp32 CUDA tensors (this runtime keeps fp32 master weights; bf16 operand copies are
@@ -47,9 +47,9 @@ class AnyPrecisionAdamW(Optimizer):
                 if p.grad.is_sparse:
                     raise RuntimeError("AnyPrecisionAdamW does not support sparse gradients")
                 if not p.is_cuda or p.dtype != torch.float32 or p.grad.dtype != torch.float32:
-                    raise MMBError("AnyPrecisionAdamW (B200): parameters and gradients must be fp32 CUDA tensors")
+                    raise MMBError("AnyPrecisionAdamW: parameters and gradients must be fp32 CUDA tensors")
                 if not p.is_contiguous() or not p.grad.is_contiguous():
-                    raise MMBError("AnyPrecisionAdamW (B200): parameters and gradients must be contiguous")
+                    raise MMBError("AnyPrecisionAdamW: parameters and gradients must be contiguous")
                 state = self.state[p]
                 if len(state) == 0:
                     state["step"] = torch.tensor(0.0)

@@ -1,7 +1,7 @@
 """Typed Python wrappers over the C ABI (include/mmb200.h).
 
 PyTorch is used here for device memory and streams only: every function takes CUDA tensors, checks dtype /
-contiguity / device, and launches hand-written sm_100a kernels on ``torch.cuda.current_stream()``.  A CPU
+contiguity / device, and launches hand-written sm_90a kernels on ``torch.cuda.current_stream()``.  A CPU
 tensor, a missing library or a non-zero status raises — there is no eager / CPU fallback.
 """
 from __future__ import annotations
@@ -105,9 +105,23 @@ def gemm(A, B, *, a_mn=False, b_mn=False, epilogue=EPI_BF16, out=None, out2=None
     return (out, out2) if epilogue == EPI_BF16_ACT else out
 
 
-def wgrad_splits(out_rows: int, out_cols: int, k: int, n_units: int = 74) -> int:
-    """Split-K factor for a weight-gradient GEMM so that the (256 x 256, one per SM pair) tile count fills the machine."""
-    tiles = ((out_rows + 255) // 256) * ((out_cols + 255) // 256)
+_CLUSTERS = {}
+
+
+def _clusters_on_current_device() -> int:
+    dev = torch.cuda.current_device()
+    if dev not in _CLUSTERS:
+        _CLUSTERS[dev] = torch.cuda.get_device_properties(dev).multi_processor_count // 2
+    return _CLUSTERS[dev]
+
+
+def wgrad_splits(out_rows: int, out_cols: int, k: int, n_units: Optional[int] = None) -> int:
+    """Split-K factor for a weight-gradient GEMM so that the (256 x 128, one per 2-CTA cluster) tile count fills the
+    machine.  n_units = 2-CTA clusters the GPU holds at once (default: half the current device's SM count, e.g. 66 on
+    an H100 SXM, 57 on an H100 PCIe)."""
+    if n_units is None:
+        n_units = _clusters_on_current_device()
+    tiles = ((out_rows + 255) // 256) * ((out_cols + 127) // 128)
     kb = (k + 63) // 64
     if tiles >= 2 * n_units:
         return 1

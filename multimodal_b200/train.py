@@ -72,11 +72,10 @@ class ContrastiveTrainer:
         self.smoothing = label_smoothing
         self.backprop_type = backprop_type
         self.grad_chunks = max(1, grad_chunks)
-        # Gradient all-reduce scheduling.  Round 1 overlapped chunked all-reduces with the image tower's backward; on
-        # 8 GPUs that cost more than it hid (190.9 vs 179.9 ms/step): the NCCL CTAs take SMs away from the persistent
-        # one-CTA-per-SM GEMMs, whose displaced CTAs then run as a second wave (GEMM throughput 1175 -> 1113 TFLOP/s),
-        # whereas the whole 600 MB all-reduce is only ~1.5 ms over NVSwitch.  Default now: both flat gradient buffers
-        # are reduced right after the backward, nothing runs beside the GEMMs (MMB_OVERLAP_ALLREDUCE=1: round-1 schedule).
+        # Gradient all-reduce scheduling.  Default: both flat gradient buffers are reduced right after the backward, so
+        # nothing runs beside the GEMMs (NCCL's CTAs would take SMs from the persistent one-CTA-per-SM GEMMs and push
+        # their displaced CTAs into a second wave).  MMB_OVERLAP_ALLREDUCE=1 overlaps chunked all-reduces with the image
+        # tower's backward instead; which is faster on a given multi-GPU box is not measured here.
         if overlap_allreduce is None:
             import os
             overlap_allreduce = os.environ.get("MMB_OVERLAP_ALLREDUCE", "0") == "1"

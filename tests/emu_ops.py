@@ -407,6 +407,15 @@ def argmax_tokens(tokens, idx, B, S):
     idx.copy_(tokens.argmax(-1).to(torch.int32))
 
 
+_real_wgrad_splits = None
+
+
+def wgrad_splits(out_rows, out_cols, k, n_units=None):
+    """No device to ask for its SM count: the split-K factor an H100 SXM (66 2-CTA clusters) would get.  The emulated
+    GEMM's result does not depend on it."""
+    return _real_wgrad_splits(out_rows, out_cols, k, 66 if n_units is None else n_units)
+
+
 NAMES = [n for n, f in list(globals().items()) if callable(f) and not n.startswith("_") and n not in ("install",)]
 
 
@@ -414,6 +423,8 @@ def install(monkeypatch):
     """Swap the kernel wrappers of multimodal_b200.ops for the emulation and lift the CUDA-device guard."""
     from multimodal_b200 import engine, ops
 
+    global _real_wgrad_splits
+    _real_wgrad_splits = ops.wgrad_splits
     for n in NAMES:
         if hasattr(ops, n):
             monkeypatch.setattr(ops, n, globals()[n])

@@ -5,7 +5,7 @@ the same order under the same seed (checked by the param checksum stored in the 
 import torch
 
 CASES = {
-    # S_image = 17, S_text = 12, S_mm = 30: every encoder on the tcgen05 attention path
+    # S_image = 17, S_text = 12, S_mm = 30: every encoder on the tensor-core attention path
     "flava_small": dict(
         kwargs=dict(image_hidden_size=128, image_num_attention_heads=2, image_num_hidden_layers=2,
                     image_intermediate_size=256, image_size=32, patch_size=8,

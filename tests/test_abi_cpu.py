@@ -30,9 +30,9 @@ def test_wgrad_split_heuristic():
     from multimodal_b200.ops import wgrad_splits
 
     for rows, cols, k in [(768, 3072, 201728), (3072, 768, 201728), (2304, 768, 201728), (768, 768, 201728), (512, 2048, 78848)]:
-        s = wgrad_splits(rows, cols, k)
-        tiles = -(-rows // 128) * -(-cols // 256) * s
-        assert tiles >= 100 and s >= 1
+        s = wgrad_splits(rows, cols, k, n_units=66)     # H100 SXM: 132 SMs = 66 clusters
+        tiles = -(-rows // 128) * -(-cols // 128) * s   # 128 x 128 CTA tiles on 132 SMs
+        assert tiles >= 88 and s >= 1
 
 
 def test_host_helpers_wgrad_splits_and_symm_layout():
@@ -43,14 +43,14 @@ def test_host_helpers_wgrad_splits_and_symm_layout():
     from multimodal_b200 import ops
     from multimodal_b200.symm import _Slots
 
-    assert ops.wgrad_splits(768, 768, 201728) >= 2                 # 9 tiles cannot fill 74 pairs without split-K
-    assert ops.wgrad_splits(8192, 8192, 4096) == 1                 # already >= 2 waves of tiles
+    assert ops.wgrad_splits(768, 768, 201728, n_units=66) >= 2                 # 18 tiles cannot fill 66 clusters without split-K
+    assert ops.wgrad_splits(8192, 8192, 4096, n_units=66) == 1                 # already >= 2 waves of tiles
     for rows, cols, k in ((768, 3072, 201728), (2304, 768, 201728), (512, 2048, 78848)):
-        s = ops.wgrad_splits(rows, cols, k)
-        tiles = -(-rows // 256) * -(-cols // 256)
+        s = ops.wgrad_splits(rows, cols, k, n_units=66)
+        tiles = -(-rows // 256) * -(-cols // 128)
         assert 1 <= s <= 64 and ((k + 63) // 64) // s >= 8
-        waves = -(-tiles * s // 74)
-        assert tiles * s / (waves * 74) >= 0.9 or s == 1
+        waves = -(-tiles * s // 66)
+        assert tiles * s / (waves * 66) >= 0.9 or s == 1
     B, E = 128, 256
     raw = torch.zeros(_Slots.size(B, E), dtype=torch.uint8)
     sl = _Slots(raw, B, E)
