@@ -1,18 +1,29 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a: TMA -> smem ring -> wgmma (register accumulators) -> fused epilogue
-// straight from the accumulator registers.
+// -> shared-memory staging -> TMA store.
 //
 // One kernel covers every dense contraction on the dual-encoder path:
 //   forward linears   y = x W^T      A K-major [M,K],  B K-major [N,K]      (torch/nn/functional.py:6478,6690;
 //                                                                            torch/nn/modules/transformer.py:980-982)
 //   dgrad             dx = dy W      A K-major [M,N'], B MN-major [N',K']
-//   wgrad             dW = dy^T x    A MN-major [tokens,N'], B MN-major [tokens,K']   (split-K, fp32 reduce-add)
+//   wgrad             dW = dy^T x    A MN-major [tokens,N'], B MN-major [tokens,K']   (split-K, fp32 partials)
 //   logits            a b^T * T      (modules/losses/contrastive_loss_with_temperature.py:90-95)
 //
-// Tile: BLOCK_M=128 x BLOCK_N=128 x BLOCK_K=64 per CTA, 6-stage smem ring (32 KB/stage).  Warp roles: warpgroup 0 =
-// TMA producer (one elected thread), warpgroups 1 and 2 = consumers, each owning 64 rows of the tile (wgmma m64n128k16,
-// 64 fp32 accumulator registers per thread) and running the epilogue of its rows.  While the consumers run an epilogue
-// the producer is already filling the ring with the next tile's k-blocks.
-// Cluster mode (CLU): two CTAs of a cluster compute a 256 x 128 tile; each loads its own 128 rows of A and HALF of
+// Tile: BLOCK_M=128 x BLOCK_N=256 x BLOCK_K=64 per CTA, 4-stage smem ring (16 KB A + 32 KB B = 48 KB per stage).  Warp
+// roles: warpgroup 0 = TMA producer (one elected thread; setmaxnreg drops it to 40 registers), warpgroups 1 and 2 =
+// consumers (raised to 232 registers), each owning 64 rows of the tile (wgmma m64n256k16, 128 fp32 accumulator
+// registers per thread) and running the epilogue of its rows.  While the consumers run an epilogue the producer is
+// already filling the ring with the next tile's k-blocks.
+// Epilogue: each consumer warpgroup converts its 64 x 256 accumulator chunk by chunk (64 bf16 or 32 fp32 columns =
+// 128-byte rows) into one of its two 8 KB 128B-swizzled staging buffers, and one thread issues a TMA store (or, for an
+// fp32 D += result, a TMA reduce-add) of the chunk.  A buffer is reused as soon as the store has READ it; the global
+// writes drain while the warpgroup goes on.  EPI_BF16_DACT brings its pre-activation chunks into the same buffers by
+// TMA (the first two are issued before the tile's main loop).  An fp32 output that TMA cannot address (base not
+// 16-byte aligned) is written with direct stores instead.
+// Shared memory: 4 x 48 KB ring + 32 KB staging + barriers = 225.3 KB of the 227 KB a block may use.  Four stages keep
+// about 4 us of operands in flight per CTA at the measured rate (DESIGN.md §9); a 3-stage ring would free room for
+// more staging but has not been measured.  ptxas: no spills except a few epilogue words in the DACT and CE_STATS
+// instantiations (tests/test_gemm_sass_cpu.py).
+// Cluster mode (CLU): two CTAs of a cluster compute a 256 x 256 tile; each loads its own 128 rows of A and HALF of
 // the B tile, multicast into both CTAs' shared memory, which halves the L2 -> SM traffic for B.
 #include "common.cuh"
 #include "mmb200_internal.h"
@@ -22,15 +33,17 @@
 namespace mmb {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = 128;
+constexpr int BLOCK_N = 256;
 constexpr int BLOCK_K = 64;
 constexpr int WG_K = 16;
-constexpr int STAGES = 6;
+constexpr int STAGES = 4;
 constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
-constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;   // 16 KB
+constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;   // 32 KB
 constexpr int GEMM_THREADS = 384;
-constexpr int COLSUM_SMEM = 8 * BLOCK_N * 4;    // per-warp column sums of the tile (bf16 epilogues with colsum)
-constexpr int GEMM_SMEM_BYTES = 1024 /*align slack*/ + STAGES * (A_BYTES + B_BYTES) + 256 + COLSUM_SMEM;
+constexpr int STG_BYTES = 64 * 128;             // one staging chunk: 64 rows x 128 B (64 bf16 / 32 fp32 columns)
+constexpr int EPI_SMEM = 4 * STG_BYTES;         // two chunks per consumer warpgroup
+constexpr int GEMM_SMEM_BYTES = 1024 /*align slack*/ + STAGES * (A_BYTES + B_BYTES) + EPI_SMEM + 256 /*barriers*/;
+static_assert(GEMM_SMEM_BYTES <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
 struct GemmArgs {
   int M, N, K;
@@ -43,8 +56,10 @@ struct GemmArgs {
   long long ldd0, ldd1;
   float* colsum_part;         // bf16 epilogues (not ACT), or nullptr: [ceil(M/128)][N] column sums of bf16(D0) per
                               // 128-row block; the host adds them into colsum[n] in block order (bias gradient)
-  float* splitk_ws;           // fp32 epilogue with split-K: [splits][M][N] partial products, reduced in split order
+  float* splitk_ws;           // fp32 epilogue with split-K: [splits][ws_rows][N] partial products, reduced in split order
+  int ws_rows;                // rows per split in splitk_ws (M rounded up to whole tiles)
   int accumulate;             // fp32 epilogue without split-K: D0 += result (one writer per element)
+  int f32_direct;             // fp32 epilogue without split-K whose D0 cannot take TMA stores: direct stores
   // ---- temperature-scaled cross-entropy epilogues (EPI_CE_STATS / EPI_CE_GRAD): logits = exp(*ce_log_scale) * acc
   // are consumed in registers and never written to HBM (contrastive_loss_with_temperature.py:90-107)
   const float* ce_log_scale;  // device scalar (logit_scale parameter)
@@ -59,28 +74,30 @@ struct GemmArgs {
   const float* ce_lse_col;    // CE_GRAD: [N] row-LSE of the other direction's global row j (transposed term) or nullptr
   const float* ce_col_w;      // CE_GRAD: [N] weights of those rows or nullptr
   int ce_col_lo, ce_col_hi;   // CE_GRAD: columns that receive the transposed term
-  float4* ce_part;            // CE_STATS: [M][ce_part_ld] partial (max, sum e^(x-max), sum e^(x-max) x, sum x)
-  int ce_part_ld, ce_part0;   // CE_STATS: row pitch (in float4) and first part index of this launch
+  float4* ce_part;            // CE_STATS: [M][ce_part_ld] partial (max, sum e^(x-max), sum e^(x-max) x, sum x) per 128
+  int ce_part_ld, ce_part0;   // CE_STATS: row pitch (in float4) and first part index of this launch     columns
   float* ce_xlabel;           // CE_STATS: [M] logit at the label column
 };
 
-__device__ __forceinline__ void store_bf16x2(void* base, long long ld, int m, int n, float a, float b) {
-  *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(base) + (long long)m * ld + n) = pack_bf16x2(a, b);
-}
+// named barrier of one consumer warpgroup (ids 2, 3; id 1 spans both consumer warpgroups)
+__device__ __forceinline__ void wg_bar_sync(int cw) { asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory"); }
 
+// tmC0: the output D0 (bf16 epilogues), the split-K workspace or D0 (fp32); tmC1: D1 (EPI_BF16_ACT) or the
+// pre-activation aux (EPI_BF16_DACT).  Both are 128B-swizzled with a 64-row x 128-byte box.
 template <bool A_MN, bool B_MN, int EPI, int ACT, bool CLU>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1, const GemmArgs p) {
   extern __shared__ uint8_t smem_raw[];
   // 1024 B alignment for the 128B-swizzle atoms (identical offset in both CTAs of a cluster: the multicast target)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));   // [STAGES]
+  uint8_t* sStg = smem + STAGES * (A_BYTES + B_BYTES);                                      // [2 wg][2][STG_BYTES]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sStg + EPI_SMEM);                        // [STAGES]
   uint64_t* empty_bar = full_bar + STAGES;                                                  // [STAGES]
-  float* sCol = reinterpret_cast<float*>(smem + STAGES * (A_BYTES + B_BYTES) + 256);        // [8 warps][BLOCK_N]
+  uint64_t* aux_bar = empty_bar + STAGES;                                                   // [2 wg][2]
   constexpr int TILE_M = CLU ? 2 * BLOCK_M : BLOCK_M;
-  const uint32_t rank = CLU ? cluster_ctarank() : 0u;
   const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
@@ -90,17 +107,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], CLU ? 4 : 2);   // one arrive per consumer warpgroup (of both CTAs of a cluster)
     }
+    for (int i = 0; i < 4; ++i) mbar_init(&aux_bar[i], 1);
     fence_mbar_init();
   }
   if (CLU) cluster_sync_all(); else __syncthreads();
 
-  const int tiles_mn = p.m_tiles * p.n_tiles;
-  const int total_tiles = tiles_mn * p.splits;
-  const int tile_first = CLU ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+  // tile schedule, computed in each role after setmaxnreg (a value live across the reallocation gets spilled)
+#define MMB_TILE_SCHEDULE                                                      \
+  const uint32_t rank = CLU ? cluster_ctarank() : 0u;                          \
+  const int tiles_mn = p.m_tiles * p.n_tiles;                                  \
+  const int total_tiles = tiles_mn * p.splits;                                 \
+  const int tile_first = CLU ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;       \
   const int tile_step = CLU ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
   if (wg == 0) {
     // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    MMB_TILE_SCHEDULE
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -124,19 +147,24 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             for (int j = 0; j < BLOCK_M / 64; ++j)
               tma_load_2d(&tmA, &full_bar[stage], a_dst + j * (64 * BLOCK_K * 2), m_row + j * 64, kb * BLOCK_K);
           }
-          // B: K-major -> rows [n0, n0 + 128) of [N][K]; MN-major -> two 64-column boxes of [K][N], 8 KB apart.
-          // Either way one 8 KB half is box / row block `h` at byte offset h * 8192.
+          // B: K-major -> rows [n0, n0 + 256) of [N][K]; MN-major -> four 64-column boxes of [K][N], 8 KB apart.
+          // Either way 64 columns of the tile are 8 KB; a cluster CTA loads (and multicasts) the 16 KB half `rank`.
           const int n0 = n_blk * BLOCK_N;
           if (CLU) {
             const int h = (int)rank;
-            if (!B_MN) tma_load_2d_multicast(&tmB, &full_bar[stage], b_dst + h * 8192, kb * BLOCK_K, n0 + h * 64, 3);
-            else       tma_load_2d_multicast(&tmB, &full_bar[stage], b_dst + h * 8192, n0 + h * 64, kb * BLOCK_K, 3);
+            if (!B_MN) {
+              tma_load_2d_multicast(&tmB, &full_bar[stage], b_dst + h * 16384, kb * BLOCK_K, n0 + h * 128, 3);
+            } else {
+#pragma unroll
+              for (int c = 2 * h; c < 2 * h + 2; ++c)
+                tma_load_2d_multicast(&tmB, &full_bar[stage], b_dst + c * 8192, n0 + c * 64, kb * BLOCK_K, 3);
+            }
           } else {
             if (!B_MN) {
               tma_load_2d(&tmB, &full_bar[stage], b_dst, kb * BLOCK_K, n0);
             } else {
-              tma_load_2d(&tmB, &full_bar[stage], b_dst, n0, kb * BLOCK_K);
-              tma_load_2d(&tmB, &full_bar[stage], b_dst + 8192, n0 + 64, kb * BLOCK_K);
+#pragma unroll
+              for (int c = 0; c < 4; ++c) tma_load_2d(&tmB, &full_bar[stage], b_dst + c * 8192, n0 + c * 64, kb * BLOCK_K);
             }
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -145,10 +173,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
   } else {
     // ===================== Consumers: wgmma main loop + epilogue =====================
+    setmaxnreg_inc<232>();
+    MMB_TILE_SCHEDULE
     const int cw = wg - 1;                       // 64-row half of the CTA's tile
     const int wq = (threadIdx.x >> 5) & 3;       // warp within the warpgroup: 16-row slice
     const int lane = threadIdx.x & 31;
     const int tq = lane & 3;
+    const int rl = wq * 16 + (lane >> 2);        // this thread's first row within the warpgroup's 64 (second: +8)
+    const bool elected = (threadIdx.x & 127) == 0;
+    uint8_t* stg = sStg + cw * 2 * STG_BYTES;    // this warpgroup's two staging buffers
     // K-major SW128: 8-row groups 1024 B apart (SBO), LBO unused.  MN-major SW128: 64-element MN blocks (one TMA box,
     // BLOCK_K rows x 128 B) 8192 B apart (LBO); 8-row k groups 1024 B apart (SBO).
     constexpr uint32_t A_KSTEP = A_MN ? (WG_K / 8) * 1024 : WG_K * 2;   // bytes per k16 step
@@ -156,13 +189,27 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     constexpr uint32_t B_LBO = B_MN ? 64 * BLOCK_K * 2 : 16;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[64];
+    uint32_t stg_next = 0;                       // staging buffer of the next stored chunk (alternates per store)
+    uint32_t aux_phase = 0;                      // EPI_BF16_DACT: parity bit per staging buffer's load barrier
+    float acc[128];
     for (int t = tile_first; t < total_tiles; t += tile_step) {
       const int split = t / tiles_mn;
       const int rem = t - split * tiles_mn;
       const int m_blk = rem / p.n_tiles, n_blk = rem - m_blk * p.n_tiles;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(kb0 + p.kb_per_split, p.kb_total);
+      const int row0 = m_blk * TILE_M + (int)rank * BLOCK_M + cw * 64;   // first row of this warpgroup
+      const int col0 = n_blk * BLOCK_N;
+      if (EPI == EPI_BF16_DACT && elected) {
+        // the first two pre-activation chunks load during the main loop (the previous tile's stores have read both)
+        tma_store_wait_read<0>();
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+          if (col0 + 64 * b < p.N) {
+            mbar_arrive_expect_tx(&aux_bar[2 * cw + b], STG_BYTES);
+            tma_load_2d(&tmC1, &aux_bar[2 * cw + b], stg + b * STG_BYTES, col0 + 64 * b, row0);
+          }
+      }
       int prev_stage = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait_quiet(&full_bar[stage], phase);
@@ -172,7 +219,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / WG_K; ++k)
-          wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + (uint64_t)((k * A_KSTEP) >> 4),
+          wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + (uint64_t)((k * A_KSTEP) >> 4),
                                                       bdesc + (uint64_t)((k * B_KSTEP) >> 4), (kb > kb0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         // keep one k-block of MMAs in flight; the one before it has read its stage -> release that stage
@@ -190,74 +237,108 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if (CLU) mbar_arrive_cluster(&empty_bar[prev_stage], rank ^ 1u);
       }
 
-      // ---------------- epilogue: rows r[0], r[1] of this thread, columns n0 + 8j + 2tq (+1) ----------------
-      const int m0 = m_blk * TILE_M + (int)rank * BLOCK_M + cw * 64 + wq * 16 + (lane >> 2);
-      const int r[2] = {m0, m0 + 8};
-      const int n0 = n_blk * BLOCK_N + 2 * tq;
+      // ---------------- epilogue: rows r[0], r[1] of this thread, columns nq + 8j (+1) ----------------
+      const int r[2] = {row0 + rl, row0 + rl + 8};
+      const int nq = col0 + 2 * tq;
+      const int n_left = p.N - nq;               // columns nq + c with c < n_left exist
       const bool add_bias = (p.bias != nullptr) && (split == 0);
       if (EPI == EPI_CE_STATS) {
         const float T = __expf(__ldg(p.ce_log_scale));
         const float T2 = T * 1.4426950408889634f;
+        // one statistics part per 128 columns: the tile's columns j = 16h .. 16h + 15 form part h
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int lab = p.ce_labels ? __ldg(p.ce_labels + min(r[i], p.M - 1)) : p.ce_label0 + r[i];
-          float gm = -INFINITY;
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-              if (n0 + 8 * j + e < p.N) gm = fmaxf(gm, acc[4 * j + 2 * i + e]);
-          float m2 = gm * T2, se = 0.f, sex = 0.f, sx = 0.f;
-          if (gm > -INFINITY) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int n = n0 + 8 * j + e;
-                if (n < p.N) {
-                  const float a = acc[4 * j + 2 * i + e];
-                  const float x = a * T;
-                  const float pe = ex2_approx(fmaf(a, T2, -m2));
-                  se += pe; sex = fmaf(pe, x, sex); sx += x;
-                  if (n == lab && r[i] < p.M) p.ce_xlabel[r[i]] = x;
-                }
-              }
-          }
-          // merge the four lanes of the quad (the row's 128 columns)
-#pragma unroll
-          for (int o = 1; o <= 2; o <<= 1) {
-            const float mo = __shfl_xor_sync(0xffffffffu, m2, o);
-            const float seo = __shfl_xor_sync(0xffffffffu, se, o);
-            const float sexo = __shfl_xor_sync(0xffffffffu, sex, o);
-            const float sxo = __shfl_xor_sync(0xffffffffu, sx, o);
-            const float mn = fmaxf(m2, mo);
-            const float f = (m2 == -INFINITY) ? 0.f : ex2_approx(m2 - mn);
-            const float fo = (mo == -INFINITY) ? 0.f : ex2_approx(mo - mn);
-            se = se * f + seo * fo; sex = sex * f + sexo * fo; sx += sxo; m2 = mn;
-          }
-          if (tq == 0 && r[i] < p.M)
-            p.ce_part[(long long)r[i] * p.ce_part_ld + p.ce_part0 + n_blk] = make_float4(m2 * 0.6931471805599453f, se, sex, sx);
-        }
-      } else if (EPI == EPI_F32) {
-        float* D = reinterpret_cast<float*>(p.d0);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int n = n0 + 8 * j;
-          if (n >= p.N) continue;
-          float b0 = 0.f, b1 = 0.f;
-          if (add_bias) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+        for (int h = 0; h < 2; ++h) {
+          if (col0 + 128 * h >= p.N) continue;
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
-            if (r[i] >= p.M) continue;
-            const float v0 = fmaf(acc[4 * j + 2 * i], p.alpha, b0), v1 = fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1);
-            if (p.splitk_ws) {
-              float* dst = p.splitk_ws + ((long long)split * p.M + r[i]) * p.N + n;
-              dst[0] = v0; dst[1] = v1;
-            } else {
+            const int lab = p.ce_labels ? __ldg(p.ce_labels + min(r[i], p.M - 1)) : p.ce_label0 + r[i];
+            const int lab_off = r[i] < p.M ? lab - nq : -1;   // the label column's offset from nq (-1: none)
+            float gm = -INFINITY;
+#pragma unroll
+            for (int j = 16 * h; j < 16 * h + 16; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                if (8 * j + e < n_left) gm = fmaxf(gm, acc[4 * j + 2 * i + e]);
+            float m2 = gm * T2, se = 0.f, sex = 0.f, sx = 0.f;
+            if (gm > -INFINITY) {
+#pragma unroll
+              for (int j = 16 * h; j < 16 * h + 16; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  if (8 * j + e < n_left) {
+                    const float a = acc[4 * j + 2 * i + e];
+                    const float x = a * T;
+                    const float pe = ex2_approx(fmaf(a, T2, -m2));
+                    se += pe; sex = fmaf(pe, x, sex); sx += x;
+                    if (8 * j + e == lab_off) p.ce_xlabel[r[i]] = x;
+                  }
+                }
+            }
+            // merge the four lanes of the quad (the row's 128 columns)
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+              const float mo = __shfl_xor_sync(0xffffffffu, m2, o);
+              const float seo = __shfl_xor_sync(0xffffffffu, se, o);
+              const float sexo = __shfl_xor_sync(0xffffffffu, sex, o);
+              const float sxo = __shfl_xor_sync(0xffffffffu, sx, o);
+              const float mn = fmaxf(m2, mo);
+              const float f = (m2 == -INFINITY) ? 0.f : ex2_approx(m2 - mn);
+              const float fo = (mo == -INFINITY) ? 0.f : ex2_approx(mo - mn);
+              se = se * f + seo * fo; sex = sex * f + sexo * fo; sx += sxo; m2 = mn;
+            }
+            if (tq == 0 && r[i] < p.M)
+              p.ce_part[(long long)r[i] * p.ce_part_ld + p.ce_part0 + 2 * n_blk + h] =
+                  make_float4(m2 * 0.6931471805599453f, se, sex, sx);
+          }
+        }
+      } else if (EPI == EPI_F32) {
+        if (p.f32_direct) {
+          float* D = reinterpret_cast<float*>(p.d0);
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const int n = nq + 8 * j;
+            if (n >= p.N) continue;
+            float b0 = 0.f, b1 = 0.f;
+            if (add_bias) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              if (r[i] >= p.M) continue;
+              const float v0 = fmaf(acc[4 * j + 2 * i], p.alpha, b0), v1 = fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1);
               float* dst = D + (long long)r[i] * p.ldd0 + n;
               if (p.accumulate) { dst[0] += v0; dst[1] += v1; }
               else              { dst[0] = v0; dst[1] = v1; }
             }
+          }
+        } else {
+          // eight chunks of 32 fp32 columns; 16-byte unit u of a 128-byte row sits at u ^ (row % 8) (SWIZZLE_128B)
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            if (col0 + 32 * q >= p.N) continue;
+            uint8_t* buf = stg + (stg_next & 1u) * STG_BYTES;
+            if (elected) tma_store_wait_read<1>();
+            wg_bar_sync(cw);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * q + jj;
+              const int n = nq + 8 * j;
+              float b0 = 0.f, b1 = 0.f;
+              if (add_bias && n < p.N) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                const int rr = rl + 8 * i;
+                float2* sp = reinterpret_cast<float2*>(buf + rr * 128 + (((2 * jj + (tq >> 1)) ^ (rr & 7)) << 4) + 8 * (tq & 1));
+                *sp = make_float2(fmaf(acc[4 * j + 2 * i], p.alpha, b0), fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1));
+              }
+            }
+            fence_proxy_async_smem();
+            wg_bar_sync(cw);
+            if (elected) {
+              if (p.splitk_ws)       tma_store_2d(&tmC0, buf, col0 + 32 * q, split * p.ws_rows + row0);
+              else if (p.accumulate) tma_reduce_add_2d(&tmC0, buf, col0 + 32 * q, row0);
+              else                   tma_store_2d(&tmC0, buf, col0 + 32 * q, row0);
+              tma_store_commit();
+            }
+            ++stg_next;
           }
         }
       } else {
@@ -277,86 +358,131 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
         }
         const bool do_colsum = (EPI == EPI_BF16 || EPI == EPI_BF16_DACT) && p.colsum_part != nullptr;
+        // this warp's column sums over its 16 rows, column pair 8j + 2tq of j = 8q + lane / 4 kept by this lane
+        float cs_keep[4][2];
+        // EPI_BF16_ACT stores PRE in the first pass and act(PRE) (recomputed from the accumulators) in the second
+        constexpr int PASSES = EPI == EPI_BF16_ACT ? 2 : 1;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int n = n0 + 8 * j;
-          const bool col_ok = n < p.N;
-          float b0 = 0.f, b1 = 0.f;
-          if (add_bias && col_ok) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
-          float cs0 = 0.f, cs1 = 0.f;
+        for (int ps = 0; ps < PASSES; ++ps) {
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const bool ok = col_ok && r[i] < p.M;
-            float f0, f1;
-            if (EPI == EPI_CE_GRAD) {
-              // d(loss_weight * mean CE) / d sims of this row block, plus (columns [col_lo, col_hi)) the transposed
-              // other-direction term rebuilt from the column LSEs -- see contrastive_ce_grad_kernel (loss.cu)
-              float f[2];
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int c = n + e;
-                const float a = acc[4 * j + 2 * i + e];
-                const float tt = ((c == p.ce_label0 + r[i]) ? (1.f - p.ce_smoothing) : 0.f) + ce_eps_n;
-                float gsum = ce_gsT[i] * (ex2_approx(fmaf(a, ce_T2, -ce_lse2[i])) - tt);
-                if (p.ce_lse_col != nullptr && c >= p.ce_col_lo && c < p.ce_col_hi && c < p.N) {
-                  const float wc = p.ce_col_w ? p.ce_loss_weight * ce_T * __ldg(p.ce_col_w + c) : ce_gcT;
-                  if (wc != 0.f) gsum += wc * (ex2_approx(fmaf(a, ce_T2, -__ldg(p.ce_lse_col + c) * 1.4426950408889634f)) - tt);
-                }
-                f[e] = gsum;
-              }
-              f0 = f[0]; f1 = f[1];
+          for (int q = 0; q < 4; ++q) {
+            cs_keep[q][0] = cs_keep[q][1] = 0.f;
+            if (col0 + 64 * q >= p.N) continue;
+            // 64-column chunk q; 16-byte unit jj of a 128-byte row sits at jj ^ (row % 8) (SWIZZLE_128B)
+            const uint32_t b = EPI == EPI_BF16_DACT ? (uint32_t)(q & 1) : (stg_next & 1u);
+            uint8_t* buf = stg + b * STG_BYTES;
+            if (EPI == EPI_BF16_DACT) {
+              mbar_wait_quiet(&aux_bar[2 * cw + b], (aux_phase >> b) & 1u);
+              aux_phase ^= 1u << b;
             } else {
-              f0 = fmaf(acc[4 * j + 2 * i], p.alpha, b0);
-              f1 = fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1);
+              if (elected) tma_store_wait_read<1>();
+              wg_bar_sync(cw);
             }
-            if (EPI == EPI_BF16_DACT && ok) {
-              const uint32_t av = *reinterpret_cast<const uint32_t*>(p.aux + (long long)r[i] * p.ld_aux + n);
-              f0 *= act_grad<ACT>(bf16_lo(av));
-              f1 *= act_grad<ACT>(bf16_hi(av));
-            }
-            if (ok) {
-              const uint32_t o = pack_bf16x2(f0, f1);
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.d0) + (long long)r[i] * p.ldd0 + n) = o;
-              if (EPI == EPI_BF16_ACT) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * q + jj;
+              const int n = nq + 8 * j;
+              const bool col_ok = n < p.N;
+              float b0 = 0.f, b1 = 0.f;
+              if (add_bias && col_ok) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+              float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                const int rr = rl + 8 * i;
+                uint32_t* sp = reinterpret_cast<uint32_t*>(buf + rr * 128 + ((jj ^ (rr & 7)) << 4) + 4 * tq);
+                float f0, f1;
+                if (EPI == EPI_CE_GRAD) {
+                  // d(loss_weight * mean CE) / d sims of this row block, plus (columns [col_lo, col_hi)) the transposed
+                  // other-direction term rebuilt from the column LSEs -- see contrastive_ce_grad_kernel (loss.cu)
+                  float f[2];
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) {
+                    const int c = n + e;
+                    const float a = acc[4 * j + 2 * i + e];
+                    const float tt = ((c == p.ce_label0 + r[i]) ? (1.f - p.ce_smoothing) : 0.f) + ce_eps_n;
+                    float gsum = ce_gsT[i] * (ex2_approx(fmaf(a, ce_T2, -ce_lse2[i])) - tt);
+                    if (p.ce_lse_col != nullptr && c >= p.ce_col_lo && c < p.ce_col_hi && c < p.N) {
+                      const float wc = p.ce_col_w ? p.ce_loss_weight * ce_T * __ldg(p.ce_col_w + c) : ce_gcT;
+                      if (wc != 0.f) gsum += wc * (ex2_approx(fmaf(a, ce_T2, -__ldg(p.ce_lse_col + c) * 1.4426950408889634f)) - tt);
+                    }
+                    f[e] = gsum;
+                  }
+                  f0 = f[0]; f1 = f[1];
+                } else {
+                  f0 = fmaf(acc[4 * j + 2 * i], p.alpha, b0);
+                  f1 = fmaf(acc[4 * j + 2 * i + 1], p.alpha, b1);
+                }
+                if (EPI == EPI_BF16_DACT) {
+                  const uint32_t av = *sp;   // pre-activation, loaded into this very slot by TMA
+                  f0 *= act_grad<ACT>(bf16_lo(av));
+                  f1 *= act_grad<ACT>(bf16_hi(av));
+                }
+                uint32_t o = pack_bf16x2(f0, f1);
                 // the activation is applied to the bf16-ROUNDED pre-activation: exactly what the backward (which only
                 // sees the stored bf16 pre-activation) differentiates
-                store_bf16x2(p.d1, p.ldd1, r[i], n, act_fn<ACT>(bf16_lo(o)), act_fn<ACT>(bf16_hi(o)));
+                if (EPI == EPI_BF16_ACT && ps == 1) o = pack_bf16x2(act_fn<ACT>(bf16_lo(o)), act_fn<ACT>(bf16_hi(o)));
+                *sp = o;
+                if (do_colsum && col_ok && r[i] < p.M) { cs0 += bf16_lo(o); cs1 += bf16_hi(o); }
               }
-              if (do_colsum) { cs0 += bf16_lo(o); cs1 += bf16_hi(o); }
-            }
-          }
-          if (do_colsum) {
-            // column sums of the rounded output over the warp's 16 rows (lanes sharing tq) -> this warp's smem row
+              if (do_colsum) {
+                // column sums of the rounded output over the warp's 16 rows (lanes sharing tq)
 #pragma unroll
-            for (int o = 4; o <= 16; o <<= 1) {
-              cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
-              cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
+                for (int o = 4; o <= 16; o <<= 1) {
+                  cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
+                  cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
+                }
+                if ((lane >> 2) == jj) { cs_keep[q][0] = cs0; cs_keep[q][1] = cs1; }
+              }
             }
-            if (lane < 4) {
-              sCol[(cw * 4 + wq) * BLOCK_N + 8 * j + 2 * tq] = cs0;
-              sCol[(cw * 4 + wq) * BLOCK_N + 8 * j + 2 * tq + 1] = cs1;
+            fence_proxy_async_smem();
+            wg_bar_sync(cw);
+            if (elected) {
+              tma_store_2d(EPI == EPI_BF16_ACT && ps == 1 ? &tmC1 : &tmC0, buf, col0 + 64 * q, row0);
+              tma_store_commit();
+              if (EPI == EPI_BF16_DACT && q + 2 < 4 && col0 + 64 * (q + 2) < p.N) {
+                // this buffer's next pre-activation chunk, once the store has read it
+                tma_store_wait_read<0>();
+                mbar_arrive_expect_tx(&aux_bar[2 * cw + b], STG_BYTES);
+                tma_load_2d(&tmC1, &aux_bar[2 * cw + b], buf, col0 + 64 * (q + 2), row0);
+              }
             }
+            if (EPI != EPI_BF16_DACT) ++stg_next;
           }
         }
         if (do_colsum) {
           // the 8 consumer warps' sums in warp order -> one partial row per 128-row block (no atomics: the host reduces
-          // the blocks in order, so the result does not depend on which CTA finishes first)
+          // the blocks in order, so the result does not depend on which CTA finishes first).  The per-warp rows live
+          // in the warpgroup's staging buffers, once their last store has read them.
+          if (elected) tma_store_wait_read<0>();
+          wg_bar_sync(cw);
+          float* sCol = reinterpret_cast<float*>(stg) + wq * BLOCK_N;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int c = 8 * (8 * q + (lane >> 2)) + 2 * tq;
+            sCol[c] = cs_keep[q][0];
+            sCol[c + 1] = cs_keep[q][1];
+          }
           asm volatile("bar.sync 1, 256;" ::: "memory");
           const int ct = threadIdx.x - 128, blk_row = m_blk * TILE_M + (int)rank * BLOCK_M;
-          if (ct < BLOCK_N && blk_row < p.M && n_blk * BLOCK_N + ct < p.N) {
-            float t = 0.f;
+          if (blk_row < p.M && col0 + ct < p.N) {
+            const float* all = reinterpret_cast<const float*>(sStg);
+            float s = 0.f;
 #pragma unroll
-            for (int w = 0; w < 8; ++w) t += sCol[w * BLOCK_N + ct];
-            p.colsum_part[(long long)(blk_row / BLOCK_M) * p.N + n_blk * BLOCK_N + ct] = t;
+            for (int w = 0; w < 8; ++w) s += all[(w >> 2) * (2 * STG_BYTES / 4) + (w & 3) * BLOCK_N + ct];
+            p.colsum_part[(long long)(blk_row / BLOCK_M) * p.N + col0 + ct] = s;
           }
+          fence_proxy_async_smem();   // these generic reads come before the next TMA writes into the staging buffers
           asm volatile("bar.sync 1, 256;" ::: "memory");
         }
       }
     }
+    // the global writes of the last stores complete before the CTA retires
+    if (elected) tma_store_wait_all<0>();
   }
   // cluster: nobody exits while the peer may still multicast into it or arrive on its barriers
   if (CLU) cluster_sync_all();
 }
+#undef MMB_TILE_SCHEDULE
 
 // ----------------------------------------------------------------------------------------------
 // Host side
@@ -456,7 +582,8 @@ int num_sms() {
 }
 
 template <bool A_MN, bool B_MN, int EPI, int ACT, bool CLU>
-static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const GemmArgs& args, cudaStream_t stream) {
+static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC0, const CUtensorMap& tC1,
+                       const GemmArgs& args, cudaStream_t stream) {
   auto kfn = gemm_kernel<A_MN, B_MN, EPI, ACT, CLU>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -479,7 +606,7 @@ static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const GemmA
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = GEMM_SMEM_BYTES;
   cfg.stream = stream;
-  return (int)cudaLaunchKernelEx(&cfg, kfn, tA, tB, args);
+  return (int)cudaLaunchKernelEx(&cfg, kfn, tA, tB, tC0, tC1, args);
 }
 
 }  // namespace mmb
@@ -487,7 +614,7 @@ static int launch_impl(const CUtensorMap& tA, const CUtensorMap& tB, const GemmA
 using namespace mmb;
 
 // Test / A-B hook: force the kernel variant mmb_gemm_bf16 dispatches to (process-wide).
-//   cta2: -1 = automatic (size heuristic), 0 = one CTA per 128x128 tile, 1 = 2-CTA clusters (256x128 tiles, B multicast)
+//   cta2: -1 = automatic (size heuristic), 0 = one CTA per 128x256 tile, 1 = 2-CTA clusters (256x256 tiles, B multicast)
 //   epilogue_warps: 0 or 8 (the two consumer warpgroups run the epilogue; kept for ABI compatibility)
 static int g_force_cta2 = -1;
 extern "C" int mmb_gemm_set_mode(int cta2, int epilogue_warps) {
@@ -496,16 +623,17 @@ extern "C" int mmb_gemm_set_mode(int cta2, int epilogue_warps) {
   return MMB_OK;
 }
 
-// D[m, n] = (accumulate ? D[m, n] : 0) + sum_{s = 0..S-1} ws[s][m][n], splits added in order (N % 4 == 0)
-__global__ void splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int N, float* __restrict__ D, long long ldd,
-                                     int accumulate) {
+// D[m, n] = (accumulate ? D[m, n] : 0) + sum_{s = 0..S-1} ws[s][m][n], splits added in order (N % 4 == 0); a split
+// holds ws_rows >= M rows
+__global__ void splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int ws_rows, int N, float* __restrict__ D,
+                                     long long ldd, int accumulate) {
   const int n = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (n >= N) return;
   for (int m = blockIdx.y; m < M; m += gridDim.y) {
     float* dst = D + (long long)m * ldd + n;
     float4 acc = accumulate ? make_float4(dst[0], dst[1], dst[2], dst[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
     for (int s = 0; s < S; ++s) {
-      const float4 v = *reinterpret_cast<const float4*>(ws + ((long long)s * M + m) * N + n);
+      const float4 v = *reinterpret_cast<const float4*>(ws + ((long long)s * ws_rows + m) * N + n);
       acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
     }
     dst[0] = acc.x; dst[1] = acc.y; dst[2] = acc.z; dst[3] = acc.w;
@@ -513,7 +641,8 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int S, int M,
 }
 
 static int gemm_launch(int a_mn_major, int b_mn_major, int epilogue, int act, bool cta2, const CUtensorMap& tA,
-                       const CUtensorMap& tB, const GemmArgs& g, cudaStream_t stream);
+                       const CUtensorMap& tB, const CUtensorMap& tC0, const CUtensorMap& tC1, const GemmArgs& g,
+                       cudaStream_t stream);
 
 static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const void* B, long long ldb, int b_mn_major,
                          void* D0, long long ldd0, void* D1, long long ldd1, int M, int N, int K, int epilogue, int act,
@@ -524,7 +653,7 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
   if ((epilogue == EPI_CE_STATS || epilogue == EPI_CE_GRAD) && (!ce || a_mn_major || b_mn_major)) return MMB_ERR_ARG;
   if ((lda & 7) || (ldb & 7)) return MMB_ERR_ARG;
   if (epilogue != EPI_CE_STATS && (epilogue == EPI_F32 ? (N & 3) : (N & 7))) return MMB_ERR_ARG;   // CE_STATS writes no tensor
-  // 2-CTA clusters (256x128 tiles, B multicast) for everything large enough to fill the SM pairs at least once
+  // 2-CTA clusters (256x256 tiles, B multicast) for everything large enough to fill the SM pairs at least once
   const long long big_tiles = (long long)((M + 2 * BLOCK_M - 1) / (2 * BLOCK_M)) * ((N + BLOCK_N - 1) / BLOCK_N);
   const bool cta2 = g_force_cta2 == 1 ||
                     (g_force_cta2 == -1 && M >= 512 && big_tiles * (splits < 1 ? 1 : splits) >= num_sms() / 2);
@@ -552,7 +681,8 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
     if (!g.colsum_part) return (int)cudaErrorMemoryAllocation;
   }
   if (epilogue == EPI_F32 && g.splits > 1) {
-    g.splitk_ws = static_cast<float*>(scratch(SCR_GEMM_SPLITK, (size_t)g.splits * M * N * sizeof(float), stream));
+    g.ws_rows = g.m_tiles * (cta2 ? 2 * BLOCK_M : BLOCK_M);   // whole tiles: TMA stores need not clip inside a split
+    g.splitk_ws = static_cast<float*>(scratch(SCR_GEMM_SPLITK, (size_t)g.splits * g.ws_rows * N * sizeof(float), stream));
     if (!g.splitk_ws) return (int)cudaErrorMemoryAllocation;
   }
 
@@ -562,23 +692,37 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
   if (!a_mn_major) rc = make_tmap_2d(&tA, A, 2, false, K, M, lda * 2, 64, BLOCK_M);
   else             rc = make_tmap_2d(&tA, A, 2, false, M, K, lda * 2, 64, BLOCK_K);
   if (rc) return rc;
-  // B: a cluster CTA loads (and multicasts) half of the 128-row tile
+  // B: a cluster CTA loads (and multicasts) half of the 256-row tile
   if (!b_mn_major) rc = make_tmap_2d(&tB, B, 2, false, K, N, ldb * 2, 64, cta2 ? BLOCK_N / 2 : BLOCK_N);
   else             rc = make_tmap_2d(&tB, B, 2, false, N, K, ldb * 2, 64, BLOCK_K);
   if (rc) return rc;
+  // epilogue tensor maps: 64-row x 128-byte boxes, clipped by TMA at M and N
+  CUtensorMap tC0 = tA, tC1 = tA;   // unused ones stay a copy of tA and are never read
   if (epilogue == EPI_F32) {
     if (ldd0 & 3) return MMB_ERR_ARG;
+    if (g.splitk_ws) {
+      rc = make_tmap_2d(&tC0, g.splitk_ws, 4, true, N, (uint64_t)g.splits * g.ws_rows, (uint64_t)N * 4, 32, 64);
+    } else if ((reinterpret_cast<uintptr_t>(D0) & 15) == 0 && (ldd0 & 3) == 0) {
+      rc = make_tmap_2d(&tC0, D0, 4, true, N, M, ldd0 * 4, 32, 64);
+    } else {
+      g.f32_direct = 1;   // e.g. a column slice of an fp32 tensor: TMA needs a 16-byte aligned base
+    }
+    if (rc) return rc;
   } else if (epilogue != EPI_CE_STATS) {
     if ((ldd0 & 7) || (reinterpret_cast<uintptr_t>(D0) & 15)) return MMB_ERR_ARG;
     if (epilogue == EPI_BF16_ACT && (!D1 || (ldd1 & 7) || (reinterpret_cast<uintptr_t>(D1) & 15))) return MMB_ERR_ARG;
     if (epilogue == EPI_BF16_DACT && (!aux || (ld_aux & 7) || (reinterpret_cast<uintptr_t>(aux) & 15))) return MMB_ERR_ARG;
+    rc = make_tmap_2d(&tC0, D0, 2, false, N, M, ldd0 * 2, 64, 64);
+    if (!rc && epilogue == EPI_BF16_ACT) rc = make_tmap_2d(&tC1, D1, 2, false, N, M, ldd1 * 2, 64, 64);
+    if (!rc && epilogue == EPI_BF16_DACT) rc = make_tmap_2d(&tC1, aux, 2, false, N, M, ld_aux * 2, 64, 64);
+    if (rc) return rc;
   }
 
-  int rc_launch = gemm_launch(a_mn_major, b_mn_major, epilogue, act, cta2, tA, tB, g, stream);
+  int rc_launch = gemm_launch(a_mn_major, b_mn_major, epilogue, act, cta2, tA, tB, tC0, tC1, g, stream);
   if (rc_launch) return rc_launch;
   if (g.splitk_ws) {
-    splitk_reduce_kernel<<<dim3((N / 4 + 127) / 128, M < 65535 ? M : 65535), 128, 0, stream>>>(g.splitk_ws, g.splits, M, N,
-                                                                         reinterpret_cast<float*>(D0), ldd0, g.accumulate);
+    splitk_reduce_kernel<<<dim3((N / 4 + 127) / 128, M < 65535 ? M : 65535), 128, 0, stream>>>(
+        g.splitk_ws, g.splits, M, g.ws_rows, N, reinterpret_cast<float*>(D0), ldd0, g.accumulate);
     rc_launch = (int)cudaGetLastError();
     if (rc_launch) return rc_launch;
   }
@@ -587,18 +731,19 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
 }
 
 static int gemm_launch(int a_mn_major, int b_mn_major, int epilogue, int act, bool cta2, const CUtensorMap& tA,
-                       const CUtensorMap& tB, const GemmArgs& g, cudaStream_t stream) {
+                       const CUtensorMap& tB, const CUtensorMap& tC0, const CUtensorMap& tC1, const GemmArgs& g,
+                       cudaStream_t stream) {
   const int am = a_mn_major ? 1 : 0, bm = b_mn_major ? 1 : 0;
   if (epilogue == EPI_CE_STATS)
-    return cta2 ? launch_impl<false, false, EPI_CE_STATS, 0, true>(tA, tB, g, stream)
-                : launch_impl<false, false, EPI_CE_STATS, 0, false>(tA, tB, g, stream);
+    return cta2 ? launch_impl<false, false, EPI_CE_STATS, 0, true>(tA, tB, tC0, tC1, g, stream)
+                : launch_impl<false, false, EPI_CE_STATS, 0, false>(tA, tB, tC0, tC1, g, stream);
   if (epilogue == EPI_CE_GRAD)
-    return cta2 ? launch_impl<false, false, EPI_CE_GRAD, 0, true>(tA, tB, g, stream)
-                : launch_impl<false, false, EPI_CE_GRAD, 0, false>(tA, tB, g, stream);
+    return cta2 ? launch_impl<false, false, EPI_CE_GRAD, 0, true>(tA, tB, tC0, tC1, g, stream)
+                : launch_impl<false, false, EPI_CE_GRAD, 0, false>(tA, tB, tC0, tC1, g, stream);
 #define MMB_CASE(AM, BM, E, AC)                                                                                   \
   if (am == AM && bm == BM && epilogue == E && (AC < 0 || act == AC))                                             \
-    return cta2 ? launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), true>(tA, tB, g, stream)                \
-                : launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), false>(tA, tB, g, stream);
+    return cta2 ? launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), true>(tA, tB, tC0, tC1, g, stream)                \
+                : launch_impl<(AM != 0), (BM != 0), E, (AC < 0 ? 0 : AC), false>(tA, tB, tC0, tC1, g, stream);
   MMB_CASE(0, 0, EPI_BF16, -1)
   MMB_CASE(0, 0, EPI_BF16_ACT, ACT_QUICK_GELU)
   MMB_CASE(0, 0, EPI_BF16_ACT, ACT_GELU_ERF)
@@ -622,8 +767,9 @@ extern "C" int mmb_gemm_bf16(const void* A, long long lda, int a_mn_major, const
 }
 
 // ---- fused similarity GEMM + temperature-scaled cross-entropy (no logits in HBM) ------------------------------------
-// Number of float4 partials per row one mmb_gemm_ce_stats launch over N columns writes (one per 128-column tile).
-extern "C" int mmb_gemm_ce_num_parts(int N) { return N <= 0 ? 0 : (N + BLOCK_N - 1) / BLOCK_N; }
+// Number of float4 partials per row one mmb_gemm_ce_stats launch over N columns writes (one per 128 columns: a
+// 256-column tile writes two).
+extern "C" int mmb_gemm_ce_num_parts(int N) { return N <= 0 ? 0 : (N + 127) / 128; }
 
 static int gemm_ce_stats_impl(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K,
                               const float* log_scale, int label0, const int* labels, void* part, int part_ld, int part0,

@@ -116,9 +116,11 @@ def _clusters_on_current_device() -> int:
 
 
 def wgrad_splits(out_rows: int, out_cols: int, k: int, n_units: Optional[int] = None) -> int:
-    """Split-K factor for a weight-gradient GEMM so that the (256 x 128, one per 2-CTA cluster) tile count fills the
-    machine.  n_units = 2-CTA clusters the GPU holds at once (default: half the current device's SM count, e.g. 66 on
-    an H100 SXM, 57 on an H100 PCIe)."""
+    """Split-K factor for a weight-gradient GEMM so that the output's 256 x 128 blocks fill the machine (a 2-CTA
+    cluster computes a 256 x 256 tile, two such blocks).  The count is kept at 256 x 128 so that every weight gradient
+    keeps its split count, and with it its fp32 summation order: a changed split count reassociates the sum, and Adam's
+    normalised update turns that into visibly different weights within a step.  n_units = 2-CTA clusters the GPU
+    holds at once (default: half the current device's SM count, e.g. 66 on an H100 SXM, 57 on an H100 PCIe)."""
     if n_units is None:
         n_units = _clusters_on_current_device()
     tiles = ((out_rows + 255) // 256) * ((out_cols + 127) // 128)
