@@ -165,18 +165,22 @@ int mmb_memset_async(void* p, int value, long long bytes, void* stream);
 int mmb_act_fwd(const float* x, float* y, long long n, int kind, void* stream);
 
 /* ---- attention --------------------------------------------------------------------------------------------- */
-/* O = softmax(Q K^T * scale [+ causal mask]) V per (batch, head), head_dim 64, S <= 384 (tensor-core kernels; larger S
- * returns MMB_ERR_UNSUPPORTED); qkv bf16 [B*S, 3*H*64] packed [q|k|v], out bf16 [B*S, H*64], lse fp32 [B,H,S].  Replaces F.scaled_dot_product_attention (torch/nn/functional.py:6682). */
+/* O = softmax(Q K^T * scale [+ causal mask]) V per (batch, head), head_dim 64, any S (tensor-core kernels: one CTA per
+ * head with the whole head in shared memory up to S = 384, K / V streamed through shared memory above); qkv bf16
+ * [B*S, 3*H*64] packed [q|k|v], out bf16 [B*S, H*64], lse fp32 [B,H,S] in natural-log units (may be NULL for
+ * forward-only callers; a row with no visible key gets O = 0 and lse = -inf).  B and H are at most 65535 above S = 384.
+ * Replaces F.scaled_dot_product_attention (torch/nn/functional.py:6682). */
 int mmb_attention_fwd(const void* qkv, void* out, float* lse, int B, int S, int H, int head_dim, int causal,
                       float scale, void* stream);
 int mmb_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, int B, int S,
                       int H, int head_dim, int causal, float scale, void* stream);
-/* Number of kernels one mmb_attention_bwd call launches at sequence length S (always 1: one kernel computes dQ, dK
- * and dV) — for callers that count launches. */
+/* Number of kernels one mmb_attention_bwd(_kmask) call launches at sequence length S — for callers that count launches.
+ * 1 up to S = 384 (one kernel computes dQ, dK and dV); 2 above (a dQ kernel that also writes rowsum(dO * O) to library
+ * scratch, then a dK / dV kernel), both deterministic without atomics. */
 int mmb_attention_bwd_launches(int S);
 
 /* Same with a key-padding mask [B,S] (1 = attend, 0 = masked_fill(-inf)): the BERT-style attention of the FLAVA text
- * tower (modules/encoders/bert_text_encoder.py:87-93 -> modules/layers/attention.py:228-229).  S <= 384. */
+ * tower (modules/encoders/bert_text_encoder.py:87-93 -> modules/layers/attention.py:228-229).  Any S, as above. */
 int mmb_attention_fwd_kmask(const void* qkv, void* out, float* lse, const unsigned char* kmask, int B, int S, int H,
                             int head_dim, int causal, float scale, void* stream);
 
@@ -209,7 +213,7 @@ int mmb_concat_tokens(const float* cls, const float* a, const float* b, float* o
 
 
 /* ---- FLAVA encoders, backward (config 3 as a training step; autograd of the files cited on the forward entries) -- */
-/* Backward of mmb_attention_fwd_kmask (S <= 384): masked keys get P = dS = 0. */
+/* Backward of mmb_attention_fwd_kmask (any S): masked keys get P = dS = 0, i.e. zero dK / dV rows. */
 int mmb_attention_bwd_kmask(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                             const unsigned char* kmask, int B, int S, int H, int head_dim, int causal, float scale,
                             void* stream);

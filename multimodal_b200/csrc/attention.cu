@@ -3,35 +3,19 @@
 // (S = 384: 48 KB each), so each direction is a single pass: no split-KV, no second kernel, no scratch in HBM.  Operands
 // are read straight out of the packed in-projection output [B*S, 3d] ([q | k | v], head h at columns h*64) and O is
 // written as [B*S, d], the operand layout of the out-projection GEMM: no head split / merge copies.
-// Replaces F.scaled_dot_product_attention + autograd (torch/nn/functional.py:6682).
+// Replaces F.scaled_dot_product_attention + autograd (torch/nn/functional.py:6682).  Longer sequences go to the
+// streamed kernels of attention_stream.cu through the same entry points.
 //
 // Math: softmax(Q K^T * scale) V with fp32 statistics; P (and dS) are rounded to bf16 for the second product.  Each warp
 // owns 16-row tiles and runs m16n8k16 bf16 MMAs (fp32 accumulate) on fragments loaded with ldmatrix from XOR-swizzled
 // shared tiles.  Optional key-padding mask [B,S] (1 = attend) and causal mask.
-#include "common.cuh"
+#include "attention_tiles.cuh"
 #include "mmb200_internal.h"
 #include <stdlib.h>
 
 namespace mmb {
 
-constexpr int HD = 64;
 constexpr int SMAX = 384;
-
-// byte offset of element (r, c) (c multiple of 8) in a [rows][64] bf16 tile with 16B-chunk XOR swizzle
-__device__ __forceinline__ uint32_t toff(int r, int c) { return (uint32_t)(r * 128 + ((((c >> 3) ^ (r & 7))) << 4)); }
-
-// A fragment (16 rows x 16 k) at rows r0.., cols c0.. of a row-major tile
-__device__ __forceinline__ void load_a(uint32_t (&a)[4], uint32_t base, int r0, int c0, int lane) {
-  ldsm_x4(a, base + toff(r0 + (lane & 7) + ((lane >> 3) & 1) * 8, c0 + (lane >> 4) * 8));
-}
-// B fragments from a tile stored [n][k] (k contiguous): 8 n-rows at n0, 32 k at k0 -> {b0,b1} for k-step k0 and k0+16
-__device__ __forceinline__ void load_b_nk(uint32_t (&b)[4], uint32_t base, int n0, int k0, int lane) {
-  ldsm_x4(b, base + toff(n0 + (lane & 7), k0 + (lane >> 3) * 8));
-}
-// B fragments from a tile stored [k][n] (n contiguous): 16 k-rows at k0, 16 n at n0 -> {b0,b1} for n-tile n0 and n0+8
-__device__ __forceinline__ void load_b_kn(uint32_t (&b)[4], uint32_t base, int k0, int n0, int lane) {
-  ldsm_x4_t(b, base + toff(k0 + (lane & 7) + ((lane >> 3) & 1) * 8, n0 + (lane >> 4) * 8));
-}
 
 // cooperative load of rows [0,S) x 64 columns of a strided bf16 matrix into a swizzled tile; rows [S,S_pad) zeroed
 __device__ __forceinline__ void load_tile(uint8_t* dst, const __nv_bfloat16* src, long long ld, int S, int S_pad) {
@@ -42,16 +26,6 @@ __device__ __forceinline__ void load_tile(uint8_t* dst, const __nv_bfloat16* src
     *reinterpret_cast<uint4*>(dst + toff(r, ch * 8)) = v;
   }
 }
-// 16-byte cp.async into shared memory; src_bytes = 0 writes zeros without reading src
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-// the mbarrier completes one arrival of this thread once all of its earlier cp.async copies have landed
-__device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
 // asynchronous form of load_tile for rows [r0, r1) (r1 <= S_pad); rows >= S are zero-filled
 __device__ __forceinline__ void cp_tile_rows(uint8_t* dst, const __nv_bfloat16* src, long long ld, int S, int r0,
                                              int r1) {
@@ -65,15 +39,6 @@ __device__ __forceinline__ void cp_tile_rows(uint8_t* dst, const __nv_bfloat16* 
 // key-valid flags: k < S and (no mask or mask[k] != 0)
 __device__ __forceinline__ void load_keymask(uint8_t* dst, const uint8_t* kmask, int S, int S_pad) {
   for (int i = threadIdx.x; i < S_pad; i += blockDim.x) dst[i] = (i < S && (!kmask || kmask[i])) ? 1 : 0;
-}
-
-__device__ __forceinline__ float quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -640,7 +605,9 @@ static int pick_threads(int S) {
 
 static int attention_fwd_impl(const void* qkv, void* out, float* lse, const uint8_t* kmask, int B, int S, int H,
                               int causal, float scale, void* stream) {
-  if (B <= 0 || S <= 0 || H <= 0 || S > SMAX) return MMB_ERR_UNSUPPORTED;
+  if (B <= 0 || S <= 0 || H <= 0) return MMB_ERR_UNSUPPORTED;
+  if (S > SMAX)   // the head no longer fits in shared memory: stream K / V
+    return attention_fwd_stream(qkv, out, lse, kmask, B, S, H, causal, scale, reinterpret_cast<cudaStream_t>(stream));
   const int S_pad = (S + 15) & ~15;
   const int smem = 3 * S_pad * 128 + 8 * (SMAX / 64) + S_pad;
   const float scale_log2 = scale * 1.4426950408889634f;
@@ -654,7 +621,10 @@ static int attention_fwd_impl(const void* qkv, void* out, float* lse, const uint
 
 static int attention_bwd_impl(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                               const uint8_t* kmask, int B, int S, int H, int causal, float scale, void* stream) {
-  if (B <= 0 || S <= 0 || H <= 0 || S > SMAX) return MMB_ERR_UNSUPPORTED;
+  if (B <= 0 || S <= 0 || H <= 0) return MMB_ERR_UNSUPPORTED;
+  if (S > SMAX)
+    return attention_bwd_stream(qkv, out, dout, lse, dqkv, kmask, B, S, H, causal, scale,
+                                reinterpret_cast<cudaStream_t>(stream));
   const int S_pad = (S + 15) & ~15;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (S_pad <= BWD_STAGED_MAX) {   // Q, K, V, dO and dS^T fit in shared memory
@@ -680,7 +650,7 @@ static int attention_bwd_impl(const void* qkv, const void* out, const void* dout
 using namespace mmb;
 
 // kernels one mmb_attention_bwd call launches at sequence length S (callers that count launches: bench.py)
-extern "C" int mmb_attention_bwd_launches(int) { return 1; }
+extern "C" int mmb_attention_bwd_launches(int S) { return S > SMAX ? ATTN_BWD_STREAM_LAUNCHES : 1; }
 
 extern "C" int mmb_attention_fwd(const void* qkv, void* out, float* lse, int B, int S, int H, int head_dim, int causal,
                                  float scale, void* stream) {

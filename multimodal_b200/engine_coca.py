@@ -93,7 +93,7 @@ class LayerStack:
             else:
                 ops.add_layernorm_fwd(XA, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
             ops.gemm(LN, wqkv, bias=bqkv, out=QKV)
-            if mask is None and hd == 64 and S <= 384:
+            if mask is None and hd == 64 and (S <= 384 or S > ops.GENERIC_FWD_MAX_S):
                 ops.attention_fwd(QKV, O, None, B, S, H, causal, scale)
             else:
                 ops.attention_fwd_generic(QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], O, B=B, Sq=S, Skv=S, H=H,

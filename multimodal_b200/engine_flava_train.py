@@ -88,8 +88,6 @@ class FlavaTrainStack:
         d, ln, pfx = self.d, self.layernorm, self.prefix
         M = B * S
         f32 = torch.float32
-        if kmask is not None and S > 256:
-            raise MMBError("training with a key-padding mask is implemented for sequence lengths <= 256")
         XM, Y = self.stack.forward(X0, B, S, True, kmask=kmask, save=save)
         XF = torch.empty((M, d), device=self.device, dtype=f32)
         LAST = torch.empty((M, d), device=self.device, dtype=f32)

@@ -78,7 +78,7 @@ def _bool_mask_u8(mask: Optional[torch.Tensor], B: int, S: int, what: str) -> Op
 def _attention(rt: _Rt, QKV: torch.Tensor, O: torch.Tensor, B: int, S: int, H: int, hd: int, mask_u8, causal: bool):
     d = H * hd
     scale = 1.0 / math.sqrt(hd)
-    if mask_u8 is None and hd == 64 and S <= 384:
+    if mask_u8 is None and hd == 64 and (S <= 384 or S > ops.GENERIC_FWD_MAX_S):
         ops.attention_fwd(QKV, O, None, B, S, H, causal, scale)
     else:
         ops.attention_fwd_generic(QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], O, B=B, Sq=S, Skv=S, H=H, head_dim=hd,

@@ -430,6 +430,12 @@ def coca_text_embed_fwd(ids, emb, cls, pos, x, B, S, d, V):
                "mmb_coca_text_embed_fwd")
 
 
+# Longest self-attention (Sq = Skv) the generic forward takes at head_dim 64: its Q, K and V tiles (144 B per row, keys
+# padded to 64) must fit in the 227 KB of shared memory an H100 CTA can opt into.  Longer unmasked head_dim-64
+# self-attention goes to attention_fwd, which streams K / V.
+GENERIC_FWD_MAX_S = 512
+
+
 def attention_fwd_generic(q, k, v, out, *, B, Sq, Skv, H, head_dim, bsq, bsk, bsv, bso, scale, mask=None, mask_bs=0,
                           mask_qs=0, causal=False):
     """q/k/v/out: 2-D bf16 views [rows, >= H*head_dim] (row-major, possibly column slices of a wider matrix)."""
@@ -455,6 +461,7 @@ def attention_bwd_kmask(qkv, out, dout, lse, dqkv, kmask, B, S, H, causal, scale
     with _timed("attn_bwd", 10.0 * S * S * 64 * H * B, "F"):
         _lib.check(_lib.lib().mmb_attention_bwd_kmask(_p(qkv), _p(out), _p(dout), _p(lse), _p(dqkv), _p(kmask), B, S, H, 64,
                                                       int(causal), float(scale), _stream()), "mmb_attention_bwd_kmask")
+        _lib.LAUNCHES += _lib.lib().mmb_attention_bwd_launches(S) - 1
 
 
 def bert_embed_ln_bwd(ids, type_ids, word, pos, type_emb, gamma, dy, dword, dpos, dtype_emb, dgamma, dbeta, B, S, d, V, eps):

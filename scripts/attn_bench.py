@@ -1,5 +1,9 @@
 """Times the fused self-attention kernels (mmb_attention_fwd / mmb_attention_bwd) at the shapes of the CLIP training
-steps: ViT-B/16 image tower (S = 197), its causal text tower (S = 77) and the ViT-L/14 image tower (S = 257).
+steps: ViT-B/16 image tower (S = 197), its causal text tower (S = 77) and the ViT-L/14 image tower (S = 257), and at
+the lengths served by the streamed kernels (S > 384): ViT-L/14@336 (577), 512-token text, FLAVA's multimodal encoder
+(710), S = 4096, and the 384 / 385 boundary between the resident and the streamed kernels.  For the streamed rows the
+same bf16 operands also go through torch's scaled_dot_product_attention (flash backend), forward and backward, as a
+reference point from the same run.
 
     python scripts/attn_bench.py [--min-seconds 0.5] [--json OUT]
 
@@ -28,7 +32,15 @@ SHAPES = [
     ("b16 image", 512, 197, 12, False),
     ("b16 text (causal)", 512, 77, 12, True),
     ("l14 image", 256, 257, 16, False),
+    ("l14@336", 64, 577, 16, False),
+    ("text 512", 64, 512, 12, False),
+    ("flava mm", 32, 710, 12, False),
+    ("long", 4, 4096, 16, False),
+    ("long (causal)", 4, 4096, 16, True),
+    ("boundary", 128, 384, 12, False),
+    ("boundary", 128, 385, 12, False),
 ]
+STREAMED_MIN_S = 385   # longer sequences take the streamed kernels
 FWD_BYTES, BWD_BYTES = 516, 1028   # per token and head
 
 
@@ -54,6 +66,27 @@ def time_fn(fn, min_seconds):
         if total >= min_seconds:
             return total / n
         n = max(2 * n, int(n * 1.2 * min_seconds / max(total, 1e-6)))
+
+
+def sdpa_fns(qkv, dout, B, S, H, causal):
+    """forward and backward of F.scaled_dot_product_attention (flash backend) on the same bf16 operands"""
+    from torch.nn.attention import SDPBackend, sdpa_kernel
+
+    q, k, v = (t.detach().requires_grad_(True) for t in qkv.view(B, S, 3, H, 64).permute(2, 0, 3, 1, 4))
+    do = dout.view(B, S, H, 64).transpose(1, 2)
+    F = torch.nn.functional
+
+    def fwd():
+        with sdpa_kernel(SDPBackend.FLASH_ATTENTION), torch.no_grad():
+            F.scaled_dot_product_attention(q, k, v, is_causal=causal, scale=0.125)
+
+    with sdpa_kernel(SDPBackend.FLASH_ATTENTION):
+        o = F.scaled_dot_product_attention(q, k, v, is_causal=causal, scale=0.125)
+
+    def bwd():
+        torch.autograd.grad(o, (q, k, v), do, retain_graph=True)
+
+    return fwd, bwd
 
 
 def main():
@@ -88,7 +121,20 @@ def main():
             r = rows[-1]
             print(f"{name:20s} {B:4d} {S:4d} {H:3d} {direction:>4s} {r['ms']:8.3f} {r['tflops']:8.1f} {r['gbps']:7.0f} "
                   f"{floor_ms:7.3f}ms")
+        if S >= STREAMED_MIN_S:
+            sfwd, sbwd = sdpa_fns(qkv, dout, B, S, H, causal)
+            for direction, fn, f in (("fwd", sfwd, flop), ("bwd", sbwd, 2.5 * flop)):
+                t = time_fn(fn, args.min_seconds)
+                rows.append({"shape": name + " sdpa-flash", "B": B, "S": S, "H": H, "causal": causal, "dir": direction,
+                             "ms": t * 1e3, "tflops": f / t / 1e12})
+                print(f"{'  torch sdpa flash':20s} {B:4d} {S:4d} {H:3d} {direction:>4s} {t * 1e3:8.3f} {f / t / 1e12:8.1f}")
+            del sfwd, sbwd
         del qkv, out, lse, dout, dqkv
+    rate = {(r["shape"], r["dir"]): r["tflops"] for r in rows}
+    for direction in ("fwd", "bwd"):
+        a, b = rate[("l14@336", direction)], rate[("l14 image", direction)]
+        print(f"{direction}: streamed S = 577 {a:.1f} TFLOP/s vs resident S = 257 {b:.1f} TFLOP/s "
+              f"({'at least' if a >= b else 'BELOW'} the resident rate)")
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"card": card(), "rows": rows}, f, indent=1)
