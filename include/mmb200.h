@@ -254,21 +254,33 @@ int mmb_coca_text_embed_fwd(const long long* ids, const float* emb, const float*
  * F.scaled_dot_product_attention at modules/layers/multi_head_attention.py:74-76,171-173.  q,k,v,out are bf16 with row
  * strides ld* and batch strides bs* (elements, multiples of 8; bsq = 0 shares the queries across the batch); head h
  * occupies columns [h*head_dim, (h+1)*head_dim).  mask (optional, uint8, 1 = attend) is addressed
- * mask[b*mask_bs + i*mask_qs + j] (mask_qs = 0: key-padding mask).  causal follows SDPA's is_causal (j <= i). */
+ * mask[b*mask_bs + i*mask_qs + j] (mask_qs = 0: key-padding mask).  causal follows SDPA's is_causal (j <= i).
+ * Any Sq and Skv.  Shapes whose Q, K and V of one head fit in a CTA's shared memory,
+ * (pad16(Sq) + 2*pad64(Skv)) * (2*head_dim + 16) <= 227 KB, run a kernel that keeps the head resident; longer ones run
+ * tensor-core kernels that stream K / V through shared memory (mmb_attention_generic_streamed tells which).  A query
+ * row with no visible key gets O = 0.  On the streamed path B and H are at most 65535 (MMB_ERR_UNSUPPORTED beyond) and
+ * q, k, v and out must be 16-byte aligned (MMB_ERR_ARG otherwise). */
 int mmb_attention_fwd_generic(const void* q, long long ldq, long long bsq, const void* k, long long ldk, long long bsk,
                               const void* v, long long ldv, long long bsv, void* out, long long ldo, long long bso,
                               const void* mask, long long mask_bs, long long mask_qs, int B, int Sq, int Skv, int H,
                               int head_dim, int causal, float scale, void* stream);
-/* Backward of mmb_attention_fwd_generic (same addressing; SIMT, fp32 arithmetic — these layers are ~3 % of CoCa's FLOPs).
- * dq / dk / dv (bf16) use the strides of q / k / v; dq_bf16 may be NULL.  dq_f32 (optional, fp32 [Sq, ldq32], accumulated
- * with atomics: zero it first) receives the gradient of batch-shared queries (bsq = 0) summed over the batch.
- * scratch: fp32 [2 * B * H * Sq] (row LSE and rowsum(P * dP)).  Autograd of F.scaled_dot_product_attention at
- * modules/layers/multi_head_attention.py:74-76,171-173 for the CoCa poolers / decoders. */
+/* Backward of mmb_attention_fwd_generic (same addressing, any Sq and Skv).  The shapes the resident forward serves run
+ * SIMT kernels in fp32 arithmetic; longer ones run the streamed tensor-core kernels (two launches, a third for dq_f32),
+ * so a forward and its backward always take the same path.  dq / dk / dv (bf16) use the strides of q / k / v; dq_bf16
+ * may be NULL; on the streamed path dq / dk / dv must be 16-byte aligned (MMB_ERR_ARG otherwise).  dq_f32 (optional, fp32 [Sq, ldq32], += : zero it first) receives the gradient of batch-shared queries
+ * (bsq = 0) summed over the batch: with fp32 atomics on the resident path, and run-to-run deterministic on the streamed
+ * path (per-batch-chunk sums in library scratch, chunks sized from the shape alone, added in a fixed order).  A masked
+ * key gets zero dK / dV rows and a query row with no visible key a zero dQ row.  scratch: fp32 [2 * B * H * Sq] (row
+ * LSE and rowsum(P * dP)).  Autograd of F.scaled_dot_product_attention at
+ * modules/layers/multi_head_attention.py:74-76,171-173 for the CoCa poolers / decoders and the standalone layers. */
 int mmb_attention_bwd_generic(const void* q, long long ldq, long long bsq, const void* k, long long ldk, long long bsk,
                               const void* v, long long ldv, long long bsv, const void* dout, long long ldo, long long bso,
                               const void* mask, long long mask_bs, long long mask_qs, void* dq_bf16, float* dq_f32,
                               long long ldq32, void* dk_bf16, void* dv_bf16, float* scratch, int B, int Sq, int Skv, int H,
                               int head_dim, int causal, float scale, void* stream);
+/* 1 when mmb_attention_fwd_generic / mmb_attention_bwd_generic run the streamed kernels for this shape (the head does not
+ * fit in shared memory), 0 when they run the resident forward and SIMT backward or head_dim is unsupported.  Host only. */
+int mmb_attention_generic_streamed(int Sq, int Skv, int head_dim);
 /* accum[0] += sum_i CE(logits[i,:], labels[i*label_stride]) over rows with label != ignore_index; accum[1] += #rows
  * — nn.CrossEntropyLoss(ignore_index=pad_idx), models/coca/coca_model.py:425,447-450 (forward). */
 int mmb_ce_labels(const float* logits, long long ld, const long long* labels, long long label_stride,

@@ -2,6 +2,8 @@
 // cross-attention (separate Q and K/V sources, Sq != Skv), head_dim 64 / 96 / 128, batch-shared queries (learned
 // pooler queries), arbitrary boolean masks.  One CTA per (batch, head); K and V of the head stay in shared memory,
 // each warp owns 16 query rows and runs an online-softmax sweep over 64-key blocks on warp-level tensor-core MMAs.
+// Shapes whose head does not fit (generic_resident_fits() in attention_generic.cuh) go to the K / V-streamed kernels
+// of attention_generic_stream.cu.
 //
 // Serves CoCa (SURVEY.md §8 a14): AttentionPooler / CascadedAttentionPooler (modules/layers/attention_pooler.py:16-101,
 // head_dim 96 for ViT-L/14), the text decoder's [causal x padding] mask with its CLS row (models/coca/text_decoder.py
@@ -11,7 +13,7 @@
 //
 // Math: softmax(Q K^T * scale + mask) V with fp32 statistics, P rounded to bf16 for the PV product.  A fully masked
 // query row yields zeros (SDPA would yield NaN; no caller on this path produces such a row).
-#include "common.cuh"
+#include "attention_generic.cuh"
 #include "mmb200_internal.h"
 
 namespace mmb {
@@ -44,17 +46,6 @@ __device__ __forceinline__ float quad_sum(float v) {
 }
 
 }  // namespace ag
-
-struct AttnGenArgs {
-  const __nv_bfloat16 *q, *k, *v;
-  __nv_bfloat16* out;
-  long long ldq, ldk, ldv, ldo;          // row strides (elements)
-  long long bsq, bsk, bsv, bso;          // batch strides (elements); bsq = 0: queries shared by the whole batch
-  const uint8_t* mask;                   // optional, 1 = attend
-  long long mask_bs, mask_qs;            // mask[b*mask_bs + i*mask_qs + j]; mask_qs = 0: key mask [B, Skv]
-  int Sq, Skv, H, causal;
-  float scale_log2;
-};
 
 // Row pitch D*2 + 16 bytes: an odd number of 16-byte chunks, so the 8 rows of an ldmatrix phase hit 8 distinct bank
 // groups without a swizzle.
@@ -199,8 +190,7 @@ __global__ void __launch_bounds__(256) attn_fwd_generic_kernel(const AttnGenArgs
 template <int D>
 static int launch_generic(const AttnGenArgs& a, int B, cudaStream_t st) {
   const int Sq_pad = (a.Sq + 15) & ~15, Skv_pad = (a.Skv + 63) & ~63;
-  const int smem = (Sq_pad + 2 * Skv_pad) * (D * 2 + 16);
-  if (smem > 227 * 1024) return MMB_ERR_UNSUPPORTED;
+  const int smem = (Sq_pad + 2 * Skv_pad) * (D * 2 + 16);   // callers check generic_resident_fits()
   int warps = Sq_pad / 16;
   warps = warps < 1 ? 1 : (warps > 8 ? 8 : warps);
   cudaFuncSetAttribute(attn_fwd_generic_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -291,12 +281,19 @@ extern "C" int mmb_attention_fwd_generic(const void* q, long long ldq, long long
   a.Sq = Sq; a.Skv = Skv; a.H = H; a.causal = causal;
   a.scale_log2 = scale * 1.4426950408889634f;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (head_dim != 64 && head_dim != 96 && head_dim != 128) return MMB_ERR_UNSUPPORTED;
+  if (!generic_resident_fits(Sq, Skv, head_dim)) return attention_fwd_gstream(a, B, head_dim, st);
   switch (head_dim) {
     case 64: return launch_generic<64>(a, B, st);
     case 96: return launch_generic<96>(a, B, st);
-    case 128: return launch_generic<128>(a, B, st);
-    default: return MMB_ERR_UNSUPPORTED;
+    default: return launch_generic<128>(a, B, st);
   }
+}
+
+// 1 when the generic entry points run the streamed kernels (attention_generic_stream.cu) for this shape, else 0
+extern "C" int mmb_attention_generic_streamed(int Sq, int Skv, int head_dim) {
+  if (Sq <= 0 || Skv <= 0 || (head_dim != 64 && head_dim != 96 && head_dim != 128)) return 0;
+  return generic_resident_fits(Sq, Skv, head_dim) ? 0 : 1;
 }
 
 // probs fp32 [B, H, S, S] from the packed QKV [B*S, 3*H*64] and the forward's row LSE [B, H, S] (head_dim 64).

@@ -17,24 +17,10 @@
 // difference is below the bf16 noise of the operands).  A fully masked query row has p = 0 everywhere (as the forward).
 #include <cstdlib>
 
-#include "common.cuh"
+#include "attention_generic.cuh"
 #include "mmb200_internal.h"
 
 namespace mmb {
-
-struct AttnGenBwdArgs {
-  const __nv_bfloat16 *q, *k, *v, *dout;
-  long long ldq, ldk, ldv, ldo;          // row strides (elements)
-  long long bsq, bsk, bsv, bso;          // batch strides (elements); bsq = 0: queries shared by the whole batch
-  const uint8_t* mask;                   // optional, 1 = attend: mask[b*mask_bs + i*mask_qs + j]
-  long long mask_bs, mask_qs;
-  __nv_bfloat16 *dq, *dk, *dv;           // bf16 outputs with the strides of q / k / v (dq may be NULL)
-  float* dq_f32;                         // optional fp32 [Sq, ldq32] (+= with atomics): batch-shared queries
-  long long ldq32;
-  float *lse, *dsum;                     // scratch [B, H, Sq]: row LSE (log2 units) and D_i
-  int B, Sq, Skv, H, causal;
-  float scale, scale_log2;
-};
 
 __device__ __forceinline__ float wred_sum(float v) {
 #pragma unroll
@@ -474,10 +460,12 @@ extern "C" int mmb_attention_bwd_generic(const void* q, long long ldq, long long
   a.B = B; a.Sq = Sq; a.Skv = Skv; a.H = H; a.causal = causal;
   a.scale = scale; a.scale_log2 = scale * 1.4426950408889634f;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (head_dim != 64 && head_dim != 96 && head_dim != 128) return MMB_ERR_UNSUPPORTED;
+  // the shapes the resident forward serves keep the SIMT kernels; every longer one runs the streamed backward
+  if (!generic_resident_fits(Sq, Skv, head_dim)) return attention_bwd_gstream(a, head_dim, st);
   switch (head_dim) {
     case 64: return launch_gen_bwd<64>(a, st);
     case 96: return launch_gen_bwd<96>(a, st);
-    case 128: return launch_gen_bwd<128>(a, st);
-    default: return MMB_ERR_UNSUPPORTED;
+    default: return launch_gen_bwd<128>(a, st);
   }
 }

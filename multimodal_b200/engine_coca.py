@@ -9,7 +9,8 @@ One generic pre-norm layer runner serves the TorchMultimodal `TransformerEncoder
 
 Attention routing: unmasked / causal self-attention with head_dim 64 runs on the tensor-core attention kernel (attention.cu);
 anything else — cross-attention, the pooler's head_dim 96, the text decoder's [causal x padding] mask — on the general
-kernel (attention_generic.cu).  Reference call stacks: models/coca/coca_model.py:69-130, models/coca/text_decoder.py
+kernels (attention_generic.cu while a head fits in shared memory, attention_generic_stream.cu at any longer length, e.g.
+the pooler over the 576 image tokens of a 336-px ViT-L/14).  Reference call stacks: models/coca/coca_model.py:69-130, models/coca/text_decoder.py
 :141-203, models/coca/multimodal_decoder.py:86-108, modules/layers/attention_pooler.py:48-101,
 modules/encoders/vision_transformer.py:56-89, modules/layers/patch_embedding.py:104-154.
 """

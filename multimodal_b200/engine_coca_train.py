@@ -7,12 +7,14 @@ All layer stacks run on ``engine.TransformerStack`` (the CLIP towers' fused sche
   vision encoder      : packed `input_proj` self-attention (tensor-core fwd / bwd), erf-GELU MLP, optional final LayerNorm
                         (modules/encoders/vision_transformer.py:56-89, patch_embedding.py:104-154)
   text decoder        : separate q / k / v projections presented as one packed operand, the [B, S, S] causal x padding
-                        mask on the general attention kernels (fwd: mma.sync, bwd: SIMT), CLS row -> ln_final -> projection
+                        mask on the general attention kernels (fwd: mma.sync; bwd: SIMT while a head fits in shared
+                        memory, K / V-streamed tensor cores at longer lengths), CLS row -> ln_final -> projection
                         (models/coca/text_decoder.py:141-203)
   multimodal decoder  : causal self-attention (tensor cores) + cross-attention to the pooled image tokens (general kernels) +
                         MLP per layer, final LayerNorm (models/coca/multimodal_decoder.py:86-108)
-  attention pooler    : LayerNorm-ed keys / values, batch-shared learned queries (their gradient is summed over the batch
-                        with fp32 atomics), ln_post (modules/layers/attention_pooler.py:48-72)
+  attention pooler    : LayerNorm-ed keys / values, batch-shared learned queries (their gradient is summed over the batch:
+                        fp32 atomics on the resident path, fixed-order per-chunk sums on the streamed one, e.g. 576 image
+                        tokens at 336 px), ln_post (modules/layers/attention_pooler.py:48-72)
   vocabulary head     : Linear -> CrossEntropy(ignore_index) with materialised fp32 logits in training (the forward-only
                         path keeps the fused statistics GEMM), backward = d logits kernel + two GEMMs
 Every training forward keeps its activations in its own Workspace (held by the autograd node).

@@ -12,7 +12,8 @@ tensor-core attention, the add+LayerNorm kernel); nothing is computed by PyTorch
 forward / backward schedule); the other standalone modules compute forward values only, and asking them for an autograd
 graph raises instead of returning detached tensors.
 Shape limits are those of the kernels: head_dim 64 (fused attention; 96 / 128 and arbitrary boolean masks go through
-the general kernel), feature sizes multiples of 8, 3-channel images.
+the general kernels), feature sizes multiples of 8, 3-channel images.  Any sequence length: the general kernels keep a
+head resident in shared memory while it fits and stream K / V through it beyond (attention_generic_stream.cu).
 """
 from __future__ import annotations
 

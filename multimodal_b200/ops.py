@@ -430,9 +430,10 @@ def coca_text_embed_fwd(ids, emb, cls, pos, x, B, S, d, V):
                "mmb_coca_text_embed_fwd")
 
 
-# Longest self-attention (Sq = Skv) the generic forward takes at head_dim 64: its Q, K and V tiles (144 B per row, keys
-# padded to 64) must fit in the 227 KB of shared memory an H100 CTA can opt into.  Longer unmasked head_dim-64
-# self-attention goes to attention_fwd, which streams K / V.
+# Longest self-attention (Sq = Skv) the generic forward keeps resident at head_dim 64: its Q, K and V tiles (144 B per
+# row, keys padded to 64) fit in the 227 KB of shared memory an H100 CTA can opt into.  Longer shapes run the generic
+# entry points' K / V-streamed kernels (any length); unmasked head_dim-64 self-attention above this length goes to
+# attention_fwd instead, whose streamed kernel is the same one the CLIP towers use.
 GENERIC_FWD_MAX_S = 512
 
 
