@@ -281,6 +281,29 @@ int mmb_attention_bwd_generic(const void* q, long long ldq, long long bsq, const
 /* 1 when mmb_attention_fwd_generic / mmb_attention_bwd_generic run the streamed kernels for this shape (the head does not
  * fit in shared memory), 0 when they run the resident forward and SIMT backward or head_dim is unsupported.  Host only. */
 int mmb_attention_generic_streamed(int Sq, int Skv, int head_dim);
+/* Decode attention: mmb_attention_fwd_generic's arguments and result for Sq <= 16 query rows over any number of keys
+ * (the autoregressive step of MultiHeadAttentionWithCache with a key / value cache,
+ * modules/layers/multi_head_attention.py:152-175).  The keys are split across CTAs (grid splits x H x B,
+ * mmb_attention_decode_splits) and the splits' fp32 partials are added in split order by a second kernel, so the result
+ * is run-to-run deterministic.  A query row with no visible key gets O = 0.  MMB_ERR_UNSUPPORTED when Sq > 16, head_dim
+ * is not 64, 96 or 128, or B / H exceed 65535; MMB_ERR_ARG when q, k, v or out is not 16-byte aligned or a stride is not
+ * a multiple of 8 elements. */
+int mmb_attention_fwd_decode(const void* q, long long ldq, long long bsq, const void* k, long long ldk, long long bsk,
+                             const void* v, long long ldv, long long bsv, void* out, long long ldo, long long bso,
+                             const void* mask, long long mask_bs, long long mask_qs, int B, int Sq, int Skv, int H,
+                             int head_dim, int causal, float scale, void* stream);
+/* Number of key splits mmb_attention_fwd_decode uses for (B, H, Skv): a function of its arguments alone (at least 4
+ * key blocks of 64 per split, about 264 CTAs, at most 64 splits), >= 1.  Host only. */
+int mmb_attention_decode_splits(int B, int H, int Skv);
+/* Key / value cache concatenation, torch.cat([past, new], dim=2) of MultiHeadAttentionWithCache
+ * (modules/layers/multi_head_attention.py:163-166): past [B, H, Sp, head_dim] (fp32 when past_f32, else bf16; element
+ * strides past_bs / past_hs / past_ss, unit stride along head_dim; may be NULL when Sp = 0) and the new projection rows
+ * new_rows bf16 [B*Sn, >= H*head_dim] (row stride ld_new) are written as one row-major [B, Sp + Sn, H*head_dim] buffer:
+ * out in fp32 (out_f32) or bf16, and / or out_bf16, a bf16 copy (the attention operand when out is fp32).  Either
+ * output may be NULL, not both. */
+int mmb_kv_cache_append(const void* past, int past_f32, long long past_bs, long long past_hs, long long past_ss,
+                        const void* new_rows, long long ld_new, void* out, int out_f32, void* out_bf16, int B, int H,
+                        int Sp, int Sn, int head_dim, void* stream);
 /* accum[0] += sum_i CE(logits[i,:], labels[i*label_stride]) over rows with label != ignore_index; accum[1] += #rows
  * — nn.CrossEntropyLoss(ignore_index=pad_idx), models/coca/coca_model.py:425,447-450 (forward). */
 int mmb_ce_labels(const float* logits, long long ld, const long long* labels, long long label_stride,

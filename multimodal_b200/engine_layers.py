@@ -11,9 +11,14 @@ tensor-core attention, the add+LayerNorm kernel); nothing is computed by PyTorch
 `TransformerEncoder` also train on their own (grad mode on: `engine_coca_train.LayersTrainRuntime`, the CLIP towers' fused
 forward / backward schedule); the other standalone modules compute forward values only, and asking them for an autograd
 graph raises instead of returning detached tensors.
+  modules/layers/multi_head_attention.py:83-180  MultiHeadAttentionWithCache (key / value cache, cross-attention)
+  modules/layers/transformer.py:262-657          TransformerDecoderLayer (pre- and post-norm), TransformerDecoder
+
 Shape limits are those of the kernels: head_dim 64 (fused attention; 96 / 128 and arbitrary boolean masks go through
 the general kernels), feature sizes multiples of 8, 3-channel images.  Any sequence length: the general kernels keep a
 head resident in shared memory while it fits and stream K / V through it beyond (attention_generic_stream.cu).
+Autoregressive decoding (queries of at most 16 rows over a key / value cache) runs the split-KV decode kernel
+(attention_decode.cu); the decoders compute forward values only (their training runs inside the CoCa runtimes).
 """
 from __future__ import annotations
 
@@ -265,3 +270,266 @@ def patch_embeddings_forward(mod: nn.Module, image: torch.Tensor, image_patches_
     ops.vit_assemble_fwd(PO, mod.cls_token if mod.include_cls_embed else None, mod.position_embeddings,
                          mod.mask_token if pm is not None else None, pm, X, B, S, d)
     return PatchEmbeddingsOutput(embeddings=X.view(B, S, d).to(image.dtype))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Decoding with a key / value cache: MultiHeadAttentionWithCache, TransformerDecoderLayer, TransformerDecoder
+# (modules/layers/multi_head_attention.py:83-180, transformer.py:262-657)
+#
+# A returned cache tensor has the reference's shape [B, H, S, hd]; it is the transposed view of a fresh row-major
+# [B, S, H*hd] buffer (the view the reference itself returns on a call without a past), so the attention kernels read it
+# with row stride H*hd.  A past in any layout is concatenated with the new projection rows by the append kernel, which
+# also writes the bf16 operand copy when the cache is fp32.  Queries of at most ops.DECODE_MAX_SQ rows run the split-KV
+# decode kernel where it is the faster one (ops.decode_attention_wins), the others the general attention kernels.
+# ---------------------------------------------------------------------------------------------------------------------
+def _rect_mask_u8(mask: Optional[torch.Tensor], B: int, Sq: int, Skv: int, what: str):
+    """bool [Sq, Skv], [B|1, Sq|1, Skv] or [B|1, 1, Sq|1, Skv] (True = attend) -> (uint8 mask, mask_bs, mask_qs): the
+    broadcast dimensions get stride 0.  Float (additive) and per-head masks are not supported."""
+    if mask is None:
+        return None, 0, 0
+    if mask.dtype != torch.bool:
+        raise NotImplementedError(f"{what}: only boolean attention masks (True = attend) are on the accelerated path")
+    if mask.dim() == 4:
+        if mask.shape[1] != 1:
+            raise NotImplementedError(f"{what}: per-head masks are not on the accelerated path (the head dim must be 1)")
+        mask = mask[:, 0]
+    if mask.dim() == 2:
+        mask = mask[None]
+    if mask.dim() != 3 or mask.shape[0] not in (1, B) or mask.shape[1] not in (1, Sq) or mask.shape[2] != Skv:
+        raise ValueError(f"{what}: attention mask shape {tuple(mask.shape)} does not broadcast to [{B}, {Sq}, {Skv}]")
+    Bm, Qm = mask.shape[0], mask.shape[1]
+    u8 = mask.to(torch.uint8).contiguous()
+    return u8, (0 if Bm == 1 else Qm * Skv), (0 if Qm == 1 else Skv)
+
+
+def _attend(q, k, v, O, B, Sq, Skv, H, hd, bsq, bsk, bsv, mask, causal):
+    """O [B*Sq, H*hd] = attention of 2-D bf16 views (row-major, batch strides bs*); mask = (u8, mask_bs, mask_qs)."""
+    fn = ops.attention_fwd_decode if ops.decode_attention_wins(B, H, Sq, Skv) else ops.attention_fwd_generic
+    fn(q, k, v, O, B=B, Sq=Sq, Skv=Skv, H=H, head_dim=hd, bsq=bsq, bsk=bsk, bsv=bsv, bso=Sq * H * hd,
+       scale=1.0 / math.sqrt(hd), mask=mask[0], mask_bs=mask[1], mask_qs=mask[2], causal=causal)
+
+
+def _cache_dtype(past: Optional[torch.Tensor], new_dtype: torch.dtype) -> torch.dtype:
+    dt = new_dtype if past is None else torch.promote_types(past.dtype, new_dtype)   # torch.cat's promotion
+    if dt not in (torch.float32, torch.bfloat16):
+        raise MMBError(f"MultiHeadAttentionWithCache: key / value cache dtype {dt} is not supported (fp32 / bf16)")
+    return dt
+
+
+def _mha_cache(mod: nn.Module, rt: _Rt, tag: str, Xq, Xk, Xv, B: int, Sq: int, Sk: int, mask, causal: bool,
+               past, use_cache: bool, kv_dtypes, out_epi: int):
+    """MultiHeadAttentionWithCache on bf16 input rows Xq [B*Sq, dim_q] and Xk / Xv [B*Sk, dim_kv] (`Xk is Xv`: one
+    packed K|V GEMM; `Xq is Xk is Xv`: one packed Q|K|V GEMM).  Returns (output-projection rows [B*Sq, d] in fp32
+    (out_epi = EPI_F32) or bf16, (K, V) caches [B, H, S, hd] or None)."""
+    ws, sh = rt.ws, rt.sh
+    d = mod.q_proj.weight.shape[0]
+    H = mod.num_heads
+    hd = d // H
+    if d % H or hd not in (64, 96, 128):
+        raise MMBError(f"MultiHeadAttentionWithCache: head_dim {d / H:g} is not supported by the attention kernels "
+                       "(64 / 96 / 128)")
+    bf = torch.bfloat16
+    qp, kp, vp = mod.q_proj, mod.k_proj, mod.v_proj
+    has_bias = qp.bias is not None
+
+    def bias(key, parts):
+        return sh.cat_f32(key, [p.bias for p in parts]) if has_bias else None
+
+    if Xq is Xk and Xk is Xv:
+        QKV = ws.get(tag + ".QKV", (B * Sq, 3 * d), bf)
+        ops.gemm(Xq, sh.get("wqkv", [qp.weight, kp.weight, vp.weight]), bias=bias("bqkv", (qp, kp, vp)), out=QKV)
+        Q, K, V, ldkv = QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], 3 * d
+    else:
+        Q = ws.get(tag + ".Q", (B * Sq, d), bf)
+        ops.gemm(Xq, sh.get("wq", [qp.weight]), bias=qp.bias, out=Q)
+        if Xk is Xv:
+            KV = ws.get(tag + ".KV", (B * Sk, 2 * d), bf)
+            ops.gemm(Xk, sh.get("wkv", [kp.weight, vp.weight]), bias=bias("bkv", (kp, vp)), out=KV)
+            K, V, ldkv = KV[:, :d], KV[:, d:], 2 * d
+        else:
+            K, V = ws.get(tag + ".K", (B * Sk, d), bf), ws.get(tag + ".V", (B * Sk, d), bf)
+            ops.gemm(Xk, sh.get("wk", [kp.weight]), bias=kp.bias, out=K)
+            ops.gemm(Xv, sh.get("wv", [vp.weight]), bias=vp.bias, out=V)
+            ldkv = d
+    Sp = 0 if past is None else past[0].shape[2]
+    St = Sp + Sk
+    caches = None
+    bsk = bsv = Sk * ldkv
+    if past is not None or use_cache:
+        caches = []
+        ops_kv = []
+        for i, (new, p) in enumerate(((K, None if past is None else past[0]), (V, None if past is None else past[1]))):
+            if p is not None and (p.dim() != 4 or tuple(p.shape[:2]) != (B, H) or p.shape[3] != hd or p.shape[2] != Sp):
+                raise ValueError(f"MultiHeadAttentionWithCache: past key / value of shape {tuple(p.shape)}, expected "
+                                 f"[{B}, {H}, S, {hd}] with the same S for both")
+            dt = _cache_dtype(p, kv_dtypes[i])
+            buf = torch.empty((B, St, d), device=Xq.device, dtype=dt) if use_cache else None
+            opnd = buf if dt == bf and buf is not None else ws.get(f"{tag}.C{i}", (B, St, d), bf)
+            ops.kv_cache_append(p, new, buf, None if opnd is buf else opnd, B=B, H=H, Sp=Sp, Sn=Sk, head_dim=hd)
+            ops_kv.append(opnd.view(B * St, d))
+            if use_cache:
+                caches.append(buf.view(B, St, H, hd).transpose(1, 2))
+        K, V = ops_kv
+        bsk = bsv = St * d
+    O = ws.get(tag + ".O", (B * Sq, d), bf)
+    _attend(Q, K, V, O, B, Sq, St, H, hd, Sq * Q.stride(0), bsk, bsv, mask, causal)
+    odt = torch.float32 if out_epi == ops.EPI_F32 else bf
+    Y = torch.empty((B * Sq, d), device=Xq.device, dtype=odt) if odt == torch.float32 else ws.get(tag + ".Y", (B * Sq, d), bf)
+    ops.gemm(O, sh.get("wo", [mod.output_proj.weight]), bias=mod.output_proj.bias, epilogue=out_epi, out=Y)
+    return Y, (tuple(caches) if use_cache else None)
+
+
+def _check_training_dropout(mod: nn.Module, what: str) -> None:
+    if mod.training and mod.dropout > 0:
+        raise NotImplementedError(f"{what}: dropout > 0 in training mode is not on the accelerated path")
+
+
+def mha_cache_forward(mod: nn.Module, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
+                      attn_mask: Optional[torch.Tensor] = None, past_key_value=None, is_causal: bool = False,
+                      use_cache: bool = False):
+    """MultiHeadAttentionWithCache.forward (multi_head_attention.py:116-180): projections (packed when the inputs are
+    the same tensor) -> cache append -> decode / general attention -> output projection."""
+    from .modules.layers.multi_head_attention import MHAWithCacheOutput
+
+    forward_only_guard(mod, "MultiHeadAttentionWithCache")
+    _check_training_dropout(mod, "MultiHeadAttentionWithCache")
+    for t, n in ((query, "query"), (key, "key"), (value, "value")):
+        _cuda(t, f"MultiHeadAttentionWithCache {n}")
+    B, Sq, _ = query.shape
+    if key.size(0) != B or value.size(0) != B:
+        raise ValueError("key and value should have the same bsz as query.")
+    Sk = key.shape[1]
+    if value.shape[1] != Sk:
+        raise ValueError(f"MultiHeadAttentionWithCache: key and value lengths differ ({Sk} vs {value.shape[1]})")
+    rt = _rt(mod, query.device)
+    Xq = _to_bf16_rows(rt, query, "mhc.Xq")
+    Xk = Xq if key is query else _to_bf16_rows(rt, key, "mhc.Xk")
+    Xv = Xk if value is key else _to_bf16_rows(rt, value, "mhc.Xv")
+    Sp = 0 if past_key_value is None else past_key_value[0].shape[2]
+    mask = _rect_mask_u8(attn_mask, B, Sq, Sp + Sk, "MultiHeadAttentionWithCache")
+    Y, cache = _mha_cache(mod, rt, "mhc", Xq, Xk, Xv, B, Sq, Sk, mask, bool(is_causal), past_key_value, use_cache,
+                          (key.dtype, value.dtype), ops.EPI_F32)
+    out = Y.view(B, Sq, -1).to(query.dtype)
+    return MHAWithCacheOutput(out, cache) if use_cache else out
+
+
+def _decoder_layer(mod: nn.Module, X: torch.Tensor, B: int, S: int, ENC: Optional[torch.Tensor], S_enc: int,
+                   mask, cross_mask, past, use_cache: bool, kv_dtype: torch.dtype):
+    """One TransformerDecoderLayer on fp32 rows X [B*S, d] (ENC: bf16 rows [B*S_enc, dim_kv] or None).  Returns fresh
+    fp32 output rows and the self-attention cache."""
+    rt = _rt(mod, X.device)
+    ws, sh = rt.ws, rt.sh
+    M, d = X.shape
+    bf, f32 = torch.bfloat16, torch.float32
+    mlp = mod.feedforward.model
+    act = _act_code(mlp[1])
+    ff = mlp[0].weight.shape[0]
+    LN, PRE, HACT = ws.get("d.LN", (M, d), bf), ws.get("d.PRE", (M, ff), bf), ws.get("d.HACT", (M, ff), bf)
+    w1, w2 = sh.get("w1", [mlp[0].weight]), sh.get("w2", [mlp[-1].weight])
+    ln1, ln2 = mod.attention_layernorm, mod.feedforward_layernorm
+    cross = mod.use_cross_attention and (ENC is not None or not mod.norm_first)
+    if cross and ENC is None:
+        raise ValueError("encoder_hidden_states must be provided for cross attention")
+    lnc = mod.cross_attention_layernorm if cross else None
+    out = torch.empty((M, d), device=X.device, dtype=f32)
+    kvd = (kv_dtype, kv_dtype)
+
+    def self_attn(inp):
+        return _mha_cache(mod.attention, _rt(mod.attention, X.device), "sa", inp, inp, inp, B, S, S, mask, False, past,
+                          use_cache, kvd, ops.EPI_BF16)
+
+    def cross_attn(inp):
+        return _mha_cache(mod.cross_attention, _rt(mod.cross_attention, X.device), "ca", inp, ENC, ENC, B, S, S_enc,
+                          cross_mask, False, None, False, kvd, ops.EPI_BF16)[0]
+
+    if mod.norm_first:   # transformer.py:390-428
+        ops.add_layernorm_fwd(X, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
+        Y, cache = self_attn(LN)
+        XA = ws.get("d.XA", (M, d), f32)                        # x + self-attention
+        if cross:
+            ops.add_layernorm_fwd(X, Y, XA, LN, None, lnc.weight, lnc.bias, None, None, M, d, lnc.eps)
+            Y = cross_attn(LN)
+            XC = ws.get("d.XC", (M, d), f32)                    # ... + cross-attention
+            ops.add_layernorm_fwd(XA, Y, XC, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+        else:
+            ops.add_layernorm_fwd(X, Y, XA, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+            XC = XA
+        ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
+        Y = ws.get("d.Y", (M, d), bf)
+        ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
+        ops.add_layernorm_fwd(XC, Y, out, None, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+    else:                # transformer.py:430-470
+        ops.cast_bf16(X.view(-1), LN.view(-1))
+        Y, cache = self_attn(LN)
+        H1 = ws.get("d.H1", (M, d), f32)                        # LN1(x + self-attention), fp32 + its bf16 copy
+        ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
+        if cross:
+            Y = cross_attn(LN)
+            H2 = ws.get("d.H2", (M, d), f32)
+            ops.add_layernorm_fwd(H1, Y, None, LN, H2, lnc.weight, lnc.bias, None, None, M, d, lnc.eps)
+            H1 = H2
+        ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
+        Y = ws.get("d.Y", (M, d), bf)
+        ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
+        ops.add_layernorm_fwd(H1, Y, None, None, out, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+    return out, cache
+
+
+def _decoder_inputs(mod: nn.Module, hidden_states, encoder_hidden_states, what: str):
+    forward_only_guard(mod, what)   # the layers' constructors already refuse dropout > 0
+    _cuda(hidden_states, what)
+    B, S, d = hidden_states.shape
+    X = hidden_states.contiguous().float().view(B * S, d)
+    ENC, S_enc = None, 0
+    if encoder_hidden_states is not None:
+        _cuda(encoder_hidden_states, what)
+        if encoder_hidden_states.size(0) != B:
+            raise ValueError("key and value should have the same bsz as query.")
+        S_enc = encoder_hidden_states.shape[1]
+        ENC = _to_bf16_rows(_rt(mod, hidden_states.device), encoder_hidden_states, "dec.ENC")
+    return B, S, d, X, ENC, S_enc
+
+
+def decoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
+                          encoder_hidden_states: Optional[torch.Tensor] = None,
+                          attention_mask: Optional[torch.Tensor] = None,
+                          cross_attention_mask: Optional[torch.Tensor] = None, past_key_value=None,
+                          use_cache: bool = False):
+    """TransformerDecoderLayer.forward (transformer.py:472-519): (output, present_key_value or None)."""
+    B, S, d, X, ENC, S_enc = _decoder_inputs(mod, hidden_states, encoder_hidden_states, "TransformerDecoderLayer")
+    Sp = 0 if past_key_value is None else past_key_value[0].shape[2]
+    mask = _rect_mask_u8(attention_mask, B, S, Sp + S, "TransformerDecoderLayer")
+    cmask = _rect_mask_u8(cross_attention_mask, B, S, S_enc, "TransformerDecoderLayer") if ENC is not None else (None, 0, 0)
+    out, cache = _decoder_layer(mod, X, B, S, ENC, S_enc, mask, cmask, past_key_value, use_cache, hidden_states.dtype)
+    return out.view(B, S, d).to(hidden_states.dtype), cache
+
+
+def decoder_forward(mod: nn.Module, hidden_states: torch.Tensor, encoder_hidden_states: Optional[torch.Tensor] = None,
+                    attention_mask: Optional[torch.Tensor] = None, cross_attention_mask: Optional[torch.Tensor] = None,
+                    past_key_values=None, use_cache: bool = False, return_hidden_states: bool = False):
+    """TransformerDecoder.forward (transformer.py:588-657).  As in the reference, cross_attention_mask is accepted and
+    not passed to the layers, and hidden_states / current_key_values are empty lists when not requested."""
+    from .modules.layers.transformer import TransformerOutput
+
+    B, S, d, X, ENC, S_enc = _decoder_inputs(mod, hidden_states, encoder_hidden_states, "TransformerDecoder")
+    dt = hidden_states.dtype
+    Sp = 0 if past_key_values is None else past_key_values[0][0].shape[2]
+    mask = _rect_mask_u8(attention_mask, B, S, Sp + S, "TransformerDecoder")
+    all_hidden, current = [], []
+    x = X
+    for i, layer in enumerate(mod.layer):
+        if return_hidden_states:
+            all_hidden.append(hidden_states if i == 0 else x.view(B, S, d).to(dt))
+        past = past_key_values[i] if past_key_values is not None else None
+        x, cache = _decoder_layer(layer, x, B, S, ENC, S_enc, mask, (None, 0, 0), past, use_cache, dt)
+        if use_cache:
+            current.append(cache)
+    if return_hidden_states:
+        all_hidden.append(x.view(B, S, d).to(dt))
+    if mod.final_layer_norm is not None:
+        ln = mod.final_layer_norm
+        y = torch.empty_like(x)
+        ops.add_layernorm_fwd(x, None, None, None, y, ln.weight, ln.bias, None, None, B * S, d, ln.eps)
+        x = y
+    return TransformerOutput(last_hidden_state=x.view(B, S, d).to(dt), hidden_states=all_hidden,
+                             current_key_values=current)

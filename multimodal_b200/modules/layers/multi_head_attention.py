@@ -1,12 +1,17 @@
 """Parameter containers mirroring torchmultimodal/modules/layers/multi_head_attention.py:19-180
 (`MultiHeadSelfAttention` with the fused ``input_proj [3d, d]``; `MultiHeadAttentionWithCache` with separate
 ``q_proj / k_proj / v_proj / output_proj``).  They execute inside the owning encoder / decoder / pooler runtime
-(engine_coca.py): packed-QKV wgmma GEMM + attention kernel; F.scaled_dot_product_attention is never called."""
-from typing import Any, Optional
+(engine_coca.py): packed-QKV wgmma GEMM + attention kernel; F.scaled_dot_product_attention is never called.  Both are
+also callable on their own (forward values, engine_layers.py); `MultiHeadAttentionWithCache` then keeps the reference's
+key / value cache (`past_key_value` / `use_cache`) for autoregressive decoding, on the split-KV decode kernel."""
+from typing import NamedTuple, Optional, Tuple, Union
 
 from torch import nn, Tensor
 
-from ..._lib import MMBError
+
+class MHAWithCacheOutput(NamedTuple):
+    attn_output: Tensor
+    past_key_value: Tuple[Tensor, Tensor]
 
 
 class MultiHeadSelfAttention(nn.Module):
@@ -34,6 +39,12 @@ class MultiHeadAttentionWithCache(nn.Module):
         self.output_proj = nn.Linear(dim_q, dim_q)
         self.dropout = dropout
 
-    def forward(self, *args: Any, **kwargs: Any) -> Tensor:
-        raise MMBError("MultiHeadAttentionWithCache is fused into the decoder / pooler runtime; not a standalone op "
-                       "here (KV-cache decoding is outside the accelerated forward path)")
+    def forward(self, query: Tensor, key: Tensor, value: Tensor, attn_mask: Optional[Tensor] = None,
+                past_key_value: Optional[Tuple[Tensor, Tensor]] = None, is_causal: bool = False,
+                use_cache: bool = False) -> Union[Tensor, MHAWithCacheOutput]:
+        """Standalone forward (values only): projections -> key / value cache append -> attention (split-KV decode
+        kernel for queries of at most 16 rows) -> out-projection.  The returned cache tensors [B, H, S, head_dim] are
+        fresh on every call, as with torch.cat in the reference."""
+        from ...engine_layers import mha_cache_forward
+
+        return mha_cache_forward(self, query, key, value, attn_mask, past_key_value, is_causal, use_cache)

@@ -2,13 +2,11 @@
 CoCa encoder returns) and the parameter containers `TransformerEncoderLayer` / `TransformerEncoder` (:31-259) and
 `TransformerDecoderLayer` / `TransformerDecoder` (:262-657) — same constructors, state-dict keys and creation order.
 The layers execute inside `engine_coca.LayerStack` (fused kernels), owned by VisionTransformer / CoCaTextDecoder /
-CoCaMultimodalDecoder; `TransformerEncoderLayer` / `TransformerEncoder` are also callable on their own (forward values,
-same kernels: `engine_layers.py`).  The decoder classes stay containers (KV-cache decoding is outside the path)."""
-from typing import Any, Callable, List, NamedTuple, Optional, Tuple
+CoCaMultimodalDecoder; all four are also callable on their own (forward values, same kernels: `engine_layers.py`), the
+decoders with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive decoding."""
+from typing import Callable, List, NamedTuple, Optional, Tuple
 
 from torch import nn, Tensor
-
-from ..._lib import MMBError
 
 
 class TransformerOutput(NamedTuple):
@@ -100,8 +98,15 @@ class TransformerDecoderLayer(nn.Module):
         self.feedforward_layernorm = Fp32LayerNorm(d_model, eps=layer_norm_eps)
         self.norm_first = norm_first
 
-    def forward(self, *args: Any, **kwargs: Any) -> Tuple[Tensor, Optional[Tuple[Tensor, Tensor]]]:
-        raise MMBError("TransformerDecoderLayer runs inside its decoder's fused runtime; not a standalone op here")
+    def forward(self, hidden_states: Tensor, encoder_hidden_states: Optional[Tensor] = None,
+                attention_mask: Optional[Tensor] = None, cross_attention_mask: Optional[Tensor] = None,
+                past_key_value: Optional[Tuple[Tensor, Tensor]] = None,
+                use_cache: bool = False) -> Tuple[Tensor, Optional[Tuple[Tensor, Tensor]]]:
+        """Standalone forward (values only; inside CoCa the layer runs in the fused LayerStack)."""
+        from ...engine_layers import decoder_layer_forward
+
+        return decoder_layer_forward(self, hidden_states, encoder_hidden_states, attention_mask, cross_attention_mask,
+                                     past_key_value, use_cache)
 
 
 class TransformerDecoder(nn.Module):
@@ -122,5 +127,12 @@ class TransformerDecoder(nn.Module):
         if final_layer_norm_eps:
             self.final_layer_norm = Fp32LayerNorm(d_model, eps=final_layer_norm_eps)
 
-    def forward(self, *args: Any, **kwargs: Any) -> TransformerOutput:
-        raise MMBError("TransformerDecoder runs inside its owner's fused runtime; not a standalone op here")
+    def forward(self, hidden_states: Tensor, encoder_hidden_states: Optional[Tensor] = None,
+                attention_mask: Optional[Tensor] = None, cross_attention_mask: Optional[Tensor] = None,
+                past_key_values: Optional[List[Tuple[Tensor, Tensor]]] = None, use_cache: bool = False,
+                return_hidden_states: bool = False) -> TransformerOutput:
+        """Standalone forward (values only; inside CoCa the stack runs in the fused LayerStack)."""
+        from ...engine_layers import decoder_forward
+
+        return decoder_forward(self, hidden_states, encoder_hidden_states, attention_mask, cross_attention_mask,
+                               past_key_values, use_cache, return_hidden_states)

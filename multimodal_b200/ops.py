@@ -450,6 +450,58 @@ def attention_fwd_generic(q, k, v, out, *, B, Sq, Skv, H, head_dim, bsq, bsk, bs
                                                     float(scale), _stream()), "mmb_attention_fwd_generic")
 
 
+# Longest query the split-KV decode kernel takes (one m16 tile); longer queries run attention_fwd_generic.
+DECODE_MAX_SQ = 16
+
+
+def decode_attention_wins(B: int, H: int, Sq: int, Skv: int) -> bool:
+    """Whether attention_fwd_decode beats attention_fwd_generic at this shape (scripts/decode_bench.py, DESIGN.md §9):
+    at every Sq <= 16 except short caches over many (batch, head) pairs, where both launch one CTA per pair and the
+    general kernel's wider CTAs win (Skv 77, B 64, H 12: 24-26 us against 34-40 us at head_dim 64)."""
+    return Sq <= DECODE_MAX_SQ and not (Skv <= 128 and B * H >= 264)
+
+
+def attention_fwd_decode(q, k, v, out, *, B, Sq, Skv, H, head_dim, bsq, bsk, bsv, bso, scale, mask=None, mask_bs=0,
+                         mask_qs=0, causal=False):
+    """attention_fwd_generic's contract for Sq <= DECODE_MAX_SQ, on the split-KV decode kernel."""
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
+        _chk(t, torch.bfloat16, n); _rowmajor(t, n)
+    if mask is not None:
+        _chk(mask, torch.uint8, "mask")
+    _lib.check(_lib.lib().mmb_attention_fwd_decode(_p(q), q.stride(0), int(bsq), _p(k), k.stride(0), int(bsk), _p(v),
+                                                   v.stride(0), int(bsv), _p(out), out.stride(0), int(bso), _p(mask),
+                                                   int(mask_bs), int(mask_qs), B, Sq, Skv, H, head_dim, int(causal),
+                                                   float(scale), _stream()), "mmb_attention_fwd_decode")
+
+
+def attention_decode_splits(B: int, H: int, Skv: int) -> int:
+    return int(_lib.lib().mmb_attention_decode_splits(int(B), int(H), int(Skv)))
+
+
+def kv_cache_append(past, new_rows, out, out_bf16, *, B, H, Sp, Sn, head_dim):
+    """cat(past, new) along the sequence into row-major [B, Sp + Sn, H*head_dim] buffers.  past: [B, H, Sp, head_dim]
+    fp32 / bf16 with unit inner stride (or None when Sp = 0); new_rows: bf16 2-D view [B*Sn, >= H*head_dim]; out: fp32
+    or bf16, out_bf16: bf16 (either may be None)."""
+    _chk(new_rows, torch.bfloat16, "new_rows"); _rowmajor(new_rows, "new_rows")
+    if past is not None:
+        if past.dtype not in (torch.float32, torch.bfloat16) or not past.is_cuda or past.stride(-1) != 1:
+            raise MMBError("kv_cache_append: past must be a CUDA fp32 / bf16 tensor with unit stride along head_dim")
+        if tuple(past.shape) != (B, H, Sp, head_dim):
+            raise MMBError(f"kv_cache_append: past shape {tuple(past.shape)} != {(B, H, Sp, head_dim)}")
+    for t, n in ((out, "out"), (out_bf16, "out_bf16")):
+        if t is not None and (not t.is_cuda or not t.is_contiguous() or t.numel() != B * (Sp + Sn) * H * head_dim):
+            raise MMBError(f"kv_cache_append: {n} must be a contiguous CUDA tensor of B * (Sp + Sn) * H * head_dim elements")
+    if out is not None and out.dtype not in (torch.float32, torch.bfloat16):
+        raise MMBError(f"kv_cache_append: out dtype {out.dtype} is not fp32 / bf16")
+    if out_bf16 is not None:
+        _chk(out_bf16, torch.bfloat16, "out_bf16")
+    ps = past.stride() if past is not None else (0, 0, 0, 1)
+    _lib.check(_lib.lib().mmb_kv_cache_append(_p(past), int(past is not None and past.dtype == torch.float32), ps[0],
+                                              ps[1], ps[2], _p(new_rows), new_rows.stride(0), _p(out),
+                                              int(out is not None and out.dtype == torch.float32), _p(out_bf16), B, H, Sp,
+                                              Sn, head_dim, _stream()), "mmb_kv_cache_append")
+
+
 def ce_labels(logits, labels, label_stride, ignore_index, M, V, row_loss, accum):
     _chk(logits, torch.float32, "logits"); _chk(labels, torch.int64, "labels"); _rowmajor(logits, "logits")
     _lib.check(_lib.lib().mmb_ce_labels(_p(logits), logits.stride(0), _p(labels), int(label_stride), int(ignore_index), M,
