@@ -193,6 +193,113 @@ def _numel(shape) -> int:
     return n
 
 
+class _Shadows:
+    """bf16 operand copies of fp32 weights outside a ParamStore, re-cast when a parameter's version changes."""
+
+    def __init__(self, device):
+        self.device = device
+        self.bufs: Dict[str, torch.Tensor] = {}
+        self.seen: Dict[str, tuple] = {}
+
+    def get(self, key: str, parts: Sequence[torch.Tensor]) -> torch.Tensor:
+        """bf16 copy of cat(parts, dim=0) (each part [n_i, k])."""
+        ver = (weight_epoch(),) + tuple((p._version, p.data_ptr()) for p in parts)
+        buf = self.bufs.get(key)
+        if buf is None:
+            rows = sum(p.shape[0] for p in parts)
+            buf = torch.empty((rows,) + tuple(parts[0].shape[1:]), device=self.device, dtype=torch.bfloat16)
+            self.bufs[key] = buf
+        if self.seen.get(key) != ver:
+            r = 0
+            for p in parts:
+                src = p.data if p.data.is_contiguous() else p.data.contiguous()
+                ops.cast_bf16(src.view(-1), buf[r:r + p.shape[0]].view(-1))
+                r += p.shape[0]
+            self.seen[key] = ver
+        return buf
+
+    def cat_f32(self, key: str, parts: Sequence[torch.Tensor]) -> torch.Tensor:
+        ver = (weight_epoch(),) + tuple((p._version, p.data_ptr()) for p in parts)
+        buf = self.bufs.get(key)
+        if buf is None:
+            buf = torch.empty(sum(p.numel() for p in parts), device=self.device, dtype=torch.float32)
+            self.bufs[key] = buf
+        if self.seen.get(key) != ver:
+            r = 0
+            for p in parts:
+                buf[r:r + p.numel()].copy_(p.data.reshape(-1))   # 3 x d floats: plumbing
+                r += p.numel()
+            self.seen[key] = ver
+        return buf
+
+
+def act_code(act: nn.Module) -> int:
+    """Kernel epilogue code of an MLP activation module."""
+    from .modules.layers.activation import SiLU
+
+    if isinstance(act, nn.GELU) and getattr(act, "approximate", "none") == "none":
+        return ops.ACT_GELU_ERF
+    if isinstance(act, SiLU):
+        return ops.ACT_QUICK_GELU
+    raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU / SiLU)")
+
+
+def wants_grad(*mods: Optional[nn.Module]) -> bool:
+    """True when the caller expects an autograd graph: grad mode on and some parameter of `mods` trainable."""
+    if not torch.is_grad_enabled():
+        return False
+    return any(p.requires_grad for m in mods if m is not None for p in m.parameters())
+
+
+def patch_embed_fwd(image: torch.Tensor, conv: nn.Module, wconv: torch.Tensor, cls: Optional[torch.Tensor],
+                    pos: torch.Tensor, mask_token: Optional[torch.Tensor], image_patches_mask: Optional[torch.Tensor],
+                    ws: Workspace, save: Workspace, prefix: str):
+    """Patch front end of a ViT (patch_embedding.py:104-154, image_encoder.py:139-175): im2col + conv GEMM (+ bias), then
+    [cls |] patch or mask token, + position embeddings, in one assembly kernel.  wconv: bf16 [d, 3*ps*ps] conv weight.
+    The im2col matrix goes to `save` (the conv weight gradient reads it), the rest of the scratch to `ws`.
+    Returns (X0 fp32 [B*S, d], allocated per call; B, S, P; the uint8 [B, P] patch mask or None)."""
+    d, ps = conv.weight.shape[0], conv.weight.shape[2]
+    image = image.contiguous().float()
+    B, _, Hh, Ww = image.shape
+    P = (Hh // ps) * (Ww // ps)
+    S = P + (1 if cls is not None else 0)
+    K = 3 * ps * ps
+    Kp = -(-K // 8) * 8   # row pitch: bf16 rows must be 16 B multiples for TMA (K = 588 -> 592 for 14x14 patches)
+    bf = torch.bfloat16
+    PATCH = save.get(f"{prefix}.PATCH", (B * P, Kp), bf)[:, :K]
+    PO = ws.get(f"{prefix}.PO", (B * P, d), bf)
+    X0 = torch.empty((B * S, d), device=image.device, dtype=torch.float32)
+    ops.im2col(image, ps, PATCH)
+    if Kp != K:   # re-pitch the (tiny) conv weight shadow the same way
+        wp = ws.get(f"{prefix}.WCONV", (d, Kp), bf)[:, :K]
+        wp.copy_(wconv)
+        wconv = wp
+    ops.gemm(PATCH, wconv, bias=conv.bias, out=PO)
+    pm = None
+    if image_patches_mask is not None and mask_token is not None:
+        pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
+    ops.vit_assemble_fwd(PO, cls, pos, mask_token if pm is not None else None, pm, X0, B, S, d)
+    return X0, B, S, P, pm
+
+
+def patch_embed_bwd(G: torch.Tensor, conv: nn.Module, cls: Optional[torch.Tensor], pos: torch.Tensor,
+                    mask_token: Optional[torch.Tensor], pm: Optional[torch.Tensor], B: int, S: int, P: int,
+                    st: "ParamStore", ws: Workspace, save: Workspace, prefix: str) -> None:
+    """Parameter gradients of patch_embed_fwd from G = d X0 (fp32 [B*S, d])."""
+    d, ps = conv.weight.shape[0], conv.weight.shape[2]
+    K = 3 * ps * ps
+    ops.batch_sum(G, st.grad(pos), B, S * d, S * d)
+    if cls is not None:
+        ops.batch_sum(G, st.grad(cls), B, S * d, d)
+    DP = ws.get(f"{prefix}.DP", (B * P, d), torch.bfloat16)
+    ops.vit_assemble_bwd(G, pm, DP, st.grad(mask_token) if pm is not None else None, B, S, d, cls is not None)
+    PATCH = save.get(f"{prefix}.PATCH", (B * P, -(-K // 8) * 8), torch.bfloat16)[:, :K]
+    ops.gemm(DP, PATCH, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad2d(conv.weight),
+             splits=ops.wgrad_splits(d, K, B * P), accumulate=True)
+    if conv.bias is not None:
+        ops.colsum_bf16(DP, st.grad(conv.bias), B * P, d, d)
+
+
 class TransformerStack:
     """L pre-norm encoder layers (torch.nn.TransformerEncoderLayer parameter layout), QuickGELU or GELU MLP."""
 
@@ -225,8 +332,6 @@ class TransformerStack:
         self._save.kmask = kmask if training else None
         self._save.mask3 = mask3 if training else None
         self._save.enc, self._save.S_enc = (enc, S_enc) if training else (None, 0)
-        if mask3 is not None and kmask is not None:
-            raise MMBError("TransformerStack: pass either a key-padding mask or a [B, S, S] mask, not both")
         st, d, ff, H = self.store, self.d, self.ff, self.H
         M = B * S
         bf, f32 = torch.bfloat16, torch.float32
@@ -253,14 +358,7 @@ class TransformerStack:
                 ops.add_layernorm_fwd(XM_prev, Y, XA, LN1, None, layer.norm1.weight, layer.norm1.bias, m1, r1, M, d,
                                       layer.norm1.eps)
             ops.gemm(LN1, st.shadow(at.in_proj_weight), bias=at.in_proj_bias, out=QKV)
-            if mask3 is not None:
-                ops.attention_fwd_generic(QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], O, B=B, Sq=S, Skv=S, H=H, head_dim=64,
-                                          bsq=S * 3 * d, bsk=S * 3 * d, bsv=S * 3 * d, bso=S * d, scale=self.scale,
-                                          mask=mask3, mask_bs=S * S, mask_qs=S, causal=self.causal)
-            elif kmask is not None:
-                ops.attention_fwd_kmask(QKV, O, LSE, kmask, B, S, H, self.causal, self.scale)
-            else:
-                ops.attention_fwd(QKV, O, LSE, B, S, H, self.causal, self.scale)
+            ops.self_attention(QKV, O, LSE, B, S, H, 64, self.causal, self.scale, kmask=kmask, mask=mask3)
             ops.gemm(O, st.shadow(at.out_proj.weight), bias=at.out_proj.bias, out=Y)
             ca = getattr(layer, "cross_attn", None)
             if ca is not None and enc is not None:
@@ -382,15 +480,8 @@ class TransformerStack:
             ops.gemm(Gb, O, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(at.out_proj.weight),
                      splits=sp(d, d, M), accumulate=True)
             ops.gemm(Gb, st.shadow(at.out_proj.weight), b_mn=True, out=T1)  # dO
-            if mask3 is not None:
-                ops.attention_bwd_generic(QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], T1, T3[:, d:2 * d], T3[:, 2 * d:],
-                                          dq=T3[:, :d], B=B, Sq=S, Skv=S, H=H, head_dim=64, bsq=S * 3 * d, bsk=S * 3 * d,
-                                          bsv=S * 3 * d, bso=S * d, scale=self.scale, mask=mask3, mask_bs=S * S, mask_qs=S,
-                                          causal=self.causal)
-            elif kmask is not None:
-                ops.attention_bwd_kmask(QKV, O, T1, LSE, T3, kmask, B, S, H, self.causal, self.scale)
-            else:
-                ops.attention_bwd(QKV, O, T1, LSE, T3, B, S, H, self.causal, self.scale)
+            ops.self_attention(QKV, O, LSE, B, S, H, 64, self.causal, self.scale, kmask=kmask, mask=mask3, dout=T1,
+                               dqkv=T3)
             ops.gemm(T3, LN1, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(at.in_proj_weight),
                      splits=sp(3 * d, d, M), accumulate=True)
             ops.colsum_bf16(T3, st.grad(at.in_proj_bias), M, 3 * d, 3 * d)
@@ -554,3 +645,36 @@ class TextTower:
         self.stack.backward(G, Gb, B, S, top_bias_done=True)
         ops.batch_sum(G, st.grad(mod.positional_embedding), B, S * d, S * d)
         ops.text_embed_bwd(self.tokens, G, st.grad(mod.token_embedding.weight), B, S, d)
+
+
+class RuntimeFunction(torch.autograd.Function):
+    """One training forward of a runtime that keeps its activations.  inputs: (runtime, data, n_diff, *diff_inputs,
+    *parameters).  rt.forward(data, diff) -> (outputs, save); rt.backward(save, *d outputs) -> gradients of diff."""
+
+    @staticmethod
+    def forward(ctx, rt, data, n_diff, *tensors):
+        ctx.set_materialize_grads(False)   # an unused output arrives as None in backward, not as a zero tensor
+        outs, save = rt.forward(data, tensors[:n_diff])
+        ctx.rt, ctx.save, ctx.n_diff = rt, save, n_diff
+        ctx.need = ctx.needs_input_grad[3 + n_diff:]
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *douts):
+        rt, save = ctx.rt, ctx.save
+        if save is None:
+            raise MMBError("this forward was already back-propagated (its activations are freed)")
+        st = rt.store
+        st.zero_grads()
+        in_grads = rt.backward(save, *douts)
+        ctx.save = None
+        g = st.g.clone()
+        grads = []
+        for p, need in zip(st.params, ctx.need):
+            o = st.off[id(p)]
+            grads.append(g[o:o + p.numel()].view(p.shape) if need else None)
+        return (None, None, None, *in_grads, *grads)
+
+
+def run(rt, data, diff: Sequence[torch.Tensor] = ()):
+    return RuntimeFunction.apply(rt, data, len(diff), *diff, *rt.store.params)

@@ -24,14 +24,7 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import Workspace
-from .engine_flava import _Shadows
-
-
-def _act_code(act: nn.Module) -> int:
-    if isinstance(act, nn.GELU) and getattr(act, "approximate", "none") == "none":
-        return ops.ACT_GELU_ERF
-    raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU only)")
+from .engine import Workspace, _Shadows, act_code, patch_embed_fwd
 
 
 class LayerStack:
@@ -51,7 +44,7 @@ class LayerStack:
         if self.hd not in (64, 96, 128):
             raise MMBError(f"unsupported head_dim {self.hd}")
         self.ff = l0.feedforward.model[0].weight.shape[0]
-        self.act = _act_code(l0.feedforward.model[1])
+        self.act = act_code(l0.feedforward.model[1])
         self.ws = Workspace(device)
         self.sh = _Shadows(device)
 
@@ -94,13 +87,7 @@ class LayerStack:
             else:
                 ops.add_layernorm_fwd(XA, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
             ops.gemm(LN, wqkv, bias=bqkv, out=QKV)
-            if mask is None and hd == 64 and (S <= 384 or S > ops.GENERIC_FWD_MAX_S):
-                ops.attention_fwd(QKV, O, None, B, S, H, causal, scale)
-            else:
-                ops.attention_fwd_generic(QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], O, B=B, Sq=S, Skv=S, H=H,
-                                          head_dim=hd, bsq=S * 3 * d, bsk=S * 3 * d, bsv=S * 3 * d, bso=S * d, scale=scale,
-                                          mask=mask, mask_bs=S * S if mask is not None else 0,
-                                          mask_qs=S if mask is not None else 0, causal=causal)
+            ops.self_attention(QKV, O, None, B, S, H, hd, causal, scale, mask=mask)
             ops.gemm(O, sh.get(f"{l}.wo", [at.output_proj.weight]), bias=at.output_proj.bias, out=Y)
             XR = XM
             if getattr(layer, "use_cross_attention", False) and enc is not None:
@@ -152,31 +139,10 @@ class VisionRuntime:
         from .modules.layers.transformer import TransformerOutput
 
         emb, st = self.mod.embeddings, self.stack
-        ws, sh, d = st.ws, st.sh, st.d
-        conv = emb.conv_projection
-        ps = conv.weight.shape[2]
-        image = images.contiguous().float()
-        B, _, Hh, Ww = image.shape
-        P = (Hh // ps) * (Ww // ps)
-        S = P + (1 if emb.include_cls_embed else 0)
-        K = 3 * ps * ps
-        Kp = -(-K // 8) * 8
-        bf, f32 = torch.bfloat16, torch.float32
-        PATCH = ws.get("vit.PATCH", (B * P, Kp), bf)[:, :K]
-        PO = ws.get("vit.PO", (B * P, d), bf)
-        X0 = torch.empty((B * S, d), device=image.device, dtype=f32)   # returned as hidden_states[0]
-        ops.im2col(image, ps, PATCH)
-        w = sh.get("conv.w", [conv.weight.view(d, K)])
-        if Kp != K:
-            wp = ws.get("vit.WCONV", (d, Kp), bf)[:, :K]
-            wp.copy_(w)
-            w = wp
-        ops.gemm(PATCH, w, bias=conv.bias, out=PO)
-        pm = None
-        if image_patches_mask is not None and emb.mask_token is not None:
-            pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
-        ops.vit_assemble_fwd(PO, emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
-                             emb.mask_token if pm is not None else None, pm, X0, B, S, d)
+        d, conv = st.d, emb.conv_projection
+        X0, B, S, _, _ = patch_embed_fwd(images, conv, st.sh.get("conv.w", [conv.weight.view(d, -1)]),
+                                         emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
+                                         emb.mask_token, image_patches_mask, st.ws, st.ws, "vit")   # hidden_states[0]
         hidden = st.run(X0, B, S, keep_hidden=True)
         fln = self.mod.encoder.final_layer_norm
         XF, LAST, _ = st.finish(B, S, fln)

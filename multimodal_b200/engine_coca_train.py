@@ -23,21 +23,14 @@ from __future__ import annotations
 
 import math
 from types import SimpleNamespace
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Optional, Sequence
 
 import torch
 from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import ParamStore, TransformerStack, Workspace
-from .engine_flava_train import wants_grad  # noqa: F401  (re-exported for the modules)
-
-
-def _act_code(act: nn.Module) -> int:
-    if isinstance(act, nn.GELU) and getattr(act, "approximate", "none") == "none":
-        return ops.ACT_GELU_ERF
-    raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU only)")
+from .engine import ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run
 
 
 def _qkv_first(layers) -> List[nn.Parameter]:
@@ -103,7 +96,7 @@ class _Stack:
         self.ws = Workspace(self.device)
         self.stack = TransformerStack(_adapters(layers, self.store), self.store, self.ws, d=self.d, heads=H,
                                       ff=l0.feedforward.model[0].weight.shape[0], causal=causal,
-                                      act=_act_code(l0.feedforward.model[1]), prefix=prefix)
+                                      act=act_code(l0.feedforward.model[1]), prefix=prefix)
         self.prefix, self.L = prefix, len(layers)
 
     def finish(self, XM, Y, M: int, ln: Optional[nn.Module], save: Workspace):
@@ -154,60 +147,29 @@ class VisionTrainRuntime:
     def forward(self, data, diff):
         images, image_patches_mask = data
         emb, s, st = self.mod.embeddings, self.s, self.store
-        d = s.d
-        conv = emb.conv_projection
-        ps = conv.weight.shape[2]
-        image = images.contiguous().float()
-        B, _, Hh, Ww = image.shape
-        P = (Hh // ps) * (Ww // ps)
-        cls = emb.cls_token if emb.include_cls_embed else None
-        S = P + (1 if cls is not None else 0)
-        K = 3 * ps * ps
-        Kp = -(-K // 8) * 8
-        bf, f32 = torch.bfloat16, torch.float32
+        d, conv = s.d, emb.conv_projection
         st.refresh()
         save = Workspace(s.device)
-        PATCH = save.get("cvit.PATCH", (B * P, Kp), bf)[:, :K]
-        PO = s.ws.get("cvit.PO", (B * P, d), bf)
-        X0 = torch.empty((B * S, d), device=image.device, dtype=f32)
-        ops.im2col(image, ps, PATCH)
-        w = st.shadow2d(conv.weight)
-        if Kp != K:
-            wp = s.ws.get("cvit.WCONV", (d, Kp), bf)[:, :K]
-            wp.copy_(w)
-            w = wp
-        ops.gemm(PATCH, w, bias=conv.bias, out=PO)
-        pm = None
-        if image_patches_mask is not None and emb.mask_token is not None:
-            pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
-        ops.vit_assemble_fwd(PO, cls, emb.position_embeddings, emb.mask_token if pm is not None else None, pm, X0, B, S, d)
+        X0, B, S, P, pm = patch_embed_fwd(images, conv, st.shadow2d(conv.weight),
+                                          emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
+                                          emb.mask_token, image_patches_mask, s.ws, save, "cvit")
         XM, Y = s.stack.forward(X0, B, S, True, save=save)
         XF, LAST = s.finish(XM, Y, B * S, self.mod.encoder.final_layer_norm, save)
-        save.B, save.S, save.P, save.K, save.pm = B, S, P, K, pm
+        save.B, save.S, save.P, save.pm = B, S, P, pm
         self.last_hidden = ([X0.view(B, S, d)] + [save.bufs[f"cvit.XA.{l}"].view(B, S, d) for l in range(1, s.L)]
                             + [XF.view(B, S, d)])
         return ((LAST if LAST is not None else XF),), save
 
     def backward(self, save, dOUT):
-        emb, s, st = self.mod.embeddings, self.s, self.store
-        d, B, S, P, K = s.d, save.B, save.S, save.P, save.K
+        emb, s = self.mod.embeddings, self.s
+        d, B, S = s.d, save.B, save.S
         M = B * S
         fln = self.mod.encoder.final_layer_norm
         dOUT = _f32(dOUT, (M, d))
         G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
         G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
-        has_cls = emb.include_cls_embed
-        conv = emb.conv_projection
-        ops.batch_sum(G, st.grad(emb.position_embeddings), B, S * d, S * d)
-        if has_cls:
-            ops.batch_sum(G, st.grad(emb.cls_token), B, S * d, d)
-        DP = s.ws.get("cvit.DP", (B * P, d), torch.bfloat16)
-        ops.vit_assemble_bwd(G, save.pm, DP, st.grad(emb.mask_token) if save.pm is not None else None, B, S, d, has_cls)
-        PATCH = save.get("cvit.PATCH", (B * P, -(-K // 8) * 8), torch.bfloat16)[:, :K]
-        ops.gemm(DP, PATCH, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad2d(conv.weight),
-                 splits=ops.wgrad_splits(d, PATCH.shape[1], B * P), accumulate=True)
-        if conv.bias is not None:
-            ops.colsum_bf16(DP, st.grad(conv.bias), B * P, d, d)
+        patch_embed_bwd(G, emb.conv_projection, emb.cls_token if emb.include_cls_embed else None,
+                        emb.position_embeddings, emb.mask_token, save.pm, B, S, save.P, self.store, s.ws, save, "cvit")
         return ()
 
 
@@ -420,39 +382,6 @@ class MultimodalDecoderTrainRuntime:
         G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
         G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
         return (G.view(B, S, d).clone(), save.dENC.view(B, save.Si, save.dv))
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-class RuntimeFunction(torch.autograd.Function):
-    """One training forward of a runtime above.  inputs: (runtime, data, n_diff, *diff_inputs, *parameters)."""
-
-    @staticmethod
-    def forward(ctx, rt, data, n_diff, *tensors):
-        ctx.set_materialize_grads(False)
-        outs, save = rt.forward(data, tensors[:n_diff])
-        ctx.rt, ctx.save, ctx.n_diff = rt, save, n_diff
-        ctx.need = ctx.needs_input_grad[3 + n_diff:]
-        return tuple(outs)
-
-    @staticmethod
-    def backward(ctx, *douts):
-        rt, save = ctx.rt, ctx.save
-        if save is None:
-            raise MMBError("this forward was already back-propagated (its activations are freed)")
-        st = rt.store
-        st.zero_grads()
-        in_grads = rt.backward(save, *douts)
-        ctx.save = None
-        g = st.g.clone()
-        grads = []
-        for p, need in zip(st.params, ctx.need):
-            o = st.off[id(p)]
-            grads.append(g[o:o + p.numel()].view(p.shape) if need else None)
-        return (None, None, None, *in_grads, *grads)
-
-
-def run(rt, data, diff: Sequence[torch.Tensor] = ()) -> Tuple[torch.Tensor, ...]:
-    return RuntimeFunction.apply(rt, data, len(diff), *diff, *rt.store.params)
 
 
 class LinearF32Function(torch.autograd.Function):

@@ -18,7 +18,7 @@ scratch is reused between forwards.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional, Sequence
+from typing import List, Optional
 
 import torch
 from torch import nn
@@ -26,48 +26,8 @@ from torch import nn
 from . import engine as _engine
 from . import ops
 from ._lib import MMBError
-from .engine import Workspace, weight_epoch
+from .engine import Workspace, _Shadows, act_code, patch_embed_fwd
 from .modules.layers.transformer import TransformerOutput
-
-
-class _Shadows:
-    """bf16 operand copies of the fp32 parameters of one encoder, re-cast when a parameter's version changes."""
-
-    def __init__(self, device):
-        self.device = device
-        self.bufs: Dict[str, torch.Tensor] = {}
-        self.seen: Dict[str, tuple] = {}
-
-    def get(self, key: str, parts: Sequence[torch.Tensor]) -> torch.Tensor:
-        """bf16 copy of cat(parts, dim=0) (each part [n_i, k])."""
-        ver = (weight_epoch(),) + tuple((p._version, p.data_ptr()) for p in parts)
-        buf = self.bufs.get(key)
-        if buf is None:
-            rows = sum(p.shape[0] for p in parts)
-            buf = torch.empty((rows,) + tuple(parts[0].shape[1:]), device=self.device, dtype=torch.bfloat16)
-            self.bufs[key] = buf
-        if self.seen.get(key) != ver:
-            r = 0
-            for p in parts:
-                src = p.data if p.data.is_contiguous() else p.data.contiguous()
-                ops.cast_bf16(src.view(-1), buf[r:r + p.shape[0]].view(-1))
-                r += p.shape[0]
-            self.seen[key] = ver
-        return buf
-
-    def cat_f32(self, key: str, parts: Sequence[torch.Tensor]) -> torch.Tensor:
-        ver = (weight_epoch(),) + tuple((p._version, p.data_ptr()) for p in parts)
-        buf = self.bufs.get(key)
-        if buf is None:
-            buf = torch.empty(sum(p.numel() for p in parts), device=self.device, dtype=torch.float32)
-            self.bufs[key] = buf
-        if self.seen.get(key) != ver:
-            r = 0
-            for p in parts:
-                buf[r:r + p.numel()].copy_(p.data.reshape(-1))   # 3 x d floats: plumbing
-                r += p.numel()
-            self.seen[key] = ver
-        return buf
 
 
 class FlavaStack:
@@ -84,11 +44,7 @@ class FlavaStack:
         if self.d // self.H != 64:
             raise MMBError("attention kernels support head_dim 64 only")
         self.ff = l0.feedforward.model[0].weight.shape[0]
-        act = l0.feedforward.model[1]
-        if isinstance(act, nn.GELU):
-            self.act = ops.ACT_GELU_ERF
-        else:
-            raise MMBError(f"unsupported MLP activation {type(act).__name__} (FLAVA uses nn.GELU)")
+        self.act = act_code(l0.feedforward.model[1])
         self.layernorm, self.pooler, self.prefix = layernorm, pooler, prefix
         dev = l0.attention.query.weight.device
         _engine._require_cuda(dev)
@@ -130,10 +86,7 @@ class FlavaStack:
             else:
                 ops.add_layernorm_fwd(XA, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
             ops.gemm(LN, wqkv, bias=bqkv, out=QKV)
-            if kmask is not None:
-                ops.attention_fwd_kmask(QKV, O, LSE, kmask, B, S, H, False, 0.125)
-            else:
-                ops.attention_fwd(QKV, O, LSE, B, S, H, False, 0.125)
+            ops.self_attention(QKV, O, LSE, B, S, H, 64, False, 0.125, kmask=kmask)
             if want_attn:
                 P = torch.empty((B, H, S, S), device=self.device, dtype=f32)
                 ops.attention_probs(QKV, LSE, kmask, P, B, S, H, False, 0.125)
@@ -178,31 +131,10 @@ class FlavaImageRuntime:
     def forward(self, pixel_values: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None,
                 want_attn: bool = False) -> TransformerOutput:
         emb, st = self.mod.embeddings, self.stack
-        ws, sh, d = st.ws, st.sh, st.d
         conv = emb.patch_embeddings.projection
-        ps = conv.weight.shape[2]
-        image = pixel_values.contiguous().float()
-        B, _, Hh, Ww = image.shape
-        P = (Hh // ps) * (Ww // ps)
-        S = P + 1
-        K = 3 * ps * ps
-        Kp = -(-K // 8) * 8
-        bf, f32 = torch.bfloat16, torch.float32
-        PATCH = ws.get("fimg.PATCH", (B * P, Kp), bf)[:, :K]
-        PO = ws.get("fimg.PO", (B * P, d), bf)
-        X0 = torch.empty((B * S, d), device=image.device, dtype=f32)   # returned as hidden_states[0]
-        ops.im2col(image, ps, PATCH)
-        w = sh.get("conv.w", [conv.weight.view(d, K)])
-        if Kp != K:
-            wp = ws.get("fimg.WCONV", (d, Kp), bf)[:, :K]
-            wp.copy_(w)
-            w = wp
-        ops.gemm(PATCH, w, bias=conv.bias, out=PO)
-        pm = None
-        if image_patches_mask is not None and emb.mask_token is not None:
-            pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
-        ops.vit_assemble_fwd(PO, emb.cls_token, emb.position_embeddings, emb.mask_token if pm is not None else None, pm, X0,
-                             B, S, d)
+        X0, B, S, _, _ = patch_embed_fwd(pixel_values, conv, st.sh.get("conv.w", [conv.weight.view(st.d, -1)]),
+                                         emb.cls_token, emb.position_embeddings, emb.mask_token, image_patches_mask,
+                                         st.ws, st.ws, "fimg")   # X0 is returned as hidden_states[0]
         return st.forward(X0, B, S, want_attn=want_attn)
 
 

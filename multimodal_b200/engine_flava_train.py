@@ -32,15 +32,8 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import ParamStore, TransformerStack, Workspace
+from .engine import ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run
 from .modules.layers.transformer import TransformerOutput
-
-
-def wants_grad(*mods: Optional[nn.Module]) -> bool:
-    """True when the caller expects an autograd graph: grad mode on and some parameter of `mods` trainable."""
-    if not torch.is_grad_enabled():
-        return False
-    return any(p.requires_grad for m in mods if m is not None for p in m.parameters())
 
 
 class FlavaTrainStack:
@@ -52,8 +45,6 @@ class FlavaTrainStack:
         l0 = layers[0]
         if not l0.norm_first:
             raise MMBError("only pre-norm (norm_first=True) FLAVA layers are on the accelerated path")
-        if not isinstance(l0.feedforward.model[1], nn.GELU):
-            raise MMBError("unsupported MLP activation (FLAVA uses nn.GELU)")
         d, H = l0.attention.dim_q, l0.attention.n_head
         ff = l0.feedforward.model[0].weight.shape[0]
         params: List[nn.Parameter] = []
@@ -78,13 +69,14 @@ class FlavaTrainStack:
             adapters.append(SimpleNamespace(self_attn=attn, norm1=layer.attention_layernorm,
                                             norm2=layer.feedforward_layernorm, linear1=mlp[0], linear2=mlp[-1]))
         self.ws = Workspace(self.device)   # scratch shared by all calls (stream-ordered)
-        self.stack = TransformerStack(adapters, st, self.ws, d=d, heads=H, ff=ff, causal=False, act=ops.ACT_GELU_ERF,
-                                      prefix=prefix)
+        self.stack = TransformerStack(adapters, st, self.ws, d=d, heads=H, ff=ff, causal=False,
+                                      act=act_code(l0.feedforward.model[1]), prefix=prefix)
         self.layernorm, self.prefix = layernorm, prefix
         self.d, self.H, self.L = d, H, len(layers)
 
     def forward(self, X0: torch.Tensor, B: int, S: int, kmask: Optional[torch.Tensor], save: Workspace):
-        """Returns (LAST, XF, hidden_states): fp32 [B*S, d] each; LAST = layernorm(XF), XF = hidden_states[-1]."""
+        """Returns ((LAST, XF), save): fp32 [B*S, d] each; LAST = layernorm(XF), XF = hidden_states[-1].  The list of
+        hidden_states goes to `last_hidden`."""
         d, ln, pfx = self.d, self.layernorm, self.prefix
         M = B * S
         f32 = torch.float32
@@ -97,7 +89,8 @@ class FlavaTrainStack:
         hidden = [X0.view(B, S, d)]
         hidden += [save.bufs[f"{pfx}.XA.{l}"].view(B, S, d) for l in range(1, self.L)]
         hidden.append(XF.view(B, S, d))
-        return LAST, XF, hidden
+        self.last_hidden = hidden
+        return (LAST, XF), save
 
     def backward(self, save: Workspace, dLAST: Optional[torch.Tensor], dXF: Optional[torch.Tensor]) -> torch.Tensor:
         """Gradient w.r.t. X0 (fp32 [B*S, d], scratch: consume before the next backward of this encoder); parameter
@@ -106,6 +99,7 @@ class FlavaTrainStack:
         B, S = save.B, save.S
         M = B * S
         f32, bf = torch.float32, torch.bfloat16
+        dLAST, dXF = _f32c(dLAST, (M, d)), _f32c(dXF, (M, d))
         G = self.ws.get(f"{pfx}.G", (M, d), f32)
         Gb = self.ws.get(f"{pfx}.Gb", (M, d), bf)
         if dLAST is None:   # only hidden_states[-1] was used downstream: LayerNorm backward of a zero gradient
@@ -134,50 +128,19 @@ class FlavaImageTrainRuntime:
     def forward(self, data, diff):
         pixel_values, image_patches_mask = data
         emb, ts, st = self.mod.embeddings, self.ts, self.store
-        d = ts.d
         conv = emb.patch_embeddings.projection
-        ps = conv.weight.shape[2]
-        image = pixel_values.contiguous().float()
-        B, _, Hh, Ww = image.shape
-        P = (Hh // ps) * (Ww // ps)
-        S = P + 1
-        K = 3 * ps * ps
-        Kp = -(-K // 8) * 8
-        bf, f32 = torch.bfloat16, torch.float32
         st.refresh()
         save = Workspace(ts.device)
-        PATCH = save.get("fimg.PATCH", (B * P, Kp), bf)[:, :K]
-        PO = ts.ws.get("fimg.PO", (B * P, d), bf)
-        X0 = torch.empty((B * S, d), device=image.device, dtype=f32)
-        ops.im2col(image, ps, PATCH)
-        w = st.shadow2d(conv.weight)
-        if Kp != K:
-            wp = ts.ws.get("fimg.WCONV", (d, Kp), bf)[:, :K]
-            wp.copy_(w)
-            w = wp
-        ops.gemm(PATCH, w, bias=conv.bias, out=PO)
-        pm = None
-        if image_patches_mask is not None and emb.mask_token is not None:
-            pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
-        ops.vit_assemble_fwd(PO, emb.cls_token, emb.position_embeddings, emb.mask_token if pm is not None else None, pm, X0,
-                             B, S, d)
-        save.pm, save.P, save.K = pm, P, K
-        LAST, XF, hidden = ts.forward(X0, B, S, None, save)
-        return LAST, XF, hidden, save
+        X0, B, S, P, pm = patch_embed_fwd(pixel_values, conv, st.shadow2d(conv.weight), emb.cls_token,
+                                          emb.position_embeddings, emb.mask_token, image_patches_mask, ts.ws, save, "fimg")
+        save.pm, save.P = pm, P
+        return ts.forward(X0, B, S, None, save)
 
     def backward(self, save, dLAST, dXF):
-        emb, ts, st = self.mod.embeddings, self.ts, self.store
-        d, B, S, P, K = ts.d, save.B, save.S, save.P, save.K
-        conv = emb.patch_embeddings.projection
+        emb, ts = self.mod.embeddings, self.ts
         G = ts.backward(save, dLAST, dXF)
-        ops.batch_sum(G, st.grad(emb.position_embeddings), B, S * d, S * d)
-        ops.batch_sum(G, st.grad(emb.cls_token), B, S * d, d)
-        DP = ts.ws.get("fimg.DP", (B * P, d), torch.bfloat16)
-        ops.vit_assemble_bwd(G, save.pm, DP, st.grad(emb.mask_token) if save.pm is not None else None, B, S, d, True)
-        PATCH = save.get("fimg.PATCH", (B * P, -(-K // 8) * 8), torch.bfloat16)[:, :K]
-        ops.gemm(DP, PATCH, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad2d(conv.weight),
-                 splits=ops.wgrad_splits(d, PATCH.shape[1], B * P), accumulate=True)
-        ops.colsum_bf16(DP, st.grad(conv.bias), B * P, d, d)
+        patch_embed_bwd(G, emb.patch_embeddings.projection, emb.cls_token, emb.position_embeddings, emb.mask_token,
+                        save.pm, save.B, save.S, save.P, self.store, ts.ws, save, "fimg")
         return ()
 
 
@@ -212,8 +175,7 @@ class FlavaTextTrainRuntime:
                 raise NotImplementedError("only [batch, seq_len] padding masks are supported on the accelerated path")
             KM = (attention_mask != 0).to(torch.uint8).contiguous().view(-1)
         save.ids, save.tt, save.V = ids, tt, V
-        LAST, XF, hidden = ts.forward(X0, B, S, KM, save)
-        return LAST, XF, hidden, save
+        return ts.forward(X0, B, S, KM, save)
 
     def backward(self, save, dLAST, dXF):
         emb, ts, st = self.mod.embeddings, self.ts, self.store
@@ -275,8 +237,7 @@ class FlavaMMTrainRuntime:
             X0 = torch.empty((B * S, d), device=image_hidden.device, dtype=f32)
             ops.concat_tokens(cls, Pi, Pt, X0, B, Si, St, d)
             save.Si, save.St, save.di, save.dt = Si, St, di, dt
-        LAST, XF, hidden = ts.forward(X0, B, S, None, save)
-        return LAST, XF, hidden, save
+        return ts.forward(X0, B, S, None, save)
 
     def backward(self, save, dLAST, dXF):
         ts, st = self.ts, self.store
@@ -306,43 +267,10 @@ class FlavaMMTrainRuntime:
         return (outs[0].view(B, Si, save.di), outs[1].view(B, St, save.dt))
 
 
-class FlavaEncodeFunction(torch.autograd.Function):
-    """One training forward of a FLAVA encoder.  inputs: (runtime, data, n_diff, *diff_inputs, *parameters);
-    outputs: (last_hidden_state, hidden_states[-1]) as fp32 [B*S, d]."""
-
-    @staticmethod
-    def forward(ctx, rt, data, n_diff, *tensors):
-        diff = tensors[:n_diff]
-        ctx.set_materialize_grads(False)   # an unused output arrives as None in backward, not as a zero tensor
-        LAST, XF, hidden, save = rt.forward(data, diff)
-        rt.last_hidden = hidden
-        ctx.rt, ctx.save, ctx.n_diff, ctx.n_par = rt, save, n_diff, len(tensors) - n_diff
-        ctx.need = ctx.needs_input_grad[3 + n_diff:]
-        return LAST, XF
-
-    @staticmethod
-    def backward(ctx, dLAST, dXF):
-        rt, save = ctx.rt, ctx.save
-        if save is None:
-            raise MMBError("this encoder forward was already back-propagated (its activations are freed)")
-        st = rt.store
-        M = save.B * save.S
-        st.zero_grads()
-        in_grads = rt.backward(save, _f32c(dLAST, (M, -1)), _f32c(dXF, (M, -1)))
-        ctx.save = None
-        g = st.g.clone()
-        grads = []
-        for p, need in zip(st.params, ctx.need):
-            o = st.off[id(p)]
-            grads.append(g[o:o + p.numel()].view(p.shape) if need else None)
-        return (None, None, None, *in_grads, *grads)
-
-
 def run_encoder(rt, data, diff: Sequence[torch.Tensor] = ()):
     """-> (LAST [M,d], XF [M,d], hidden_states list) with LAST / XF attached to the autograd graph."""
-    LAST, XF = FlavaEncodeFunction.apply(rt, data, len(diff), *diff, *rt.store.params)
-    hidden = rt.last_hidden
-    rt.last_hidden = None
+    LAST, XF = run(rt, data, diff)
+    hidden, rt.ts.last_hidden = rt.ts.last_hidden, None
     return LAST, XF, hidden
 
 

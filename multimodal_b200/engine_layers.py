@@ -30,8 +30,7 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import Workspace
-from .engine_flava import _Shadows
+from .engine import Workspace, _Shadows, act_code, patch_embed_fwd
 
 
 def forward_only_guard(mod: nn.Module, what: str) -> None:
@@ -81,18 +80,6 @@ def _bool_mask_u8(mask: Optional[torch.Tensor], B: int, S: int, what: str) -> Op
     return mask.to(torch.uint8).contiguous()
 
 
-def _attention(rt: _Rt, QKV: torch.Tensor, O: torch.Tensor, B: int, S: int, H: int, hd: int, mask_u8, causal: bool):
-    d = H * hd
-    scale = 1.0 / math.sqrt(hd)
-    if mask_u8 is None and hd == 64 and (S <= 384 or S > ops.GENERIC_FWD_MAX_S):
-        ops.attention_fwd(QKV, O, None, B, S, H, causal, scale)
-    else:
-        ops.attention_fwd_generic(QKV[:, :d], QKV[:, d:2 * d], QKV[:, 2 * d:], O, B=B, Sq=S, Skv=S, H=H, head_dim=hd,
-                                  bsq=S * 3 * d, bsk=S * 3 * d, bsv=S * 3 * d, bso=S * d, scale=scale, mask=mask_u8,
-                                  mask_bs=S * S if mask_u8 is not None else 0, mask_qs=S if mask_u8 is not None else 0,
-                                  causal=causal)
-
-
 def _to_bf16_rows(rt: _Rt, x: torch.Tensor, name: str) -> torch.Tensor:
     xf = x.contiguous().float()
     out = rt.ws.get(name, (xf.numel() // xf.shape[-1], xf.shape[-1]), torch.bfloat16)
@@ -116,20 +103,11 @@ def mhsa_forward(mod: nn.Module, query: torch.Tensor, attn_mask: Optional[torch.
     QKV = rt.ws.get("mhsa.QKV", (B * S, 3 * d), bf)
     O = rt.ws.get("mhsa.O", (B * S, d), bf)
     ops.gemm(Xb, rt.sh.get("wqkv", [mod.input_proj.weight]), bias=mod.input_proj.bias, out=QKV)
-    _attention(rt, QKV, O, B, S, H, d // H, _bool_mask_u8(attn_mask, B, S, "MultiHeadSelfAttention"), bool(is_causal))
+    ops.self_attention(QKV, O, None, B, S, H, d // H, bool(is_causal), 1.0 / math.sqrt(d // H),
+                       mask=_bool_mask_u8(attn_mask, B, S, "MultiHeadSelfAttention"))
     out = torch.empty((B * S, d), device=query.device, dtype=torch.float32)
     ops.gemm(O, rt.sh.get("wo", [mod.output_proj.weight]), bias=mod.output_proj.bias, epilogue=ops.EPI_F32, out=out)
     return out.view(B, S, d).to(query.dtype)
-
-
-def _act_code(act: nn.Module) -> int:
-    from .modules.layers.activation import SiLU
-
-    if isinstance(act, nn.GELU) and getattr(act, "approximate", "none") == "none":
-        return ops.ACT_GELU_ERF
-    if isinstance(act, SiLU):
-        return ops.ACT_QUICK_GELU
-    raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU / SiLU)")
 
 
 def mlp_forward(mod: nn.Module, x: torch.Tensor) -> torch.Tensor:
@@ -140,7 +118,7 @@ def mlp_forward(mod: nn.Module, x: torch.Tensor) -> torch.Tensor:
     if len(seq) != 3 or not isinstance(seq[0], nn.Linear) or not isinstance(seq[2], nn.Linear):
         raise MMBError("standalone MLP supports the [Linear, activation, Linear] form (one hidden layer, no normalisation)")
     rt = _rt(mod, x.device)
-    act = _act_code(seq[1])
+    act = act_code(seq[1])
     Xb = _to_bf16_rows(rt, x, "mlp.X")
     M = Xb.shape[0]
     ff, dout = seq[0].weight.shape[0], seq[2].weight.shape[0]
@@ -174,7 +152,7 @@ def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
     ws, sh = rt.ws, rt.sh
     M = B * S
     bf, f32 = torch.bfloat16, torch.float32
-    act = _act_code(mlp[1])
+    act = act_code(mlp[1])
     ff = mlp[0].weight.shape[0]
     mask_u8 = _bool_mask_u8(attention_mask, B, S, "TransformerEncoderLayer")
     X = hidden_states.contiguous().float().view(M, d)
@@ -187,7 +165,7 @@ def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
     if mod.norm_first:
         ops.add_layernorm_fwd(X, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
         ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
-        _attention(rt, QKV, O, B, S, H, hd, mask_u8, False)
+        ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
         ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
         XM = ws.get("l.XM", (M, d), f32)                       # x + attention(LN(x)); LN2 of it for the MLP
         ops.add_layernorm_fwd(X, Y, XM, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
@@ -198,7 +176,7 @@ def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
     else:
         ops.cast_bf16(X.view(-1), LN.view(-1))                 # attention(x) on the raw input
         ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
-        _attention(rt, QKV, O, B, S, H, hd, mask_u8, False)
+        ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
         ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
         H1 = ws.get("l.H1", (M, d), f32)                       # LN1(x + attention(x)), fp32 + its bf16 operand copy
         ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
@@ -242,33 +220,14 @@ def patch_embeddings_forward(mod: nn.Module, image: torch.Tensor, image_patches_
     forward_only_guard(mod, "PatchEmbeddings")
     _cuda(image, "PatchEmbeddings")
     conv = mod.conv_projection
-    d, ps = conv.weight.shape[0], conv.weight.shape[2]
-    img = image.contiguous().float()
-    B, C, Hh, Ww = img.shape
+    C, Hh, Ww = image.shape[1:]
     if C != 3 or (Hh, Ww) != tuple(mod.image_size):
         raise ValueError(f"Input image shape {tuple(image.shape)} doesn't match the model's 3 x {mod.image_size}")
-    P = (Hh // ps) * (Ww // ps)
-    S = P + (1 if mod.include_cls_embed else 0)
-    K = 3 * ps * ps
-    Kp = -(-K // 8) * 8
     rt = _rt(mod, image.device)
-    ws, sh = rt.ws, rt.sh
-    bf = torch.bfloat16
-    PATCH = ws.get("pe.PATCH", (B * P, Kp), bf)[:, :K]
-    PO = ws.get("pe.PO", (B * P, d), bf)
-    ops.im2col(img, ps, PATCH)
-    w = sh.get("conv.w", [conv.weight.view(d, K)])
-    if Kp != K:
-        wp = ws.get("pe.WCONV", (d, Kp), bf)[:, :K]
-        wp.copy_(w)
-        w = wp
-    ops.gemm(PATCH, w, bias=conv.bias, out=PO)
-    pm = None
-    if image_patches_mask is not None and mod.mask_token is not None:
-        pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
-    X = torch.empty((B * S, d), device=image.device, dtype=torch.float32)
-    ops.vit_assemble_fwd(PO, mod.cls_token if mod.include_cls_embed else None, mod.position_embeddings,
-                         mod.mask_token if pm is not None else None, pm, X, B, S, d)
+    d = conv.weight.shape[0]
+    X, B, S, _, _ = patch_embed_fwd(image, conv, rt.sh.get("conv.w", [conv.weight.view(d, -1)]),
+                                    mod.cls_token if mod.include_cls_embed else None, mod.position_embeddings,
+                                    mod.mask_token, image_patches_mask, rt.ws, rt.ws, "pe")
     return PatchEmbeddingsOutput(embeddings=X.view(B, S, d).to(image.dtype))
 
 
@@ -422,7 +381,7 @@ def _decoder_layer(mod: nn.Module, X: torch.Tensor, B: int, S: int, ENC: Optiona
     M, d = X.shape
     bf, f32 = torch.bfloat16, torch.float32
     mlp = mod.feedforward.model
-    act = _act_code(mlp[1])
+    act = act_code(mlp[1])
     ff = mlp[0].weight.shape[0]
     LN, PRE, HACT = ws.get("d.LN", (M, d), bf), ws.get("d.PRE", (M, ff), bf), ws.get("d.HACT", (M, ff), bf)
     w1, w2 = sh.get("w1", [mlp[0].weight]), sh.get("w2", [mlp[-1].weight])

@@ -97,7 +97,7 @@ class CoCaModel(nn.Module):
 
     def _vision_proj(self, x: Tensor) -> Tensor:
         """self.vision_proj(x) for x [B, 1, d] or [B, d] (coca_model.py:115) as a wgmma GEMM, fp32 out."""
-        from ...engine_flava import _Shadows
+        from ...engine import _Shadows
 
         if torch.is_grad_enabled() and (x.requires_grad or self.vision_proj.weight.requires_grad):
             from ...engine_coca_train import linear_f32

@@ -41,14 +41,14 @@ class CoCaMultimodalDecoder(_RuntimeOwner):
             return self._runtime().forward(texts, images)
 
     def wants_graph(self, texts: Tensor, images: Tensor) -> bool:
-        from ... import engine_coca_train as T
-        return T.wants_grad(self) or (torch.is_grad_enabled() and (texts.requires_grad or images.requires_grad))
+        from ...engine import wants_grad
+        return wants_grad(self) or (torch.is_grad_enabled() and (texts.requires_grad or images.requires_grad))
 
     def hidden_states(self, texts: Tensor, images: Tensor) -> Tensor:
         """Training path: the decoder output after its final LayerNorm, [B, S, d] with autograd history (the vocabulary
         projection is applied by the caller: `forward`, or fused with the cross-entropy in CoCaForPretraining)."""
-        from ... import engine_coca_train as T
-        (out,) = T.run(self._train_runtime(), None, (texts, images))
+        from ...engine import run
+        (out,) = run(self._train_runtime(), None, (texts, images))
         return out.view(texts.shape[0], texts.shape[1], -1)
 
 

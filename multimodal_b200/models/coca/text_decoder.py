@@ -96,9 +96,9 @@ class CoCaTextDecoder(_RuntimeOwner):
         mask_u8 = None
         if mask.dim() == 4:   # [B, 1, S, S] (batch-dependent); a bare causal_mask runs as the kernels' causal flag
             mask_u8 = (mask[:, 0] != 0).to(torch.uint8).contiguous()
-        from ... import engine_coca_train as T
-        if T.wants_grad(self):
-            pooled, XF = T.run(self._train_runtime(), (input_ids, mask_u8, S), ())
+        from ...engine import run, wants_grad
+        if wants_grad(self):
+            pooled, XF = run(self._train_runtime(), (input_ids, mask_u8, S), ())
             B = input_ids.shape[0]
             return pooled, XF.view(B, S, -1)[:, :-1]       # tokens: every row but the appended CLS one (:190-191)
         with torch.no_grad():

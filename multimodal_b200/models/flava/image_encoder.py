@@ -79,7 +79,8 @@ class ImageTransformer(_RuntimeOwner):
         if image_patches_mask is not None and self.embeddings.mask_token is None:
             warnings.warn("image_patches_mask passed but use_image_masking in init was false. Ignoring.")
         from ... import engine_flava_train as T
-        if T.wants_grad(self):   # training: forward keeps activations, autograd nodes carry the explicit backward
+        from ...engine import wants_grad
+        if wants_grad(self):   # training: forward keeps activations, autograd nodes carry the explicit backward
             if getattr(self, "output_attentions", False):
                 raise NotImplementedError("attention probabilities are not produced by the training forward")
             return T.encoder_output(self._train_runtime(), (pixel_values, image_patches_mask), (), self.pooler)

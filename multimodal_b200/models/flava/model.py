@@ -145,7 +145,8 @@ class FLAVAModel(nn.Module):
     @staticmethod
     def _project_cls(encoder: nn.Module, out: TransformerOutput, linear: nn.Module, key: str) -> Tensor:
         from ... import engine_flava_train as T
-        if torch.is_grad_enabled() and (out.last_hidden_state.requires_grad or T.wants_grad(linear)):
+        from ...engine import wants_grad
+        if torch.is_grad_enabled() and (out.last_hidden_state.requires_grad or wants_grad(linear)):
             return T.first_token_linear(out.last_hidden_state, linear)
         with torch.no_grad():
             return encoder._runtime().stack.project_first_token(out.last_hidden_state, linear, key)
@@ -161,8 +162,9 @@ class FLAVAModel(nn.Module):
         if image_embedding is None or text_embedding is None:
             return TransformerOutput()
         from ... import engine_flava_train as T
+        from ...engine import wants_grad
         enc, ip, tp = self.mm_encoder, self.image_to_mm_projection, self.text_to_mm_projection
-        if T.wants_grad(enc, ip, tp) or (torch.is_grad_enabled() and
+        if wants_grad(enc, ip, tp) or (torch.is_grad_enabled() and
                                           (image_embedding.requires_grad or text_embedding.requires_grad)):
             return T.encoder_output(enc._train_runtime(ip, tp), None, (image_embedding, text_embedding), enc.pooler)
         with torch.no_grad():

@@ -117,7 +117,8 @@ class FLAVATransformerWithoutEmbeddings(_RuntimeOwner):
         if attention_mask is not None:
             raise NotImplementedError("attention_mask on the multimodal encoder is not on the accelerated path")
         from ... import engine_flava_train as T
-        if T.wants_grad(self) or (torch.is_grad_enabled() and hidden_states.requires_grad):
+        from ...engine import wants_grad
+        if wants_grad(self) or (torch.is_grad_enabled() and hidden_states.requires_grad):
             return T.encoder_output(self._train_runtime(None, None), None, (hidden_states,), self.pooler)
         with torch.no_grad():
             return self._runtime().forward(hidden_states, want_attn=bool(getattr(self, "output_attentions", False)))

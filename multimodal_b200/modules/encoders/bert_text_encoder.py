@@ -38,7 +38,8 @@ class BERTTextEncoder(_RuntimeOwner):
         if self.layernorm is None:
             raise NotImplementedError("BERTTextEncoder without a final layernorm is not on the accelerated path")
         from ... import engine_flava_train as T
-        if T.wants_grad(self):   # training: forward keeps activations, autograd nodes carry the explicit backward
+        from ...engine import wants_grad
+        if wants_grad(self):   # training: forward keeps activations, autograd nodes carry the explicit backward
             if return_attn_weights:
                 raise NotImplementedError("attention probabilities are not produced by the training forward")
             out = T.encoder_output(self._train_runtime(), (input_ids, attention_mask, token_type_ids), (), self.pooler)

@@ -34,10 +34,10 @@ class VisionTransformer(_RuntimeOwner):
                 {emb.image_size[0]}*{emb.image_size[1]} expected by model")
         if image_patches_mask is not None and emb.mask_token is None:
             warnings.warn("image_patches_mask passed but use_image_masking in init was false. Ignoring.")
-        from ... import engine_coca_train as T
-        if T.wants_grad(self):   # training: forward keeps activations, the autograd node carries the explicit backward
+        from ...engine import run, wants_grad
+        if wants_grad(self):   # training: forward keeps activations, the autograd node carries the explicit backward
             rt = self._train_runtime()
-            (last,) = T.run(rt, (images, image_patches_mask), ())
+            (last,) = run(rt, (images, image_patches_mask), ())
             hidden, rt.last_hidden = rt.last_hidden, None
             B, S, d = hidden[0].shape
             out = TransformerOutput(last_hidden_state=last.view(B, S, d), pooler_output=None, hidden_states=hidden,

@@ -23,9 +23,9 @@ class AttentionPooler(_RuntimeOwner):
         self.ln_post = nn.LayerNorm(output_embed_dim, layer_norm_eps)
 
     def forward(self, x: Tensor) -> Tensor:
-        from ... import engine_coca_train as T
-        if T.wants_grad(self) or (torch.is_grad_enabled() and x.requires_grad):
-            (out,) = T.run(self._train_runtime(), None, (x,))
+        from ...engine import run, wants_grad
+        if wants_grad(self) or (torch.is_grad_enabled() and x.requires_grad):
+            (out,) = run(self._train_runtime(), None, (x,))
             return out.view(x.shape[0], self.query.shape[0], self.query.shape[1])
         with torch.no_grad():
             return self._runtime().forward(x)

@@ -430,11 +430,36 @@ def coca_text_embed_fwd(ids, emb, cls, pos, x, B, S, d, V):
                "mmb_coca_text_embed_fwd")
 
 
-# Longest self-attention (Sq = Skv) the generic forward keeps resident at head_dim 64: its Q, K and V tiles (144 B per
-# row, keys padded to 64) fit in the 227 KB of shared memory an H100 CTA can opt into.  Longer shapes run the generic
-# entry points' K / V-streamed kernels (any length); unmasked head_dim-64 self-attention above this length goes to
-# attention_fwd instead, whose streamed kernel is the same one the CLIP towers use.
-GENERIC_FWD_MAX_S = 512
+def self_attention(qkv, out, lse, B, S, H, head_dim, causal, scale, *, kmask=None, mask=None, dout=None, dqkv=None):
+    """Self-attention on a packed [B*S, 3*H*head_dim] QKV buffer: the forward, or with dout / dqkv its backward.  The
+    one place that picks the kernel, so a forward and its backward, in any grad mode, always run the same one:
+      kmask (uint8 [B*S] key-padding mask)      -> the key-masked fused kernels (head_dim 64 only);
+      mask (uint8 [B, S, S]) or head_dim != 64  -> the general kernels (lse unused);
+      otherwise                                 -> the fused kernels."""
+    if kmask is not None and mask is not None:
+        raise MMBError("self_attention: pass either a key-padding mask or a [B, S, S] mask, not both")
+    if kmask is not None and head_dim != 64:
+        raise MMBError(f"self_attention: the key-padding-mask kernels support head_dim 64 only (got {head_dim}); "
+                       "pass the mask as a [B, S, S] mask instead")
+    if kmask is not None:
+        if dout is None:
+            attention_fwd_kmask(qkv, out, lse, kmask, B, S, H, causal, scale)
+        else:
+            attention_bwd_kmask(qkv, out, dout, lse, dqkv, kmask, B, S, H, causal, scale)
+    elif mask is not None or head_dim != 64:
+        d = H * head_dim
+        kw = dict(B=B, Sq=S, Skv=S, H=H, head_dim=head_dim, bsq=S * 3 * d, bsk=S * 3 * d, bsv=S * 3 * d, bso=S * d,
+                  scale=scale, mask=mask, mask_bs=S * S if mask is not None else 0,
+                  mask_qs=S if mask is not None else 0, causal=causal)
+        if dout is None:
+            attention_fwd_generic(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], out, **kw)
+        else:
+            attention_bwd_generic(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], dout, dqkv[:, d:2 * d], dqkv[:, 2 * d:],
+                                  dq=dqkv[:, :d], **kw)
+    elif dout is None:
+        attention_fwd(qkv, out, lse, B, S, H, causal, scale)
+    else:
+        attention_bwd(qkv, out, dout, lse, dqkv, B, S, H, causal, scale)
 
 
 def attention_fwd_generic(q, k, v, out, *, B, Sq, Skv, H, head_dim, bsq, bsk, bsv, bso, scale, mask=None, mask_bs=0,
