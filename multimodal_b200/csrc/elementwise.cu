@@ -965,6 +965,7 @@ extern "C" int mmb_vit_embed_ln_bwd(const void* patch_out, const float* cls, con
 
 extern "C" int mmb_batch_sum(const float* in, float* out, int Bn, long long ld, int n, void* stream) {
   if (n & 3) return MMB_ERR_ARG;
+  if (n <= 0 || Bn <= 0) return MMB_OK;   // empty sum: out is unchanged (the chunking below divides by both)
   const int bx = (n / 4 + 127) / 128;
   int chunks = (num_sms() * 4 + bx - 1) / bx;
   if (chunks > Bn) chunks = Bn;
@@ -980,6 +981,7 @@ extern "C" int mmb_batch_sum(const float* in, float* out, int Bn, long long ld, 
 
 extern "C" int mmb_colsum_bf16(const void* x, float* out, int M, int N, long long ld, void* stream) {
   if ((N & 7) || (ld & 7)) return MMB_ERR_ARG;
+  if (M <= 0 || N <= 0) return MMB_OK;   // empty sum: out is unchanged (the chunking below divides by both)
   const int bx = (N + 255) / 256;
   int chunks = (num_sms() * 6 + bx - 1) / bx;
   int rows_per_block = (M + chunks - 1) / chunks;

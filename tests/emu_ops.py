@@ -233,9 +233,12 @@ def concat_tokens(cls, a, b, out, B, Sa, Sb, d):
     parts = []
     if cls is not None:
         parts.append(cls.detach().view(1, 1, d).expand(B, 1, d))
-    parts.append(a.detach().reshape(B, -1, d)[:, :Sa])
+    # the kernel reads a and b as compact [B*Sa, d] / [B*Sb, d] rows (b is not read when Sb == 0)
+    assert a.is_contiguous() and a.numel() == B * Sa * d, (tuple(a.shape), B, Sa, d)
+    parts.append(a.detach().view(B, Sa, d))
     if Sb:
-        parts.append(b.detach().reshape(B, Sb, d))
+        assert b.is_contiguous() and b.numel() == B * Sb * d, (tuple(b.shape), B, Sb, d)
+        parts.append(b.detach().view(B, Sb, d))
     out.view(B, -1, d).copy_(torch.cat(parts, 1))
 
 
@@ -276,7 +279,8 @@ def gather_rows_idx_cast(x, idx, out, d):
 
 
 def scatter_rows_idx_add(src, idx, dst, d):
-    dst.view(-1, d).index_add_(0, idx, src)
+    rows = int(idx.max().item()) + 1 if idx.numel() else 0
+    torch.as_strided(dst, (rows, d), (dst.stride(-2), 1)).index_add_(0, idx, src)
 
 
 def ce_labels(logits, labels, label_stride, ignore_index, M, V, row_loss, accum):
@@ -307,6 +311,15 @@ def act_bwd(dy, pre, dx, kind):
 def cast_f32(src, out):
     out.copy_(src.float())
     return out
+
+
+def act_fwd(x, kind):
+    return _act(x.detach(), kind)
+
+
+def sum_scale(inp, n, scale, out, accumulate=False):
+    s = inp.detach().reshape(-1)[:n].sum() * scale
+    out.view(-1)[:1].copy_((out.view(-1)[0] + s if accumulate else s).view(1))
 
 
 def matmul_f32(A, B, *, ta=False, tb=False, out=None, alpha=1.0, accumulate=False):

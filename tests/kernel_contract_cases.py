@@ -1,0 +1,1382 @@
+"""Contract checks of the HBM-bound kernels (casts, im2col, token assembly, LayerNorm, embeddings, L2 norm, activations,
+gathers / scatters, losses, the key / value cache) and of every other kernel the CPU emulation restates, each against a
+float64 reference written from include/mmb200.h.
+
+``check_<op>(impl, device, case)`` builds the inputs of one shape case on the CPU from a fixed seed, moves them to
+`device`, calls ``impl.<op>`` and compares the results with the float64 reference.  `impl` is ``multimodal_b200.ops``
+(device cuda) or the CPU emulation of tests/emu_ops.py + tests/emu_decode_ops.py (device cpu), so the same check proves
+the kernel and the emulation that the CPU schedule tests trust.  Inputs the kernel reads as bf16 are bf16 before the
+reference is formed.  The references never call the emulation.
+
+Tolerance classes (each check returns its compared outputs as ``{name: Rec}`` so that two implementations can be held
+against each other under the same class):
+  exact  bit-exact (NaN compared by position): casts, im2col, gathers / assembly / concat / split, scatter_rows_add,
+         kv_cache_append, argmax_tokens, kmask_out.  Each rounds at most once or adds once in fp32.
+  bf16   bf16 outputs of fp32 math: at most 1 bf16 ulp from bf16(ref64) and at least `min_equal` (99 %) of the elements
+         equal to it, which catches round-toward-zero where a relative bar does not.
+  bound  fp32 results: |got - ref64| <= bound, elementwise.  For reductions the bound is k * 2^-24 * sum|terms| with k
+         the length of the kernel's longest summation chain (plus the roundings of the terms), derived in each check.
+  rel    GEMM / attention outputs with bf16 operands inside the kernel: max|got - ref| <= tol * max|ref|.
+Accumulating outputs (colsum, batch_sum, dgamma / dbeta / gsum, ce accum, dmask_token, the embedding tables) start
+from non-zero buffers, so `+=` is checked rather than `=`.
+
+CASES maps every checked op to its shape cases.  A case with ``"gpu": True`` is sized for the GPU (grid caps, real
+vocabularies) and is skipped by the CPU run of the emulation.
+"""
+import math
+
+import torch
+
+U = 2.0 ** -24          # unit roundoff of fp32
+F32, BF, F64 = torch.float32, torch.bfloat16, torch.float64
+H100_SMS = 132          # SM count assumed for the chain lengths when no GPU is present (H100 SXM)
+
+
+# ---- reference helpers ---------------------------------------------------------------------------------------------
+def rne_bf16(x: torch.Tensor) -> torch.Tensor:
+    """fp32 -> bf16, round to nearest even on the bit pattern (written out, not torch's cast); NaN stays NaN."""
+    x = x.to(F32).contiguous()
+    b = x.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    r = ((b + 0x7FFF + ((b >> 16) & 1)) >> 16) & 0xFFFF
+    r = torch.where(torch.isnan(x), torch.full_like(r, 0x7FC0), r)
+    r = torch.where(r >= 0x8000, r - 0x10000, r).to(torch.int16)
+    return r.view(BF)
+
+
+def d64(t: torch.Tensor) -> torch.Tensor:
+    return t.detach().cpu().to(F32).to(F64)
+
+
+def _sms(device) -> int:
+    dev = torch.device(device)
+    if dev.type == "cuda":
+        return torch.cuda.get_device_properties(dev).multi_processor_count
+    return H100_SMS
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def _gen(case):
+    return torch.Generator().manual_seed(1000 + case.get("seed", 0))
+
+
+def _ord16(t):
+    i = t.contiguous().view(torch.int16).to(torch.int32) & 0xFFFF
+    return torch.where(i >= 0x8000, -(i & 0x7FFF), i)
+
+
+def _bits(t):
+    if t.dtype == F32:
+        return t.contiguous().view(torch.int32)
+    if t.dtype == BF:
+        return t.contiguous().view(torch.int16)
+    return t
+
+
+class Rec:
+    """One compared output: the value (on the CPU), its class and the class's parameter; `ratio` is the largest
+    |got - ref| / bound seen (bound class only)."""
+
+    def __init__(self, kind, got, param=None, ratio=0.0):
+        self.kind, self.got, self.param, self.ratio = kind, got, param, ratio
+
+
+def assert_exact(name, got, ref):
+    assert got.shape == ref.shape and got.dtype == ref.dtype, (name, got.shape, got.dtype, ref.shape, ref.dtype)
+    if got.is_floating_point():
+        gn, rn = torch.isnan(got.float()), torch.isnan(ref.float())
+        assert torch.equal(gn, rn), f"{name}: NaN positions differ"
+        bad = (_bits(got) != _bits(ref)) & ~gn
+    else:
+        bad = got != ref
+    if bad.any():
+        i = bad.nonzero()[0].tolist()
+        raise AssertionError(f"{name}: {int(bad.sum())} of {bad.numel()} elements differ, first at {i}: "
+                             f"got {got[tuple(i)].item()!r}, want {ref[tuple(i)].item()!r}")
+
+
+def assert_bf16(name, got, ref64, min_equal=0.99, err=None):
+    """At most 1 bf16 ulp from bf16(ref64), and at least `min_equal` of the elements equal to it.  err (optional): an
+    elementwise bound of the fp32 value's own error before the rounding; where it spans more than a bf16 ulp (a result
+    formed by cancellation) the element may instead lie anywhere within 1 ulp of [bf16(ref - err), bf16(ref + err)],
+    and it does not count towards the equal fraction."""
+    ref = rne_bf16(ref64.to(F32))
+    assert got.dtype == BF and got.shape == ref.shape, (name, got.dtype, got.shape, ref.shape)
+    assert torch.equal(torch.isnan(got.float()), torch.isnan(ref.float())), f"{name}: NaN positions differ"
+    og = _ord16(got)
+    dist = (og - _ord16(ref)).abs()
+    ok = dist <= 1
+    counted = torch.ones_like(ok)
+    if err is not None:
+        lo, hi = _ord16(rne_bf16((ref64 - err).to(F32))), _ord16(rne_bf16((ref64 + err).to(F32)))
+        ok = ok | ((og >= lo - 1) & (og <= hi + 1))
+        counted = lo == hi          # the fraction counts the elements whose fp32 value resolves to one bf16 value
+    eq = (dist[counted] == 0).float().mean().item() if counted.any() else 1.0
+    assert bool(ok.all()), \
+        f"{name}: {int((~ok).sum())} elements more than 1 bf16 ulp from the reference (max {dist[~ok].max().item()})"
+    assert eq >= min_equal, f"{name}: only {eq:.4f} of the elements equal bf16(ref64) (need {min_equal})"
+    return eq
+
+
+def assert_bound(name, got, ref64, bound):
+    err = (got.detach().cpu().to(F64) - ref64).abs()
+    bound = torch.as_tensor(bound, dtype=F64).expand_as(ref64)
+    bad = ~(err <= bound)
+    if bad.any():
+        i = bad.nonzero()[0].tolist()
+        raise AssertionError(f"{name}: {int(bad.sum())} of {bad.numel()} elements outside the bound, first at {i}: "
+                             f"got {got.cpu()[tuple(i)].item()!r}, "
+                             f"ref {ref64[tuple(i)].item()!r}, bound {bound[tuple(i)].item():.3e}")
+    pos = bound > 0
+    return (err[pos] / bound[pos]).max().item() if pos.any() else 0.0
+
+
+def assert_rel(name, got, ref64, tol):
+    err = (got.detach().cpu().to(F64) - ref64).abs().max().item()
+    scale = ref64.abs().max().item()
+    assert err <= tol * scale, f"{name}: max error {err:.3e} > {tol} * max|ref| {scale:.3e}"
+    return err / scale if scale else 0.0
+
+
+class _Out:
+    def __init__(self, op=None):
+        self.op, self.rec = op, {}
+
+    def exact(self, name, got, ref):
+        got = got.detach().cpu()
+        assert_exact(name, got, ref)
+        self.rec[name] = Rec("exact", got)
+
+    def bf16(self, name, got, ref64, min_equal=0.99, err=None):
+        got = got.detach().cpu()
+        eq = assert_bf16(name, got, ref64, min_equal, err)
+        self.rec[name] = Rec("bf16", got, (min_equal, err), 1.0 - eq)
+
+    def bound(self, name, got, ref64, bound):
+        got = got.detach().cpu()
+        bound = TIGHTENED.get(f"{self.op}.{name}", 1.0) * torch.as_tensor(bound, dtype=F64)
+        r = assert_bound(name, got, ref64, bound)
+        self.rec[name] = Rec("bound", got, torch.as_tensor(bound, dtype=F64).expand_as(ref64).clone(), r)
+
+    def rel(self, name, got, ref64, tol):
+        got = got.detach().cpu()
+        r = assert_rel(name, got, ref64, tol)
+        self.rec[name] = Rec("rel", got, (tol, ref64.abs().max().item()), r)
+
+
+def compare_recs(name, a: Rec, b: Rec, slack=0.0):
+    """Holds two implementations' results of the same check against each other under the output's class.  slack widens
+    a bound where the output sums another compared output that may legitimately differ (gsum over g_bf16)."""
+    assert a.kind == b.kind
+    if a.kind == "exact":
+        assert_exact(name, a.got, b.got)
+    elif a.kind == "bf16":
+        min_equal, err = a.param
+        assert_bf16(name, a.got, b.got.to(F64), min_equal, None if err is None else 2 * err)
+    elif a.kind == "bound":   # both lie within the bound of the same reference
+        assert_bound(name, a.got, b.got.to(F64), 2 * a.param + slack)
+    else:
+        tol, scale = a.param
+        err = (a.got.to(F64) - b.got.to(F64)).abs().max().item()
+        assert err <= 2 * tol * scale, f"{name}: implementations differ by {err:.3e} > 2 * {tol} * {scale:.3e}"
+
+
+# Bounds tightened from measurement: where the largest |got - ref| / bound over every case, measured on an H100 80GB HBM3
+# (132 SMs) for the kernel and on the CPU for the emulation, was far below the derived k * 2^-24 * sum|terms| bound, the
+# bar is about 3x the larger of the two measured maxima (factor applied to the derived bound).  Every other bound is the
+# derived one.
+TIGHTENED = {
+    "sum_scale.out": 0.01,                   # measured 0.0027 (kernel and emulation: the final rounding only)
+    "gemm.D": 0.04,                          # EPI_F32 accumulate: 0.013 kernel, 0.012 emulation
+    "colsum_bf16.out": 0.11,                 # 0.036 / 0.036
+    "ce_labels.accum": 0.11,                 # 0.036 / 0.036
+    "layernorm_bwd.gsum": 0.28,              # 0.091 / 0.091
+    "vit_embed_ln_fwd.mean": 0.11,           # 0.034 / 0.026
+    "vit_assemble_bwd.dmask_token": 0.17,    # 0.054 / 0.054
+    "bert_embed_ln_bwd.dgamma": 0.11,        # 0.034 / 0.034
+    "bert_embed_ln_bwd.dbeta": 0.27,         # 0.089 / 0.067
+    "bert_embed_ln_bwd.dpos": 0.2,           # 0.065 / 0.062
+    "bert_embed_ln_bwd.dtype": 0.1,          # 0.033 / 0.024
+}
+
+
+# ---- special values --------------------------------------------------------------------------------------------------
+_F32_SPECIAL_BITS = [
+    0x00000000, 0x80000000,                  # +-0
+    0x00000001, 0x80000001, 0x00008000,      # smallest subnormals, a subnormal tie (-> 0, even)
+    0x00018000, 0x007FFFFF, 0x807FFFFF,      # subnormal tie (-> up), largest subnormal (-> smallest normal)
+    0x7F800000, 0xFF800000,                  # +-inf
+    0x7FC00000, 0xFFC00001, 0x7F800001,      # NaNs (quiet, negative quiet, signalling)
+    0x7F7F8000, 0xFF7F8000, 0x7F7FFFFF,      # ties at the top (-> +-inf), FLT_MAX (-> inf)
+    0x7F7F7FFF,                              # just below the tie (-> bf16 max)
+    0x3F808000, 0x3F818000, 0x3F808001, 0x3F807FFF,   # 1 + 2^-8 tie (-> 1), tie (-> up), above / below a tie
+]
+
+
+def f32_specials():
+    b = torch.tensor([v - (1 << 32) if v >= 1 << 31 else v for v in _F32_SPECIAL_BITS], dtype=torch.int32)
+    return b.view(F32)
+
+
+def _with_specials(x, sp):
+    k = min(len(sp), x.numel())
+    x = x.clone()
+    x.view(-1)[:k] = sp[:k]
+    return x
+
+
+ACT_SPECIALS = torch.tensor([10.0, -10.0, 0.0, -0.0, 3.0, -3.0, 1.0, -1.0], dtype=F32)
+
+
+# ---- casts -------------------------------------------------------------------------------------------------------------
+def check_cast_bf16(impl, device, case):
+    o = _Out("cast_bf16")
+    n = case["n"]
+    x = _with_specials(torch.randn(n, generator=_gen(case)) * 3, f32_specials())
+    out = torch.empty(n, dtype=BF, device=device)
+    impl.cast_bf16(x.to(device, copy=True), out)
+    o.exact("out", out, rne_bf16(x))
+    return o.rec
+
+
+def check_cast_f32(impl, device, case):
+    """Every bf16 bit pattern but one (an odd count exercises the scalar tail), in a shuffled order."""
+    o = _Out("cast_f32")
+    n = case["n"]
+    bits = torch.arange(-32768, 32767, dtype=torch.int32)
+    bits = bits[torch.randperm(bits.numel(), generator=_gen(case))][:n]
+    src = bits.to(torch.int16).view(BF)
+    out = torch.empty(n, dtype=F32, device=device)
+    impl.cast_f32(src.to(device, copy=True), out)
+    o.exact("out", out, (bits << 16).view(F32))
+    return o.rec
+
+
+# ---- patch im2col --------------------------------------------------------------------------------------------------------
+def check_im2col(impl, device, case):
+    o = _Out("im2col")
+    B, H, W, ps, ld = case["B"], case["H"], case["W"], case["ps"], case["ld"]
+    K, gh, gw = 3 * ps * ps, H // ps, W // ps
+    img = torch.randn(B, 3, H, W, generator=_gen(case))
+    buf = torch.full((B * gh * gw, ld), -7.0, dtype=BF, device=device)
+    impl.im2col(img.to(device, copy=True), ps, buf[:, :K])
+    ref = img.view(B, 3, gh, ps, gw, ps).permute(0, 2, 4, 1, 3, 5).reshape(B * gh * gw, K)
+    got = buf.cpu()
+    o.exact("out", got[:, :K], rne_bf16(ref))
+    o.exact("pad", got[:, K:], torch.full((B * gh * gw, ld - K), -7.0, dtype=BF))
+    return o.rec
+
+
+# ---- LayerNorm -------------------------------------------------------------------------------------------------------
+def _ln_ref(x64, gamma64, beta64, eps):
+    mu = x64.mean(-1, keepdim=True)
+    var = ((x64 - mu) ** 2).mean(-1, keepdim=True)
+    rstd = 1.0 / torch.sqrt(var + eps)
+    h = (x64 - mu) * rstd
+    return h * gamma64 + beta64, mu.squeeze(-1), rstd.squeeze(-1), h
+
+
+def _ln_fwd_bounds(x64, gamma64, beta64, eps, nv, in_err=None):
+    """Bounds of the warp-per-row forward (ln_stats): mean = (sum of 4*nv values per lane, 5 shuffle levels) / d;
+    var the same over squared deviations; rstd = rsqrtf(var + eps); out = (x - mean) * rstd * gamma + beta.
+    in_err: elementwise absolute error of the kernel's input relative to x64 (fp32 sums formed in the kernel)."""
+    out, mu, rstd, h = _ln_ref(x64, gamma64, beta64, eps)
+    d = x64.shape[-1]
+    k_mean = 4 * nv + 5 + 1
+    k_var = 4 * nv + 5 + 3
+    ax = x64.abs().mean(-1, keepdim=True)
+    b_mean = k_mean * U * ax.squeeze(-1)
+    b_rstd = (k_var / 2 + 3) * U * rstd
+    g = gamma64.abs()
+    b_out = U * (g * h.abs() * (k_var / 2 + 6) + k_mean * g * ax * rstd[:, None] + out.abs() + beta64.abs())
+    if in_err is not None:
+        me = in_err.mean(-1, keepdim=True)
+        b_mean = b_mean + me.squeeze(-1)
+        b_rstd = b_rstd + rstd * (h.abs() * in_err).mean(-1) * rstd
+        b_out = b_out + g * rstd[:, None] * (in_err + me + h.abs() * (h.abs() * in_err).mean(-1, keepdim=True))
+    return out, mu, rstd, b_out, b_mean, b_rstd
+
+
+def check_add_layernorm_fwd(impl, device, case):
+    o = _Out("add_layernorm_fwd")
+    g = _gen(case)
+    M, d, eps = case["M"], case["d"], 1e-5
+    rpg, gather = case.get("rpg", 0), case.get("gather")
+    R = M * rpg if rpg else M
+    x = torch.randn(R, d, generator=g) * 2 + 0.5
+    y = (torch.randn(R, d, generator=g) * 2).to(BF)
+    gamma, beta = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    use_x, use_y = case.get("x", True), case.get("y", True)
+    row_idx = torch.randint(0, max(rpg, 1), (M,), generator=g, dtype=torch.int32) if gather == "idx" else None
+    tod = lambda t: None if t is None else t.to(device, copy=True)  # noqa: E731
+    x_out = torch.full((M, d), 9.0, device=device)
+    ln_bf16 = torch.empty(M, d, dtype=BF, device=device)
+    ln_f32 = torch.empty(M, d, device=device)
+    mean, rstd = torch.empty(M, device=device), torch.empty(M, device=device)
+    impl.add_layernorm_fwd(tod(x) if use_x else None, tod(y) if use_y else None, x_out, ln_bf16, ln_f32, tod(gamma),
+                           tod(beta), mean, rstd, M, d, eps, row_idx=tod(row_idx), rows_per_group=rpg)
+    phys = torch.arange(M) * rpg + (row_idx.long() if row_idx is not None else 0) if rpg else torch.arange(M)
+    xs = torch.zeros(M, d, dtype=F64)
+    if use_x:
+        xs = xs + d64(x)[phys]
+    if use_y:
+        xs = xs + d64(y)[phys]
+    xr = xs.to(F32)                      # x_out: one fp32 add; the LayerNorm normalises the stored sum
+    o.exact("x_out", x_out, xr)
+    out, mu, rs, b_out, b_mean, b_rstd = _ln_fwd_bounds(xr.to(F64), d64(gamma), d64(beta), eps, d // 128)
+    o.bound("mean", mean, mu, b_mean)
+    o.bound("rstd", rstd, rs, b_rstd)
+    o.bound("ln_f32", ln_f32, out, b_out)
+    o.bf16("ln_bf16", ln_bf16, out, err=b_out)
+    return o.rec
+
+
+def check_vit_embed_ln_fwd(impl, device, case):
+    o = _Out("vit_embed_ln_fwd")
+    g = _gen(case)
+    B, S, d, eps = case["B"], case["S"], case["d"], 1e-5
+    patch = (torch.randn(B * (S - 1), d, generator=g) * 2).to(BF)
+    cls, pos = torch.randn(d, generator=g), torch.randn(S, d, generator=g) * 0.5
+    gamma, beta = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    x0 = torch.empty(B * S, d, device=device)
+    mean, rstd = torch.empty(B * S, device=device), torch.empty(B * S, device=device)
+    impl.vit_embed_ln_fwd(patch.to(device, copy=True), cls.to(device, copy=True), pos.to(device, copy=True), gamma.to(device, copy=True), beta.to(device, copy=True), x0, mean,
+                          rstd, B, S, d, eps)
+    t = torch.cat([d64(cls).view(1, 1, d).expand(B, 1, d), d64(patch).view(B, S - 1, d)], 1) + d64(pos).view(1, S, d)
+    t = t.reshape(B * S, d)
+    out, mu, rs, b_out, b_mean, b_rstd = _ln_fwd_bounds(t, d64(gamma), d64(beta), eps, d // 128, in_err=U * t.abs())
+    o.bound("mean", mean, mu, b_mean)
+    o.bound("rstd", rstd, rs, b_rstd)
+    o.bound("x0", x0, out, b_out)
+    return o.rec
+
+
+def _ln_bwd_grid(M, d, sms):
+    nv = d // 128
+    per_sm = min(1536 // (nv * 32), 24)
+    return min(sms * per_sm, M)
+
+
+def _ln_bwd_ref(x64, dy64, mean64, rstd64, gamma64, nv):
+    """dx of the one-CTA-per-row backward and its bound.  h = (x - mean) * rstd (2 roundings), dyg = dy * gamma (1),
+    s1 / s2 = row sums over 4 (thread) + 5 (shuffle) + nv (cross-warp) terms, / d;
+    dx = rstd * (dyg - s1 - h * s2) (+ g_in)."""
+    d = x64.shape[-1]
+    h = (x64 - mean64[:, None]) * rstd64[:, None]
+    dyg = dy64 * gamma64
+    s1 = dyg.mean(-1, keepdim=True)
+    s2 = (dyg * h).mean(-1, keepdim=True)
+    dx = rstd64[:, None] * (dyg - s1 - h * s2)
+    k1 = 4 + 5 + nv + 1
+    k2 = 4 + 5 + nv + 4
+    a1 = dyg.abs().mean(-1, keepdim=True)
+    a2 = (dyg * h).abs().mean(-1, keepdim=True)
+    b = U * (rstd64[:, None] * (5 * (dyg.abs() + s1.abs() + (h * s2).abs()) + k1 * a1 + k2 * h.abs() * a2) + dx.abs())
+    return dx, b, h
+
+
+def check_layernorm_bwd(impl, device, case):
+    o = _Out("layernorm_bwd")
+    g = _gen(case)
+    M, d = case["M"], case["d"]
+    nv = d // 128
+    rpg, gather = case.get("rpg", 0), case.get("gather")
+    R = M * rpg if rpg else M
+    x = torch.randn(M, d, generator=g) * 2 + 0.5
+    x64 = d64(x)
+    mu = x64.mean(-1)
+    rs = 1.0 / torch.sqrt(((x64 - mu[:, None]) ** 2).mean(-1) + 1e-5)
+    mean, rstd = mu.to(F32), rs.to(F32)
+    gamma = torch.randn(d, generator=g)
+    dyb = case.get("dy", "f32") == "bf16"
+    dy = torch.randn(M, d, generator=g).to(BF if dyb else F32)
+    alias, use_gin = case.get("alias", False), case.get("gin", True)
+    row_idx = torch.randint(0, max(rpg, 1), (M,), generator=g, dtype=torch.int32) if gather == "idx" else None
+    phys = torch.arange(M) * rpg + (row_idx.long() if row_idx is not None else 0) if rpg else torch.arange(M)
+    gin = torch.randn(R, d, generator=g)
+    dg0, db0, gs0 = torch.randn(d, generator=g), torch.randn(d, generator=g), torch.randn(d, generator=g)
+    want_bf, want_gsum = case.get("g_bf16", True), case.get("gsum", True)
+
+    G_in = gin.to(device, copy=True) if use_gin else None
+    G_out = G_in if alias else torch.zeros(R, d, device=device)
+    Gb = torch.zeros(R, d, dtype=BF, device=device) if want_bf else None
+    dgamma, dbeta = dg0.to(device, copy=True), db0.to(device, copy=True)
+    gsum = gs0.to(device, copy=True) if want_gsum else None
+    impl.layernorm_bwd(x.to(device, copy=True), dy.to(device, copy=True) if dyb else None, None if dyb else dy.to(device, copy=True), mean.to(device, copy=True),
+                       rstd.to(device, copy=True), gamma.to(device, copy=True), G_in, G_out, Gb, dgamma, dbeta, M, d,
+                       row_idx=None if row_idx is None else row_idx.to(device, copy=True), rows_per_group=rpg, gsum=gsum)
+
+    dy64 = d64(dy)
+    dx, b_dx, h = _ln_bwd_ref(x64, dy64, d64(mean), d64(rstd), d64(gamma), nv)
+    gin64 = d64(gin)
+    ref_g = gin64.clone() if alias else torch.zeros(R, d, dtype=F64)
+    b_g = torch.zeros(R, d, dtype=F64)
+    ref_g[phys] = dx + (gin64[phys] if use_gin else 0)
+    b_g[phys] = b_dx + U * ref_g[phys].abs()
+    o.bound("g_out", G_out, ref_g, b_g)
+    # dgamma / dbeta: per-CTA running sums over ceil(M / grid) rows, then reduce_partials (ceil(grid / 8) + 8 terms)
+    # and the += into the caller's buffer; each term dy * h carries 3 roundings.
+    grid = _ln_bwd_grid(M, d, _sms(device))
+    k = _cdiv(M, grid) + _cdiv(grid, 8) + 8 + 1 + 3
+    tg, tb = (dy64 * h).abs().sum(0) + d64(dg0).abs(), dy64.abs().sum(0) + d64(db0).abs()
+    o.bound("dgamma", dgamma, d64(dg0) + (dy64 * h).sum(0), k * U * tg)
+    o.bound("dbeta", dbeta, d64(db0) + dy64.sum(0), k * U * tb)
+    if want_bf:
+        gb = Gb.cpu()
+        other = torch.ones(R, dtype=torch.bool)
+        other[phys] = False
+        o.bf16("g_bf16", gb[phys], ref_g[phys], err=b_g[phys])
+        o.exact("g_bf16_untouched", gb[other], torch.zeros(int(other.sum()), d, dtype=BF))
+        if want_gsum:   # the header's contract: the sum of the bf16-rounded g as stored
+            terms = d64(gb[phys])
+            o.bound("gsum", gsum, d64(gs0) + terms.sum(0), (k - 3) * U * (terms.abs().sum(0) + d64(gs0).abs()))
+    return o.rec
+
+
+def check_vit_embed_ln_bwd(impl, device, case):
+    o = _Out("vit_embed_ln_bwd")
+    g = _gen(case)
+    B, S, d = case["B"], case["S"], case["d"]
+    M, nv = B * S, d // 128
+    patch = (torch.randn(B * (S - 1), d, generator=g) * 2).to(BF)
+    cls, pos = torch.randn(d, generator=g), torch.randn(S, d, generator=g) * 0.5
+    # the kernel re-assembles t = pos + (cls | patch) in fp32 (one rounding): the statistics belong to that t
+    t = (torch.cat([d64(cls).view(1, 1, d).expand(B, 1, d), d64(patch).view(B, S - 1, d)], 1)
+         + d64(pos).view(1, S, d)).reshape(M, d).to(F32).to(F64)
+    mu = t.mean(-1)
+    rs = 1.0 / torch.sqrt(((t - mu[:, None]) ** 2).mean(-1) + 1e-5)
+    mean, rstd = mu.to(F32), rs.to(F32)
+    gamma = torch.randn(d, generator=g)
+    dy = torch.randn(M, d, generator=g)
+    dg0, db0 = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    dt = torch.empty(M, d, device=device)
+    dpatch = torch.empty(B * (S - 1), d, dtype=BF, device=device)
+    dgamma, dbeta = dg0.to(device, copy=True), db0.to(device, copy=True)
+    impl.vit_embed_ln_bwd(patch.to(device, copy=True), cls.to(device, copy=True), pos.to(device, copy=True), dy.to(device, copy=True), mean.to(device, copy=True),
+                          rstd.to(device, copy=True), gamma.to(device, copy=True), dt, dpatch, dgamma, dbeta, B, S, d)
+    dy64 = d64(dy)
+    dx, b_dx, h = _ln_bwd_ref(t, dy64, d64(mean), d64(rstd), d64(gamma), nv)
+    o.bound("dt_f32", dt, dx, b_dx)
+    o.bf16("dpatch", dpatch, dx.view(B, S, d)[:, 1:].reshape(-1, d), err=b_dx.view(B, S, d)[:, 1:].reshape(-1, d))
+    grid = _ln_bwd_grid(M, d, _sms(device))
+    k = _cdiv(M, grid) + _cdiv(grid, 8) + 8 + 1 + 3
+    o.bound("dgamma", dgamma, d64(dg0) + (dy64 * h).sum(0), k * U * ((dy64 * h).abs().sum(0) + d64(dg0).abs()))
+    o.bound("dbeta", dbeta, d64(db0) + dy64.sum(0), k * U * (dy64.abs().sum(0) + d64(db0).abs()))
+    return o.rec
+
+
+# ---- column / batch sums ---------------------------------------------------------------------------------------------
+def batch_sum_chunks(n, sms):
+    """Number of batch chunks mmb_batch_sum splits the rows into when Bn is large (its blockIdx.y extent)."""
+    bx = _cdiv(n // 4, 128)
+    return _cdiv(sms * 4, bx)
+
+
+def _resolve(v, n, device):
+    if isinstance(v, tuple):   # ("chunks", delta): relative to the chunk count of this device
+        return batch_sum_chunks(n, _sms(device)) + v[1]
+    return v
+
+
+def check_batch_sum(impl, device, case):
+    o = _Out("batch_sum")
+    g = _gen(case)
+    n, ld = case["n"], case["ld"]
+    Bn = _resolve(case["Bn"], n, device)
+    inp = torch.randn(Bn, ld, generator=g)
+    out0 = torch.randn(n + 4, generator=g)
+    out = out0.to(device, copy=True)
+    impl.batch_sum(inp.to(device, copy=True), out, Bn, ld, n)
+    chunks = max(min(batch_sum_chunks(n, _sms(device)), Bn), 1)
+    b_chunk = _cdiv(Bn, chunks)
+    k = b_chunk + _cdiv(_cdiv(Bn, b_chunk), 8) + 8 + 1      # chunk chain, reduce_partials, the +=
+    terms = d64(inp)[:, :n]
+    ref = d64(out0).clone()
+    ref[:n] += terms.sum(0)
+    bnd = torch.zeros(n + 4, dtype=F64)
+    bnd[:n] = k * U * (terms.abs().sum(0) + d64(out0)[:n].abs())
+    o.bound("out", out, ref, bnd)
+    return o.rec
+
+
+def check_colsum_bf16(impl, device, case):
+    o = _Out("colsum_bf16")
+    g = _gen(case)
+    M, N, ld = case["M"], case["N"], case["ld"]
+    x = torch.randn(M, ld, generator=g).to(BF)
+    out0 = torch.randn(N, generator=g)
+    out = out0.to(device, copy=True)
+    impl.colsum_bf16(x.to(device, copy=True), out, M, N, ld)
+    bx = _cdiv(N, 256)
+    chunks = _cdiv(_sms(device) * 6, bx)
+    rpb = _cdiv(_cdiv(M, chunks), 8) * 8
+    # per thread rpb / 8 rows, 8 row lanes in shared memory, reduce_partials over the row chunks, the +=
+    k = _cdiv(rpb, 8) + 8 + _cdiv(_cdiv(M, rpb), 8) + 8 + 1
+    terms = d64(x)[:, :N]
+    o.bound("out", out, d64(out0) + terms.sum(0), k * U * (terms.abs().sum(0) + d64(out0).abs()))
+    return o.rec
+
+
+def check_sum_scale(impl, device, case):
+    o = _Out("sum_scale")
+    g = _gen(case)
+    n, scale, acc = case["n"], case["scale"], case["accumulate"]
+    inp = torch.randn(n, generator=g)
+    out0 = torch.randn(1, generator=g)
+    out = out0.to(device, copy=True)
+    impl.sum_scale(inp.to(device, copy=True), n, scale, out, accumulate=acc)
+    k = _cdiv(n, 256) + 5 + 8 + 2        # per thread, warp shuffles, 8 warp sums, * scale and +=
+    s = d64(inp).sum()
+    s32 = torch.tensor(scale, dtype=F32).to(F64)
+    ref = (d64(out0) if acc else 0) + s * s32
+    bnd = k * U * (d64(inp).abs().sum() * abs(s32.item()) + (d64(out0).abs() if acc else 0))
+    o.bound("out", out, ref.view(1), torch.as_tensor(bnd, dtype=F64).view(1))
+    return o.rec
+
+
+def check_matmul_f32(impl, device, case):
+    o = _Out("matmul_f32")
+    g = _gen(case)
+    M, N, K, ta, tb, acc, alpha = case["M"], case["N"], case["K"], case["ta"], case["tb"], case["acc"], case["alpha"]
+    A = torch.randn(K, M, generator=g) if ta else torch.randn(M, K, generator=g)
+    Bm = torch.randn(N, K, generator=g) if tb else torch.randn(K, N, generator=g)
+    C0 = torch.randn(M, N, generator=g)
+    C = C0.to(device, copy=True)
+    impl.matmul_f32(A.to(device, copy=True), Bm.to(device, copy=True), ta=ta, tb=tb, out=C, alpha=alpha, accumulate=acc)
+    a64 = d64(A).t() if ta else d64(A)
+    b64 = d64(Bm).t() if tb else d64(Bm)
+    ref = alpha * (a64 @ b64) + (d64(C0) if acc else 0)
+    bnd = (K + 3) * U * (abs(alpha) * (a64.abs() @ b64.abs()) + (d64(C0).abs() if acc else 0))
+    o.bound("C", C, ref, bnd)
+    return o.rec
+
+
+# ---- embeddings ------------------------------------------------------------------------------------------------------
+def check_text_embed_fwd(impl, device, case):
+    o = _Out("text_embed_fwd")
+    g = _gen(case)
+    B, S, d, V = case["B"], case["S"], case["d"], case["V"]
+    tok = torch.randint(0, V, (B, S), generator=g)
+    tok[0, 0], tok[-1, -1] = 0, V - 1
+    emb, pos = torch.randn(V, d, generator=g), torch.randn(S, d, generator=g)
+    x = torch.empty(B * S, d, device=device)
+    impl.text_embed_fwd(tok.to(device, copy=True), emb.to(device, copy=True), pos.to(device, copy=True), x, B, S, d, V)
+    o.exact("x", x, (d64(emb)[tok] + d64(pos).view(1, S, d)).reshape(B * S, d).to(F32))
+    return o.rec
+
+
+def check_text_embed_bwd(impl, device, case):
+    """Padding: the tail of every sequence is token 0, so thousands of rows add into one table row."""
+    o = _Out("text_embed_bwd")
+    g = _gen(case)
+    B, S, d, V = case["B"], case["S"], case["d"], case["V"]
+    tok = torch.randint(1, V, (B, S), generator=g)
+    lens = torch.randint(1, S + 1, (B,), generator=g)
+    tok[torch.arange(S).view(1, S) >= lens.view(B, 1) * case.get("keep", 1.0)] = 0
+    grad = torch.randn(B * S, d, generator=g)
+    demb0 = torch.randn(V, d, generator=g) * 0.1
+    demb = demb0.to(device, copy=True)
+    impl.text_embed_bwd(tok.to(device, copy=True), grad.to(device, copy=True), demb, B, S, d)
+    flat = tok.view(-1)
+    ref = d64(demb0).index_add(0, flat, d64(grad))
+    mag = d64(demb0).abs().index_add(0, flat, d64(grad).abs())
+    # one CTA adds the rows of a token id in row order: the chain is that id's count + 1
+    cnt = torch.bincount(flat, minlength=V).to(F64).view(V, 1)
+    o.bound("demb", demb, ref, (cnt + 1) * U * mag)
+    return o.rec
+
+
+def check_argmax_tokens(impl, device, case):
+    o = _Out("argmax_tokens")
+    g = _gen(case)
+    B, S = case["B"], case["S"]
+    tok = torch.randint(0, case.get("V", 49408), (B, S), generator=g)
+    tok[0] = 7                                     # all equal: the first index
+    if B > 1:
+        tok[1, S // 3] = tok[1, S - 1] = 10 ** 6   # a tie: the first of them
+    if B > 2:
+        tok[2, -1] = 10 ** 6 + 1
+    idx = torch.empty(B, dtype=torch.int32, device=device)
+    impl.argmax_tokens(tok.to(device, copy=True), idx, B, S)
+    first = [next(s for s in range(S) if tok[b, s] == tok[b].max()) for b in range(B)]
+    o.exact("idx", idx, torch.tensor(first, dtype=torch.int32))
+    return o.rec
+
+
+def check_coca_text_embed_fwd(impl, device, case):
+    o = _Out("coca_text_embed_fwd")
+    g = _gen(case)
+    B, S, d, V, with_cls = case["B"], case["S"], case["d"], case["V"], case["cls"]
+    T = S - 1 if with_cls else S
+    ids = torch.randint(0, V, (B, T), generator=g)
+    emb, cls, pos = torch.randn(V, d, generator=g), torch.randn(d, generator=g), torch.randn(S + 3, d, generator=g)
+    x = torch.empty(B * S, d, device=device)
+    impl.coca_text_embed_fwd(ids.to(device, copy=True), emb.to(device, copy=True), cls.to(device, copy=True) if with_cls else None, pos.to(device, copy=True), x,
+                             B, S, d, V)
+    e = d64(emb)[ids]
+    if with_cls:
+        e = torch.cat([e, d64(cls).view(1, 1, d).expand(B, 1, d)], 1)
+    o.exact("x", x, (e + d64(pos)[:S].view(1, S, d)).reshape(B * S, d).to(F32))
+    return o.rec
+
+
+def _bert_inputs(case):
+    g = _gen(case)
+    B, S, d, V, P, T = case["B"], case["S"], case["d"], case["V"], case["S"] + 5, 2
+    ids = torch.randint(0, V, (B, S), generator=g)
+    ids[:, -3:] = case.get("pad", 0)
+    tt = torch.randint(0, T, (B, S), generator=g) if case.get("types", True) else None
+    word, pos, typ = torch.randn(V, d, generator=g), torch.randn(P, d, generator=g), torch.randn(T, d, generator=g)
+    gamma, beta = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    return g, ids, tt, word, pos, typ, gamma, beta
+
+
+def _bert_sum(ids, tt, word, pos, typ, S):
+    t0 = tt if tt is not None else torch.zeros_like(ids)
+    e = d64(word)[ids] + d64(pos)[:S].unsqueeze(0) + d64(typ)[t0]
+    mag = d64(word)[ids].abs() + d64(pos)[:S].unsqueeze(0).abs() + d64(typ)[t0].abs()
+    return e.reshape(-1, e.shape[-1]), mag.reshape(-1, e.shape[-1]), t0
+
+
+def check_bert_embed_ln_fwd(impl, device, case):
+    o = _Out("bert_embed_ln_fwd")
+    _, ids, tt, word, pos, typ, gamma, beta = _bert_inputs(case)
+    B, S, d, V, pad = case["B"], case["S"], case["d"], case["V"], case.get("pad", 0)
+    x = torch.empty(B * S, d, device=device)
+    km = torch.full((B * S,), 7, dtype=torch.uint8, device=device)
+    tod = lambda t: None if t is None else t.to(device, copy=True)  # noqa: E731
+    impl.bert_embed_ln_fwd(tod(ids), tod(tt), tod(word), tod(pos), tod(typ), tod(gamma), tod(beta), x, km, pad, B, S,
+                           d, V, 1e-12)
+    e, mag, _ = _bert_sum(ids, tt, word, pos, typ, S)
+    out, _, _, b_out, _, _ = _ln_fwd_bounds(e, d64(gamma), d64(beta), 1e-12, d // 128, in_err=2 * U * mag)
+    o.bound("x", x, out, b_out)
+    o.exact("kmask_out", km, (ids != pad).to(torch.uint8).view(-1))
+    return o.rec
+
+
+def check_bert_embed_ln_bwd(impl, device, case):
+    """The statistics are recomputed in fp32 from the tables, and everything lands in fp32 atomics (any order)."""
+    o = _Out("bert_embed_ln_bwd")
+    g, ids, tt, word, pos, typ, gamma, _ = _bert_inputs(case)
+    B, S, d, V = case["B"], case["S"], case["d"], case["V"]
+    M, nv = B * S, d // 128
+    dy = torch.randn(M, d, generator=g)
+    dw0, dp0, dt0 = torch.randn(V, d, generator=g), torch.randn(S + 5, d, generator=g), torch.randn(2, d, generator=g)
+    dg0, db0 = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    bufs = [t.to(device, copy=True) for t in (dw0, dp0, dt0, dg0, db0)]
+    tod = lambda t: None if t is None else t.to(device, copy=True)  # noqa: E731
+    impl.bert_embed_ln_bwd(tod(ids), tod(tt), tod(word), tod(pos), tod(typ), tod(gamma), tod(dy), *bufs, B, S, d, V,
+                           1e-12)
+    e, mag, t0 = _bert_sum(ids, tt, word, pos, typ, S)
+    _, mu, rs, h = _ln_ref(e, d64(gamma), torch.zeros(d, dtype=F64), 1e-12)
+    dy64 = d64(dy)
+    dx, b_dx, _ = _ln_bwd_ref(e, dy64, mu, rs, d64(gamma), nv)
+    # the recomputed xhat is off by the forward's statistics error: widen dx by its effect (|d dx / d xhat| <= rstd *
+    # (|s2| + |dyg| / d + ...), folded into one term per row)
+    _, _, _, b_h, _, _ = _ln_fwd_bounds(e, torch.ones(d, dtype=F64), torch.zeros(d, dtype=F64), 1e-12, nv,
+                                        in_err=2 * U * mag)
+    dyg = dy64 * d64(gamma)
+    b_dx = b_dx + rs[:, None] * (dyg * h).abs().mean(-1, keepdim=True) * b_h \
+        + rs[:, None] * (dyg.abs().mean(-1, keepdim=True) * b_h.mean(-1, keepdim=True)) * 2
+    flat_ids, flat_pos, flat_t = ids.reshape(-1), torch.arange(S).repeat(B), t0.reshape(-1)
+    for name, buf, init, index in (("dword", bufs[0], dw0, flat_ids), ("dpos", bufs[1], dp0, flat_pos),
+                                   ("dtype", bufs[2], dt0, flat_t)):
+        ref = d64(init).index_add(0, index, dx)
+        cnt = torch.bincount(index, minlength=init.shape[0]).to(F64).view(-1, 1)
+        bnd = d64(torch.zeros_like(init)).index_add(0, index, b_dx) \
+            + (cnt + 1) * U * d64(init).abs().index_add(0, index, dx.abs())
+        o.bound(name, buf, ref, bnd)
+    k = M + 4      # per-warp register sums and one atomic per warp, in any order: at most M + 1 additions
+    o.bound("dgamma", bufs[3], d64(dg0) + (dy64 * h).sum(0),
+            k * U * ((dy64 * h).abs().sum(0) + d64(dg0).abs()) + (dy64.abs() * b_h).sum(0))
+    o.bound("dbeta", bufs[4], d64(db0) + dy64.sum(0), k * U * (dy64.abs().sum(0) + d64(db0).abs()))
+    return o.rec
+
+
+# ---- L2 normalisation ------------------------------------------------------------------------------------------------
+def check_l2norm_fwd(impl, device, case):
+    o = _Out("l2norm_fwd")
+    g = _gen(case)
+    B, E, eps = case["B"], case["E"], 1e-12
+    x = torch.randn(B, E, generator=g) * 3
+    if case.get("zero_row") is not None:
+        x[case["zero_row"]] = 0
+    y = torch.empty(B, E, device=device)
+    yb = torch.empty(B, E, dtype=BF, device=device)
+    inv = torch.empty(B, device=device)
+    impl.l2norm_fwd(x.to(device, copy=True), y, yb, inv, B, E, eps)
+    x64 = d64(x)
+    eps32 = torch.tensor(eps, dtype=F32).item()
+    inv64 = 1.0 / torch.clamp_min(x64.norm(dim=1), eps32)
+    k = _cdiv(E, 32) + 5 + 1           # per-lane squares, shuffles
+    o.bound("inv_norm", inv, inv64, (k / 2 + 3) * U * inv64)
+    y64 = x64 * inv64[:, None]
+    o.bound("y", y, y64, (k / 2 + 4) * U * y64.abs())
+    o.bf16("y_bf16", yb, y64, err=(k / 2 + 4) * U * y64.abs())
+    return o.rec
+
+
+def check_l2norm_bwd(impl, device, case):
+    o = _Out("l2norm_bwd")
+    g = _gen(case)
+    B, E = case["B"], case["E"]
+    x = torch.randn(B, E, generator=g)
+    y = (x / x.norm(dim=1, keepdim=True)).to(F32)
+    inv = torch.rand(B, generator=g) + 0.2
+    dy = torch.randn(B, E, generator=g)
+    dx = torch.empty(B, E, device=device)
+    dxb = torch.empty(B, E, dtype=BF, device=device)
+    impl.l2norm_bwd(dy.to(device, copy=True), y.to(device, copy=True), inv.to(device, copy=True), dx, dxb, B, E)
+    y64, dy64, inv64 = d64(y), d64(dy), d64(inv)[:, None]
+    s = (y64 * dy64).sum(1, keepdim=True)
+    ref = inv64 * (dy64 - y64 * s)
+    k = _cdiv(E, 32) + 5 + 1
+    bnd = U * (inv64 * (3 * (dy64.abs() + (y64 * s).abs()) + k * y64.abs() * (y64 * dy64).abs().sum(1, keepdim=True))
+               + ref.abs())
+    o.bound("dx", dx, ref, bnd)
+    o.bf16("dx_bf16", dxb, ref, err=bnd)
+    return o.rec
+
+
+# ---- activations -------------------------------------------------------------------------------------------------------
+_RSQRT2 = 1.0 / math.sqrt(2.0)
+
+
+def _phi_cdf(x64):
+    return 0.5 * torch.special.erfc(-x64 * _RSQRT2)
+
+
+def _act64(x64, kind):
+    if kind == 0:
+        return x64 * torch.sigmoid(1.702 * x64)
+    return x64 * _phi_cdf(x64)
+
+
+def _act_grad64(x64, kind):
+    if kind == 0:
+        s = torch.sigmoid(1.702 * x64)
+        return s * (1 + 1.702 * x64 * (1 - s))
+    return _phi_cdf(x64) + x64 * torch.exp(-0.5 * x64 * x64) / math.sqrt(2 * math.pi)
+
+
+def _act_input(case, n):
+    x = torch.randn(n, generator=_gen(case)) * 3
+    return _with_specials(x, ACT_SPECIALS)
+
+
+def check_act_fwd(impl, device, case):
+    """QuickGELU: x / (1 + exp(-1.702 x)) with an approximate exp whose argument error grows with |x|; exact GELU:
+    0.5 x (1 + erf(x / sqrt 2)), where 1 + erf cancels for negative x (an absolute error of a few ulp of |x|)."""
+    o = _Out("act_fwd")
+    n, kind = case["n"], case["kind"]
+    x = _act_input(case, n)
+    y = impl.act_fwd(x.to(device, copy=True), kind)
+    x64 = d64(x)
+    ref = _act64(x64, kind)
+    if kind == 0:
+        bnd = (2.5 * 1.702 * x64.abs() + 8) * U * ref.abs()
+    else:
+        bnd = 4 * U * ref.abs() + 8 * U * x64.abs()
+    o.bound("y", y, ref, bnd)
+    return o.rec
+
+
+def check_tanh_(impl, device, case):
+    o = _Out("tanh_")
+    n = case["n"]
+    x = _act_input(case, n)
+    xd = x.to(device, copy=True)
+    impl.tanh_(xd)
+    ref = torch.tanh(d64(x))
+    o.bound("x", xd, ref, 4 * U * ref.abs())
+    o.exact("signed_zeros", xd.cpu()[2:4], torch.tensor([0.0, -0.0]))
+    return o.rec
+
+
+def check_tanh_bwd(impl, device, case):
+    o = _Out("tanh_bwd")
+    g = _gen(case)
+    n = case["n"]
+    y = torch.tanh(torch.randn(n, generator=g) * 2)
+    dy = torch.randn(n, generator=g)
+    dx = torch.empty(n, device=device)
+    dxb = torch.empty(n, dtype=BF, device=device)
+    impl.tanh_bwd(dy.to(device, copy=True), y.to(device, copy=True), dx, dxb)
+    y64, dy64 = d64(y), d64(dy)
+    ref = dy64 * (1 - y64 * y64)
+    bnd = 3 * U * dy64.abs() * ((1 - y64 * y64).abs() + y64 * y64)
+    o.bound("dx", dx, ref, bnd)
+    o.bf16("dx_bf16", dxb, ref, err=bnd)
+    return o.rec
+
+
+def check_act_bwd(impl, device, case):
+    o = _Out("act_bwd")
+    g = _gen(case)
+    n, kind = case["n"], case["kind"]
+    pre = _act_input(case, n).to(BF)
+    dy = torch.randn(n, generator=g).to(BF)
+    dx = torch.empty(n, dtype=BF, device=device)
+    impl.act_bwd(dy.to(device, copy=True), pre.to(device, copy=True), dx, kind)
+    x64, dy64 = d64(pre), d64(dy)
+    if kind == 0:
+        # tanh.approx (relative error 2^-11) inside 0.5 (1 + t + u (1 - t^2)), u = 0.851 x
+        u = 0.851 * x64
+        t = torch.tanh(u)
+        err = dy64.abs() * (0.5 * (1 - 2 * u * t).abs() * 2.0 ** -11 * t.abs() + 8 * U * (1 + u.abs()))
+    else:
+        # Phi(x) = 0.5 (1 + erf) carries an absolute error of a few ulp of 1; exp of -x^2/2 a relative one ~ x^2 u
+        err = dy64.abs() * (8 * U + (8 + x64 * x64) * U * (x64 * torch.exp(-0.5 * x64 * x64)).abs())
+    o.bf16("dx", dx, dy64 * _act_grad64(x64, kind), case.get("min_equal", 0.99), err=err)
+    return o.rec
+
+
+# ---- gathers, scatters, token assembly -----------------------------------------------------------------------------------
+def check_gather_rows_cast(impl, device, case):
+    o = _Out("gather_rows_cast")
+    B, rpg, row, d = case["B"], case["rpg"], case["row"], case["d"]
+    x = torch.randn(B * rpg, d, generator=_gen(case))
+    out = torch.empty(B, d, dtype=BF, device=device)
+    impl.gather_rows_cast(x.to(device, copy=True), out, B, rpg, row, d)
+    o.exact("out", out, rne_bf16(x.view(B, rpg, d)[:, row]))
+    return o.rec
+
+
+def check_gather_rows_idx_cast(impl, device, case):
+    o = _Out("gather_rows_idx_cast")
+    g = _gen(case)
+    R, ld, d, n = case["R"], case["ld"], case["d"], case["n"]
+    buf = torch.randn(R, ld, generator=g)
+    idx = torch.randint(0, R, (n,), generator=g)
+    if n > 2:
+        idx[1] = idx[0]            # repeated rows
+        idx[-1] = R - 1
+    out = torch.empty(n, d, dtype=BF, device=device)
+    impl.gather_rows_idx_cast(buf.to(device, copy=True)[:, :d], idx.to(device, copy=True), out, d)
+    o.exact("out", out, rne_bf16(buf[idx, :d]))
+    return o.rec
+
+
+def check_scatter_rows_add(impl, device, case):
+    o = _Out("scatter_rows_add")
+    g = _gen(case)
+    B, rpg, row, d = case["B"], case["rpg"], case["row"], case["d"]
+    src = torch.randn(B, d, generator=g)
+    dst0 = torch.randn(B * rpg, d, generator=g)
+    dst = dst0.to(device, copy=True)
+    impl.scatter_rows_add(src.to(device, copy=True), dst, B, rpg, row, d)
+    ref = d64(dst0).view(B, rpg, d).clone()
+    ref[:, row] += d64(src)
+    o.exact("dst", dst, ref.view(B * rpg, d).to(F32))
+    return o.rec
+
+
+def check_scatter_rows_idx_add(impl, device, case):
+    """fp32 atomics: repeated rows add in any order, so each destination row gets (count + 1) * u * sum|terms|."""
+    o = _Out("scatter_rows_idx_add")
+    g = _gen(case)
+    R, ld, d, n = case["R"], case["ld"], case["d"], case["n"]
+    src = torch.randn(n, d, generator=g)
+    idx = torch.randint(0, R, (n,), generator=g)
+    if n > 3:
+        idx[: n // 3] = idx[0]
+    buf0 = torch.randn(R, ld, generator=g)
+    buf = buf0.to(device, copy=True)
+    impl.scatter_rows_idx_add(src.to(device, copy=True), idx.to(device, copy=True), buf[:, :d], d)
+    ref = d64(buf0).clone()
+    ref[:, :d] = ref[:, :d].index_add(0, idx, d64(src))
+    cnt = torch.bincount(idx, minlength=R).to(F64).view(R, 1)
+    bnd = torch.zeros(R, ld, dtype=F64)
+    bnd[:, :d] = (cnt + 1) * U * d64(buf0)[:, :d].abs().index_add(0, idx, d64(src).abs())
+    o.bound("dst", buf, ref, bnd)
+    return o.rec
+
+
+def check_concat_tokens(impl, device, case):
+    o = _Out("concat_tokens")
+    g = _gen(case)
+    B, Sa, Sb, d, with_cls = case["B"], case["Sa"], case["Sb"], case["d"], case["cls"]
+    cls = torch.randn(d, generator=g)
+    a, b = torch.randn(B * Sa, d, generator=g), torch.randn(B * Sb, d, generator=g)
+    So = (1 if with_cls else 0) + Sa + Sb
+    out = torch.empty(B * So, d, device=device)
+    ad = a.to(device, copy=True)
+    impl.concat_tokens(cls.to(device, copy=True) if with_cls else None, ad, b.to(device, copy=True) if Sb else ad, out, B, Sa, Sb, d)
+    parts = ([cls.view(1, 1, d).expand(B, 1, d)] if with_cls else []) + [a.view(B, Sa, d), b.view(B, Sb, d)]
+    o.exact("out", out, torch.cat(parts, 1).reshape(B * So, d))
+    return o.rec
+
+
+def check_split_tokens_cast(impl, device, case):
+    o = _Out("split_tokens_cast")
+    B, Sa, Sb, d, has_cls = case["B"], case["Sa"], case["Sb"], case["d"], case["cls"]
+    off = 1 if has_cls else 0
+    gr = torch.randn(B * (off + Sa + Sb), d, generator=_gen(case))
+    a = torch.empty(B * Sa, d, dtype=BF, device=device)
+    b = torch.empty(B * Sb, d, dtype=BF, device=device) if Sb else None
+    impl.split_tokens_cast(gr.to(device, copy=True), a, b, B, Sa, Sb, d, has_cls=has_cls)
+    gv = gr.view(B, off + Sa + Sb, d)
+    o.exact("a", a, rne_bf16(gv[:, off:off + Sa].reshape(-1, d)))
+    if Sb:
+        o.exact("b", b, rne_bf16(gv[:, off + Sa:].reshape(-1, d)))
+    return o.rec
+
+
+def check_vit_assemble_fwd(impl, device, case):
+    o = _Out("vit_assemble_fwd")
+    g = _gen(case)
+    B, S, d, with_cls, masked = case["B"], case["S"], case["d"], case["cls"], case["mask"]
+    off = 1 if with_cls else 0
+    P = S - off
+    patch = torch.randn(B * P, d, generator=g).to(BF)
+    cls, pos, mtok = torch.randn(d, generator=g), torch.randn(S, d, generator=g), torch.randn(d, generator=g)
+    pm = (torch.rand(B * P, generator=g) < 0.4).to(torch.uint8)
+    x = torch.empty(B * S, d, device=device)
+    tod = lambda t: t.to(device, copy=True)  # noqa: E731
+    impl.vit_assemble_fwd(tod(patch), tod(cls) if with_cls else None, tod(pos), tod(mtok) if masked else None,
+                          tod(pm) if masked else None, x, B, S, d)
+    e = d64(patch).view(B, P, d)
+    if masked:
+        e = torch.where(pm.view(B, P, 1).bool(), d64(mtok).view(1, 1, d), e)
+    if with_cls:
+        e = torch.cat([d64(cls).view(1, 1, d).expand(B, 1, d), e], 1)
+    o.exact("x", x, (e + d64(pos).view(1, S, d)).reshape(B * S, d).to(F32))
+    return o.rec
+
+
+def check_vit_assemble_bwd(impl, device, case):
+    o = _Out("vit_assemble_bwd")
+    g = _gen(case)
+    B, S, d, has_cls, masked = case["B"], case["S"], case["d"], case["cls"], case["mask"]
+    off = 1 if has_cls else 0
+    P = S - off
+    gr = torch.randn(B * S, d, generator=g)
+    pm = (torch.rand(B * P, generator=g) < 0.4).to(torch.uint8)
+    dm0 = torch.randn(d, generator=g)
+    dpatch = torch.empty(B * P, d, dtype=BF, device=device)
+    dm = dm0.to(device, copy=True)
+    impl.vit_assemble_bwd(gr.to(device, copy=True), pm.to(device, copy=True) if masked else None, dpatch, dm if masked else None, B, S, d,
+                          has_cls=has_cls)
+    gp = gr.view(B, S, d)[:, off:].reshape(B * P, d)
+    if masked:
+        keep = ~pm.bool().view(-1, 1)
+        o.exact("dpatch", dpatch, torch.where(keep, rne_bf16(gp), torch.zeros((), dtype=BF)))
+        terms = d64(gp)[pm.bool()]
+        k = 16 + _cdiv(B * P, 16) + 1      # a 16-row strip per thread, then one atomic per strip
+        o.bound("dmask_token", dm, d64(dm0) + terms.sum(0), k * U * (terms.abs().sum(0) + d64(dm0).abs()))
+    else:
+        o.exact("dpatch", dpatch, rne_bf16(gp))
+        o.exact("dmask_token_untouched", dm, dm0)
+    return o.rec
+
+
+def check_zero_(impl, device, case):
+    o = _Out("zero_")
+    t = torch.randn(case["n"], generator=_gen(case)).to(device, copy=True)
+    impl.zero_(t)
+    o.exact("t", t, torch.zeros(case["n"]))
+    return o.rec
+
+
+def check_kv_cache_append(impl, device, case):
+    o = _Out("kv_cache_append")
+    g = _gen(case)
+    B, H, Sp, Sn, hd = case["B"], case["H"], case["Sp"], case["Sn"], case["hd"]
+    past_dt, out_dt, want_bf = case["past"], case["out"], case["out_bf16"]
+    d = H * hd
+    past = None
+    if Sp:   # stored [B, Sp, H, hd]: a [B, H, Sp, hd] view with non-contiguous strides
+        past = torch.randn(B, Sp, H, hd, generator=g).to(past_dt).transpose(1, 2)
+    newbuf = torch.randn(B * Sn, d + 8, generator=g).to(BF)
+    out = torch.empty(B * (Sp + Sn) * d, dtype=out_dt, device=device) if out_dt is not None else None
+    outb = torch.empty(B * (Sp + Sn) * d, dtype=BF, device=device) if want_bf else None
+    impl.kv_cache_append(None if past is None else past.to(device, copy=True), newbuf.to(device, copy=True)[:, :d], out, outb, B=B, H=H,
+                         Sp=Sp, Sn=Sn, head_dim=hd)
+    new = newbuf[:, :d].to(F32).view(B, Sn, d)
+    cat = new if past is None else torch.cat([past.to(F32).transpose(1, 2).reshape(B, Sp, d), new], 1)
+    cat = cat.reshape(-1)
+    if out is not None:
+        o.exact("out", out, cat if out_dt == F32 else rne_bf16(cat))
+    if outb is not None:
+        o.exact("out_bf16", outb, rne_bf16(cat))
+    return o.rec
+
+
+# ---- losses --------------------------------------------------------------------------------------------------------------
+def _ce_inputs(case):
+    g = _gen(case)
+    M, V, stride, ignore = case["M"], case["V"], case["stride"], case.get("ignore", -100)
+    logits = torch.randn(M, V, generator=g) * case.get("scale", 3.0)
+    lab = torch.randint(0, V, (M,), generator=g)
+    lab[0] = V - 1
+    nig = case.get("n_ignored", 0)
+    if nig:
+        lab[torch.randperm(M, generator=g)[:nig]] = ignore
+    labels = torch.full((M * stride,), 12345, dtype=torch.int64)   # the other slots of a strided label view
+    labels[::stride] = lab
+    return g, logits, lab, labels, ignore
+
+
+def check_ce_labels(impl, device, case):
+    """row loss = max + log(sum exp(x - max)) - x[label] with an approximate exp (relative error ~(2 + 1.44 |z|) u for
+    argument z) summed over ceil(V / 256) + 5 + 8 terms; accum[0] adds the kept rows through reduce_partials."""
+    o = _Out("ce_labels")
+    g, logits, lab, labels, ignore = _ce_inputs(case)
+    M, V, stride = case["M"], case["V"], case["stride"]
+    row_loss = torch.full((M,), 5.0, device=device)
+    acc0 = torch.tensor([1.5, 2.0])
+    accum = acc0.to(device, copy=True)
+    impl.ce_labels(logits.to(device, copy=True), labels.to(device, copy=True), stride, ignore, M, V, row_loss, accum)
+    l64 = d64(logits)
+    keep = lab != ignore
+    lse = torch.logsumexp(l64, 1)
+    mx = l64.max(1).values
+    nll = torch.where(keep, lse - l64.gather(1, lab.clamp(0, V - 1).view(-1, 1)).squeeze(1), torch.zeros((), dtype=F64))
+    zspan = (mx - l64.min(1).values)
+    k = _cdiv(V, 256) + 5 + 8 + 4
+    b_row = U * ((k + 2 + 1.5 * zspan) + 2 * (mx.abs() + lse.abs() + l64.abs().max(1).values))
+    b_row = torch.where(keep, b_row, torch.zeros((), dtype=F64))
+    o.bound("row_loss", row_loss, nll, b_row)
+    kr = _cdiv(M, 8) + 8 + 1
+    o.bound("accum", accum, torch.stack([d64(acc0)[0] + nll.sum(), d64(acc0)[1] + keep.sum().to(F64)]),
+            torch.stack([b_row.sum() + kr * U * (nll.abs().sum() + abs(acc0[0].item())), torch.zeros((), dtype=F64)]))
+    return o.rec
+
+
+def check_ce_labels_bwd(impl, device, case):
+    o = _Out("ce_labels_bwd")
+    g, logits, lab, labels, ignore = _ce_inputs(case)
+    M, V, stride = case["M"], case["V"], case["stride"]
+    keep = lab != ignore
+    count = float(keep.sum())
+    accum = torch.tensor([3.0, count])
+    gscale = torch.tensor([0.75]) if case.get("gscale") else None
+    dl = torch.empty(M, V, dtype=BF, device=device)
+    impl.ce_labels_bwd(logits.to(device, copy=True), labels.to(device, copy=True), stride, ignore, M, V, accum.to(device, copy=True), 1.25, dl,
+                       gscale=None if gscale is None else gscale.to(device, copy=True))
+    l64 = d64(logits)
+    p = torch.softmax(l64, 1)
+    oh = torch.zeros(M, V, dtype=F64)
+    oh[torch.arange(M)[keep], lab[keep]] = 1
+    w = 1.25 * (0.75 if gscale is not None else 1.0) / max(count, 1.0)
+    zspan = (l64.max(1).values - l64.min(1).values).view(-1, 1)
+    k = _cdiv(V, 256) + 5 + 8 + 4
+    err = abs(w) * ((k + 2 + 1.5 * zspan) * U * p + 2 * U * (p - oh).abs()) * keep.view(-1, 1)
+    o.bf16("dlogits", dl, w * (p - oh) * keep.view(-1, 1), err=err)
+    return o.rec
+
+
+# ---- GEMM and attention: a small case each, so the emulation meets the kernel ---------------------------------------------
+def check_gemm(impl, device, case):
+    o = _Out("gemm")
+    g = _gen(case)
+    M, N, K = case["M"], case["N"], case["K"]
+    A, Bm = torch.randn(M, K, generator=g).to(BF), torch.randn(N, K, generator=g).to(BF)
+    bias = torch.randn(N, generator=g)
+    ref = d64(A) @ d64(Bm).t()
+    mag = d64(A).abs() @ d64(Bm).abs().t()
+    if case["epi"] == "f32":
+        C0 = torch.randn(M, N, generator=g)
+        C = C0.to(device, copy=True)
+        impl.gemm(A.to(device, copy=True), Bm.to(device, copy=True), epilogue=3, out=C, accumulate=True)
+        o.bound("D", C, ref + d64(C0), (K + 3) * U * (mag + d64(C0).abs()))
+    else:
+        D = impl.gemm(A.to(device, copy=True), Bm.to(device, copy=True), bias=bias.to(device, copy=True))
+        o.bf16("D", D, ref + d64(bias), err=(K + 3) * U * (mag + d64(bias).abs()))
+    return o.rec
+
+
+def _attn64(q, k, v, causal, scale, kmask=None, mask=None):
+    """q [B, H, Sq, D], k / v [B, H, Skv, D] float64; masks broadcast to [B, 1, Sq, Skv]; empty rows give 0."""
+    s = (q @ k.transpose(-1, -2)) * scale
+    Sq, Skv = s.shape[-2:]
+    allow = torch.ones(Sq, Skv, dtype=torch.bool)
+    if causal:
+        allow = torch.ones(Sq, Skv, dtype=torch.bool).tril()
+    allow = allow.view(1, 1, Sq, Skv)
+    if kmask is not None:
+        allow = allow & kmask.bool().view(kmask.shape[0], 1, 1, Skv)
+    if mask is not None:
+        allow = allow & mask.bool().view(mask.shape[0], 1, Sq, Skv)
+    s = s.masked_fill(~allow, float("-inf"))
+    p = torch.nan_to_num(torch.softmax(s, -1), nan=0.0)
+    return p @ v, torch.logsumexp(s, -1)
+
+
+def _packed_attn_inputs(case):
+    g = _gen(case)
+    B, S, H = case["B"], case["S"], case["H"]
+    qkv = torch.randn(B * S, 3 * H * 64, generator=g).to(BF)
+    kmask = None
+    if case.get("kmask"):
+        kmask = (torch.rand(B, S, generator=g) < 0.8).to(torch.uint8)
+        kmask[:, 0] = 1
+    dout = torch.randn(B * S, H * 64, generator=g).to(BF)
+    return qkv, kmask, dout
+
+
+def _split_heads(t, B, S, H):
+    return t.view(B, S, H, 64).transpose(1, 2)
+
+
+def _attn_packed_ref(qkv, kmask, B, S, H, causal, scale, dout=None):
+    d = H * 64
+    q, k, v = (_split_heads(d64(qkv)[:, i * d:(i + 1) * d], B, S, H).clone().requires_grad_(dout is not None)
+               for i in range(3))
+    with torch.enable_grad():
+        out, lse = _attn64(q, k, v, causal, scale, kmask=kmask)
+        out2 = out.transpose(1, 2).reshape(B * S, d)
+        if dout is None:
+            return out2.detach(), lse.detach().reshape(-1), None
+        out2.backward(d64(dout))
+    grads = [t.grad.transpose(1, 2).reshape(B * S, d) for t in (q, k, v)]
+    return out2.detach(), lse.detach(), torch.cat(grads, 1)
+
+
+def _check_attention_fwd(impl, device, case, kmasked):
+    o = _Out()
+    B, S, H, causal = case["B"], case["S"], case["H"], case["causal"]
+    scale = 0.125
+    qkv, kmask, _ = _packed_attn_inputs(case)
+    out = torch.empty(B * S, H * 64, dtype=BF, device=device)
+    lse = torch.empty(B * H * S, device=device)
+    if kmasked:
+        impl.attention_fwd_kmask(qkv.to(device, copy=True), out, lse, kmask.to(device, copy=True), B, S, H, causal, scale)
+    else:
+        impl.attention_fwd(qkv.to(device, copy=True), out, lse, B, S, H, causal, scale)
+    ref, rlse, _ = _attn_packed_ref(qkv, kmask if kmasked else None, B, S, H, causal, scale)
+    o.rel("out", out, ref, 1e-2)
+    o.bound("lse", lse, rlse.reshape(-1), 1e-3 * (1 + rlse.abs().reshape(-1)))
+    return o.rec
+
+
+def check_attention_fwd(impl, device, case):
+    return _check_attention_fwd(impl, device, case, False)
+
+
+def check_attention_fwd_kmask(impl, device, case):
+    return _check_attention_fwd(impl, device, case, True)
+
+
+def _check_attention_bwd(impl, device, case, kmasked):
+    o = _Out("attention_fwd_kmask")
+    B, S, H, causal = case["B"], case["S"], case["H"], case["causal"]
+    scale = 0.125
+    qkv, kmask, dout = _packed_attn_inputs(case)
+    qd = qkv.to(device, copy=True)
+    out = torch.empty(B * S, H * 64, dtype=BF, device=device)
+    lse = torch.empty(B * H * S, device=device)
+    dqkv = torch.empty(B * S, 3 * H * 64, dtype=BF, device=device)
+    if kmasked:
+        km = kmask.to(device, copy=True)
+        impl.attention_fwd_kmask(qd, out, lse, km, B, S, H, causal, scale)
+        impl.attention_bwd_kmask(qd, out, dout.to(device, copy=True), lse, dqkv, km, B, S, H, causal, scale)
+    else:
+        impl.attention_fwd(qd, out, lse, B, S, H, causal, scale)
+        impl.attention_bwd(qd, out, dout.to(device, copy=True), lse, dqkv, B, S, H, causal, scale)
+    _, _, ref = _attn_packed_ref(qkv, kmask if kmasked else None, B, S, H, causal, scale, dout)
+    o.rel("dqkv", dqkv, ref, 2e-2)
+    return o.rec
+
+
+def check_attention_bwd(impl, device, case):
+    return _check_attention_bwd(impl, device, case, False)
+
+
+def check_attention_bwd_kmask(impl, device, case):
+    return _check_attention_bwd(impl, device, case, True)
+
+
+def _generic_inputs(case):
+    g = _gen(case)
+    B, Sq, Skv, H, hd = case["B"], case["Sq"], case["Skv"], case["H"], case["hd"]
+    d = H * hd
+    q = torch.randn(B * Sq, d, generator=g).to(BF)
+    k = torch.randn(B * Skv, d, generator=g).to(BF)
+    v = torch.randn(B * Skv, d, generator=g).to(BF)
+    mask = None
+    if case.get("mask"):
+        mask = (torch.rand(B, Skv, generator=g) < 0.7).to(torch.uint8)
+        mask[:, 0] = 1
+    dout = torch.randn(B * Sq, d, generator=g).to(BF)
+    return q, k, v, mask, dout
+
+
+def _generic_ref(q, k, v, mask, case, dout=None):
+    B, Sq, Skv, H, hd = case["B"], case["Sq"], case["Skv"], case["H"], case["hd"]
+    sp = lambda t, S: d64(t).view(B, S, H, hd).transpose(1, 2).clone().requires_grad_(dout is not None)  # noqa: E731
+    qh, kh, vh = sp(q, Sq), sp(k, Skv), sp(v, Skv)
+    with torch.enable_grad():
+        out, _ = _attn64(qh, kh, vh, case.get("causal", False), 1 / math.sqrt(hd), kmask=mask)
+        out2 = out.transpose(1, 2).reshape(B * Sq, H * hd)
+        if dout is None:
+            return out2.detach(), None
+        out2.backward(d64(dout))
+    return out2.detach(), [t.grad.transpose(1, 2).reshape(-1, H * hd) for t in (qh, kh, vh)]
+
+
+def _generic_kw(case):
+    B, Sq, Skv, H, hd = case["B"], case["Sq"], case["Skv"], case["H"], case["hd"]
+    d = H * hd
+    return dict(B=B, Sq=Sq, Skv=Skv, H=H, head_dim=hd, bsq=Sq * d, bsk=Skv * d, bsv=Skv * d, bso=Sq * d,
+                scale=1 / math.sqrt(hd), mask_bs=Skv if case.get("mask") else 0, mask_qs=0,
+                causal=case.get("causal", False))
+
+
+def check_attention_fwd_generic(impl, device, case):
+    o = _Out("attention_fwd_generic")
+    q, k, v, mask, _ = _generic_inputs(case)
+    out = torch.empty(q.shape, dtype=BF, device=device)
+    impl.attention_fwd_generic(q.to(device, copy=True), k.to(device, copy=True), v.to(device, copy=True), out,
+                               mask=None if mask is None else mask.to(device, copy=True), **_generic_kw(case))
+    o.rel("out", out, _generic_ref(q, k, v, mask, case)[0], 1e-2)
+    return o.rec
+
+
+def check_attention_fwd_decode(impl, device, case):
+    o = _Out("attention_fwd_decode")
+    q, k, v, mask, _ = _generic_inputs(case)
+    out = torch.empty(q.shape, dtype=BF, device=device)
+    impl.attention_fwd_decode(q.to(device, copy=True), k.to(device, copy=True), v.to(device, copy=True), out,
+                              mask=None if mask is None else mask.to(device, copy=True), **_generic_kw(case))
+    o.rel("out", out, _generic_ref(q, k, v, mask, case)[0], 1e-2)
+    return o.rec
+
+
+def check_attention_bwd_generic(impl, device, case):
+    o = _Out("attention_bwd_generic")
+    q, k, v, mask, dout = _generic_inputs(case)
+    dq, dk, dv = (torch.empty(t.shape, dtype=BF, device=device) for t in (q, k, v))
+    impl.attention_bwd_generic(q.to(device, copy=True), k.to(device, copy=True), v.to(device, copy=True), dout.to(device, copy=True), dk, dv, dq=dq,
+                               mask=None if mask is None else mask.to(device, copy=True), **_generic_kw(case))
+    _, (rq, rk, rv) = _generic_ref(q, k, v, mask, case, dout)
+    o.rel("dq", dq, rq, 2e-2)
+    o.rel("dk", dk, rk, 2e-2)
+    o.rel("dv", dv, rv, 2e-2)
+    return o.rec
+
+
+# ---- cases -----------------------------------------------------------------------------------------------------------------
+_WIDTHS = [128 * nv for nv in range(1, 9)]
+
+CASES = {
+    "cast_bf16": [{"n": 1}, {"n": 3}, {"n": 21}, {"n": 1001, "seed": 1}, {"n": 3_000_003, "gpu": True}],
+    "cast_f32": [{"n": 1}, {"n": 7}, {"n": 65535}],
+    "im2col": [{"B": 1, "H": 32, "W": 48, "ps": 16, "ld": 768}, {"B": 2, "H": 28, "W": 42, "ps": 14, "ld": 592},
+               {"B": 2, "H": 224, "W": 224, "ps": 14, "ld": 592, "gpu": True},
+               {"B": 64, "H": 224, "W": 224, "ps": 14, "ld": 592, "gpu": True},
+               {"B": 64, "H": 224, "W": 224, "ps": 16, "ld": 768, "gpu": True}],
+    "add_layernorm_fwd": [{"M": 37, "d": d, "seed": d} for d in _WIDTHS] + [
+        {"M": 9, "d": 512, "rpg": 77, "gather": "idx"},           # ln_final at the EOT rows (CLIP text)
+        {"M": 5, "d": 768, "rpg": 50, "gather": "zero"},          # ln_post at the CLS rows (CLIP vision)
+        {"M": 40, "d": 256, "y": False}, {"M": 40, "d": 384, "x": False},
+        {"M": 17000, "d": 128, "gpu": True}, {"M": 17000, "d": 1024, "gpu": True},
+        {"M": 300, "d": 768, "rpg": 77, "gather": "idx", "gpu": True}],
+    "layernorm_bwd": [{"M": 37, "d": d, "seed": d} for d in _WIDTHS] + [
+        {"M": 23, "d": 768, "dy": "bf16", "alias": True},          # the encoder layers' (..., G, G, Gb, ...) call
+        {"M": 9, "d": 512, "rpg": 77, "gather": "idx"},
+        {"M": 6, "d": 768, "rpg": 50, "gather": "zero", "gin": False},
+        {"M": 31, "d": 256, "g_bf16": False, "gsum": False},
+        {"M": 4000, "d": 128, "dy": "bf16", "alias": True, "gpu": True},     # above num_sms * 24 rows
+        {"M": 1000, "d": 1024, "dy": "bf16", "alias": True, "gpu": True},    # above num_sms * 6 rows
+        {"M": 3, "d": 1024, "gpu": True},
+        {"M": 640, "d": 512, "rpg": 77, "gather": "idx", "gpu": True}],
+    "vit_embed_ln_fwd": [{"B": 3, "S": 5, "d": d, "seed": d} for d in _WIDTHS] + [
+        {"B": 64, "S": 197, "d": 768, "gpu": True}, {"B": 70, "S": 257, "d": 1024, "gpu": True}],
+    "vit_embed_ln_bwd": [{"B": 3, "S": 5, "d": d, "seed": d} for d in _WIDTHS] + [
+        {"B": 64, "S": 197, "d": 768, "gpu": True}, {"B": 16, "S": 257, "d": 1024, "gpu": True}],
+    "batch_sum": [{"Bn": 7, "n": 512, "ld": 520}, {"Bn": ("chunks", 0), "n": 512, "ld": 512},
+                  {"Bn": ("chunks", 1), "n": 512, "ld": 512}, {"Bn": 2000, "n": 512, "ld": 516},
+                  {"Bn": 5, "n": 12, "ld": 3 * 12}, {"Bn": 33, "n": 64, "ld": 77 * 64},
+                  {"Bn": 64, "n": 197 * 768, "ld": 197 * 768, "gpu": True}],
+    "colsum_bf16": [{"M": 37, "N": 264, "ld": 264}, {"M": 1001, "N": 776, "ld": 784}, {"M": 1, "N": 8, "ld": 8},
+                    {"M": 31, "N": 2056, "ld": 2064}, {"M": 4096, "N": 3072, "ld": 3072, "gpu": True},
+                    {"M": 12608, "N": 768, "ld": 768, "gpu": True}],
+    "sum_scale": [{"n": 1, "scale": 0.5, "accumulate": False}, {"n": 300, "scale": -1.5, "accumulate": True},
+                  {"n": 5000, "scale": 1 / 3, "accumulate": False}, {"n": 2, "scale": 2.0, "accumulate": True}],
+    "matmul_f32": [{"M": 3, "N": 5, "K": 7, "ta": False, "tb": False, "acc": False, "alpha": 1.0},
+                   {"M": 33, "N": 17, "K": 65, "ta": True, "tb": True, "acc": True, "alpha": -0.5},
+                   {"M": 40, "N": 9, "K": 3, "ta": False, "tb": True, "acc": False, "alpha": 2.0}],
+    "text_embed_fwd": [{"B": 3, "S": 7, "d": 64, "V": 100}, {"B": 33, "S": 77, "d": 512, "V": 49408, "gpu": True}],
+    "text_embed_bwd": [{"B": 4, "S": 16, "d": 64, "V": 50}, {"B": 3, "S": 9, "d": 12, "V": 1000},
+                       {"B": 64, "S": 77, "d": 512, "V": 49408, "keep": 0.3, "gpu": True},
+                       {"B": 256, "S": 77, "d": 768, "V": 1024, "gpu": True}],
+    "argmax_tokens": [{"B": 3, "S": 77}, {"B": 13, "S": 5}, {"B": 70, "S": 100, "gpu": True}],
+    "coca_text_embed_fwd": [{"B": 2, "S": 6, "d": 64, "V": 40, "cls": True},
+                            {"B": 3, "S": 5, "d": 32, "V": 40, "cls": False}],
+    "bert_embed_ln_fwd": [{"B": 2, "S": 9, "d": 128, "V": 30}, {"B": 3, "S": 5, "d": 768, "V": 30, "types": False},
+                          {"B": 16, "S": 512, "d": 768, "V": 30522, "gpu": True}],
+    "bert_embed_ln_bwd": [{"B": 2, "S": 9, "d": 128, "V": 30}, {"B": 3, "S": 5, "d": 768, "V": 30, "types": False},
+                          {"B": 16, "S": 128, "d": 768, "V": 1000, "gpu": True}],
+    "l2norm_fwd": [{"B": 5, "E": 512, "zero_row": 1}, {"B": 9, "E": 77}, {"B": 3, "E": 1},
+                   {"B": 1000, "E": 768, "zero_row": 999, "gpu": True}],
+    "l2norm_bwd": [{"B": 5, "E": 512}, {"B": 9, "E": 77}, {"B": 1000, "E": 768, "gpu": True}],
+    "act_fwd": [{"n": 8, "kind": 0}, {"n": 8, "kind": 1}, {"n": 1001, "kind": 0}, {"n": 1001, "kind": 1},
+                {"n": 1_000_001, "kind": 1, "gpu": True}],
+    "tanh_": [{"n": 9}, {"n": 1001}],
+    "tanh_bwd": [{"n": 9}, {"n": 1001}],
+    "act_bwd": [{"n": 9, "kind": 0}, {"n": 9, "kind": 1}, {"n": 4001, "kind": 0}, {"n": 4001, "kind": 1},
+                {"n": 1_000_001, "kind": 0, "gpu": True}, {"n": 1_000_001, "kind": 1, "gpu": True}],
+    "gather_rows_cast": [{"B": 3, "rpg": 5, "row": 0, "d": 64}, {"B": 4, "rpg": 7, "row": 6, "d": 12}],
+    "gather_rows_idx_cast": [{"R": 50, "ld": 72, "d": 64, "n": 13}, {"R": 9, "ld": 12, "d": 12, "n": 1},
+                             {"R": 5000, "ld": 772, "d": 768, "n": 3000, "gpu": True}],
+    "scatter_rows_add": [{"B": 3, "rpg": 5, "row": 0, "d": 64}, {"B": 4, "rpg": 7, "row": 6, "d": 12}],
+    "scatter_rows_idx_add": [{"R": 50, "ld": 72, "d": 64, "n": 30}, {"R": 9, "ld": 12, "d": 12, "n": 1},
+                             {"R": 2000, "ld": 772, "d": 768, "n": 3000, "gpu": True}],
+    "concat_tokens": [{"B": 2, "Sa": 3, "Sb": 4, "d": 16, "cls": True}, {"B": 3, "Sa": 5, "Sb": 0, "d": 8, "cls": True},
+                      {"B": 2, "Sa": 2, "Sb": 3, "d": 4, "cls": False}],
+    "split_tokens_cast": [{"B": 2, "Sa": 3, "Sb": 4, "d": 16, "cls": True}, {"B": 3, "Sa": 5, "Sb": 0, "d": 8, "cls": True},
+                          {"B": 2, "Sa": 2, "Sb": 3, "d": 4, "cls": False}],
+    "vit_assemble_fwd": [{"B": 2, "S": 5, "d": 16, "cls": True, "mask": True},
+                         {"B": 2, "S": 4, "d": 8, "cls": False, "mask": False},
+                         {"B": 3, "S": 10, "d": 32, "cls": True, "mask": False}],
+    "vit_assemble_bwd": [{"B": 2, "S": 5, "d": 16, "cls": True, "mask": True},
+                         {"B": 2, "S": 4, "d": 8, "cls": False, "mask": False},
+                         {"B": 64, "S": 197, "d": 768, "cls": True, "mask": True, "gpu": True}],
+    "zero_": [{"n": 5}, {"n": 4096}],
+    "kv_cache_append": [
+        {"B": 2, "H": 3, "Sp": 5, "Sn": 2, "hd": 64, "past": F32, "out": F32, "out_bf16": True},
+        {"B": 2, "H": 2, "Sp": 4, "Sn": 1, "hd": 96, "past": BF, "out": BF, "out_bf16": False},
+        {"B": 1, "H": 2, "Sp": 0, "Sn": 3, "hd": 128, "past": F32, "out": F32, "out_bf16": True},
+        {"B": 3, "H": 1, "Sp": 7, "Sn": 5, "hd": 64, "past": F32, "out": None, "out_bf16": True},
+        {"B": 4, "H": 12, "Sp": 300, "Sn": 1, "hd": 64, "past": BF, "out": BF, "out_bf16": False, "gpu": True}],
+    "ce_labels": [{"M": 6, "V": 49408, "stride": 2, "n_ignored": 2}, {"M": 5, "V": 97, "stride": 1},
+                  {"M": 4, "V": 49408, "stride": 3, "n_ignored": 4},              # every row ignored
+                  {"M": 300, "V": 49408, "stride": 2, "n_ignored": 50, "gpu": True}],
+    "ce_labels_bwd": [{"M": 6, "V": 49408, "stride": 2, "n_ignored": 2, "gscale": True}, {"M": 5, "V": 97, "stride": 1},
+                      {"M": 4, "V": 49408, "stride": 3, "n_ignored": 4},
+                      {"M": 300, "V": 49408, "stride": 2, "n_ignored": 50, "gpu": True}],
+    "gemm": [{"M": 128, "N": 256, "K": 192, "epi": "bf16"}, {"M": 64, "N": 128, "K": 128, "epi": "f32"}],
+    "attention_fwd": [{"B": 2, "S": 40, "H": 2, "causal": True}],
+    "attention_fwd_kmask": [{"B": 2, "S": 40, "H": 2, "causal": False, "kmask": True}],
+    "attention_bwd": [{"B": 2, "S": 40, "H": 2, "causal": True}],
+    "attention_bwd_kmask": [{"B": 2, "S": 40, "H": 2, "causal": False, "kmask": True}],
+    "attention_fwd_generic": [{"B": 2, "Sq": 16, "Skv": 40, "H": 2, "hd": 64, "mask": True}],
+    "attention_bwd_generic": [{"B": 2, "Sq": 16, "Skv": 40, "H": 2, "hd": 96}],
+    "attention_fwd_decode": [{"B": 2, "Sq": 3, "Skv": 100, "H": 2, "hd": 64, "mask": True}],
+}
+
+# Kernels whose results DESIGN.md §4 documents as run-to-run bit-exact (no floating-point atomics).
+DETERMINISTIC = ["layernorm_bwd", "vit_embed_ln_bwd", "batch_sum", "colsum_bf16", "text_embed_bwd", "ce_labels",
+                 "sum_scale"]
+
+CHECKS = {op: globals()["check_" + op] for op in CASES}
+
+
+def case_id(case):
+    return ",".join(f"{k}={getattr(v, '__name__', None) or (str(v).replace('torch.', ''))}"
+                    for k, v in case.items() if k != "gpu")
+
+
+def emulation():
+    """The CPU emulation of every kernel (tests/emu_ops.py + tests/emu_decode_ops.py) as one `impl`."""
+    import types
+
+    import emu_decode_ops
+    import emu_ops
+
+    ns = {n: getattr(emu_ops, n) for n in emu_ops.NAMES}
+    ns.update(attention_fwd_decode=emu_decode_ops.attention_fwd_decode, kv_cache_append=emu_decode_ops.kv_cache_append)
+    return types.SimpleNamespace(**ns)

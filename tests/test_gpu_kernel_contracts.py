@@ -1,0 +1,58 @@
+"""The kernel contracts of tests/kernel_contract_cases.py on the GPU: every check with the CUDA kernels at the full case
+set, the same check with the CPU emulation on identical inputs held against the kernel's result under the same
+tolerance class (the emulation the CPU schedule tests trust matches the kernel), and run-to-run bit-exactness of the
+kernels DESIGN.md §4 documents as free of floating-point atomics."""
+import pytest
+import torch
+
+import kernel_contract_cases as KC
+from multimodal_b200 import ops
+
+pytestmark = pytest.mark.gpu
+
+_ALL = [(op, c) for op, cases in KC.CASES.items() for c in cases]
+_IDS = [f"{op}[{KC.case_id(c)}]" for op, c in _ALL]
+
+
+@pytest.fixture(scope="module")
+def dev():
+    return torch.device("cuda:0")
+
+
+@pytest.mark.parametrize("op,case", _ALL, ids=_IDS)
+def test_kernel_meets_float64_contract_and_matches_emulation(dev, op, case):
+    got = KC.CHECKS[op](ops, dev, case)
+    torch.cuda.synchronize()
+    emu = KC.CHECKS[op](KC.emulation(), "cpu", case)
+    assert got.keys() == emu.keys()
+    for name in got:
+        slack = 0.0
+        if name == "gsum":   # sums the stored g_bf16, whose elements may differ by one bf16 ulp between the two
+            slack = (got["g_bf16"].got.double() - emu["g_bf16"].got.double()).abs().sum(0)
+        KC.compare_recs(f"{op}.{name} kernel vs emulation", got[name], emu[name], slack)
+
+
+_DET = [(op, c) for op, c in _ALL if op in KC.DETERMINISTIC]
+
+
+@pytest.mark.parametrize("op,case", _DET, ids=[f"{op}[{KC.case_id(c)}]" for op, c in _DET])
+def test_atomic_free_kernels_are_bit_exact_run_to_run(dev, op, case):
+    a = KC.CHECKS[op](ops, dev, case)
+    b = KC.CHECKS[op](ops, dev, case)
+    for name in a:
+        KC.assert_exact(f"{op}.{name} second run", b[name].got, a[name].got)
+
+
+@pytest.mark.parametrize("rows,N", [(7, 7), (300, 1024), (1000, 4000)])
+def test_contrastive_ce_stats_dscale_is_bit_exact_run_to_run(dev, rows, N):
+    g = torch.Generator().manual_seed(rows)
+    sims = (torch.rand(rows, N, generator=g) * 2 - 1).to(dev)
+    scale = torch.tensor([2.6592], device=dev)
+    outs = []
+    for _ in range(2):
+        row_loss, lse = torch.empty(rows, device=dev), torch.empty(rows, device=dev)
+        dscale = torch.full((1,), 0.25, device=dev)
+        ops.contrastive_ce_stats(sims, scale, rows, N, N - rows, 0.1, 0.5, row_loss, lse, dscale)
+        outs.append((row_loss, lse, dscale))
+    for x, y in zip(*outs):
+        KC.assert_exact("contrastive_ce_stats", y.cpu(), x.cpu())
