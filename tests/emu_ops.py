@@ -161,9 +161,16 @@ def _attn(qkv, B, S, H, causal, scale, kmask):
     return q, k, v, s
 
 
+def _softmax_rows(s):
+    """softmax over the keys; a row with no visible key (all -inf) gets p = 0, with a zero gradient, as the kernels
+    give it O = 0 and no backward contribution (include/mmb200.h)."""
+    vis = (s > float("-inf")).any(-1, keepdim=True)
+    return torch.softmax(torch.where(vis, s, torch.zeros_like(s)), -1) * vis
+
+
 def attention_fwd(qkv, out, lse, B, S, H, causal, scale, kmask=None):
     q, k, v, s = _attn(qkv, B, S, H, causal, scale, kmask)
-    out.copy_((torch.softmax(s, -1) @ v).transpose(1, 2).reshape(B * S, H * 64).to(BF))
+    out.copy_((_softmax_rows(s) @ v).transpose(1, 2).reshape(B * S, H * 64).to(BF))
     if lse is not None:
         lse.copy_(torch.logsumexp(s, -1).reshape(-1))
 
@@ -176,13 +183,20 @@ def attention_bwd(qkv, out, dout, lse, dqkv, B, S, H, causal, scale, kmask=None)
     qf = qkv.float().requires_grad_(True)
     with torch.enable_grad():
         _, _, v, s = _attn(qf, B, S, H, causal, scale, kmask)
-        o = (torch.softmax(s, -1) @ v).transpose(1, 2).reshape(B * S, H * 64)
+        o = (_softmax_rows(s) @ v).transpose(1, 2).reshape(B * S, H * 64)
         o.backward(dout.float())
     dqkv.copy_(qf.grad.to(BF))
 
 
 def attention_bwd_kmask(qkv, out, dout, lse, dqkv, kmask, B, S, H, causal, scale):
     attention_bwd(qkv, out, dout, lse, dqkv, B, S, H, causal, scale, kmask)
+
+
+def attention_probs(qkv, lse, kmask, probs, B, S, H, causal, scale):
+    """exp(q.k * scale - lse) from the lse the forward wrote; 0 where the key is masked, causal-future or the row empty."""
+    _, _, _, s = _attn(qkv, B, S, H, causal, scale, kmask)
+    vis = s > float("-inf")
+    probs.copy_(torch.where(vis, torch.exp(s - lse.view(B, H, S, 1)), torch.zeros_like(s)))
 
 
 def vit_assemble_fwd(patch_out, cls, pos, mask_token, patch_mask, x, B, S, d):
@@ -330,9 +344,9 @@ def matmul_f32(A, B, *, ta=False, tb=False, out=None, alpha=1.0, accumulate=Fals
     return out
 
 
-def _gen_attn(q, k, v, B, Sq, Skv, H, hd, bsq, scale, mask, causal):
-    d = H * hd
-    qh = (q.view(1, Sq, H, hd).expand(B, Sq, H, hd) if bsq == 0 else q.reshape(B, Sq, H, hd)).transpose(1, 2)
+def _gen_scores(q, k, v, B, Sq, Skv, H, hd, bsq, scale, mask, causal):
+    """Scores [B, H, Sq, Skv] (-inf where masked) and V [B, H, Skv, hd] of the general attention."""
+    qh = (q.reshape(1, Sq, H, hd).expand(B, Sq, H, hd) if bsq == 0 else q.reshape(B, Sq, H, hd)).transpose(1, 2)
     kh, vh = k.reshape(B, Skv, H, hd).transpose(1, 2), v.reshape(B, Skv, H, hd).transpose(1, 2)
     s = (qh @ kh.transpose(-1, -2)) * scale
     if causal:
@@ -341,8 +355,12 @@ def _gen_attn(q, k, v, B, Sq, Skv, H, hd, bsq, scale, mask, causal):
         mk = mask.bool()
         mk = mk.view(B, 1, Sq, Skv) if mk.numel() == B * Sq * Skv else mk.view(B, 1, 1, Skv)
         s = s.masked_fill(~mk, float("-inf"))
-    p = torch.nan_to_num(torch.softmax(s, -1), nan=0.0)
-    return (p @ vh).transpose(1, 2).reshape(B * Sq, d)
+    return s, vh
+
+
+def _gen_attn(q, k, v, B, Sq, Skv, H, hd, bsq, scale, mask, causal):
+    s, vh = _gen_scores(q, k, v, B, Sq, Skv, H, hd, bsq, scale, mask, causal)
+    return (_softmax_rows(s) @ vh).transpose(1, 2).reshape(B * Sq, H * hd)
 
 
 def attention_fwd_generic(q, k, v, out, *, B, Sq, Skv, H, head_dim, bsq, bsk, bsv, bso, scale, mask=None, mask_bs=0,

@@ -24,7 +24,6 @@ def test_emulation_meets_float64_contract(op, case):
 # Public wrappers of multimodal_b200.ops without an entry in CASES, each with the test file that covers it.
 ALLOWLIST = {
     "self_attention": "test_attention_router_cpu.py",
-    "attention_probs": "test_gpu_attention_long.py",
     "clip_image_transform": "test_gpu_clip_transform.py",
     "clip_image_transform_max_taps": "test_clip_transform_cpu.py",
     "gemm_ce_stats": "test_gpu_gemm_wide.py",
@@ -127,6 +126,96 @@ def _batch_sum_skips_last(inp, out, Bn, ld, n):
     emu_ops.batch_sum(inp, out, Bn - 1, ld, n)
 
 
+def _online_attn_fwd(qkv, out, lse, B, S, H, causal, scale, kmask=None, *, rescale=True, drop_block=None, diag=0,
+                     kmask_last_block=True):
+    """The kernels' online softmax over 64-key blocks (running max m, sum l, O in fp32, P rounded to bf16 for PV), with
+    the defects the mutants below switch on."""
+    inf = float("inf")
+    km = kmask
+    if km is not None and not kmask_last_block:
+        km = km.clone().view(B, S)
+        km[:, (S - 1) // 64 * 64:] = 1
+    _, _, v, s = emu_ops._attn(qkv, B, S, H, False, scale, km)
+    if causal:
+        s = s + torch.full((S, S), -inf).triu(1 + diag)
+    m = torch.full((B, H, S, 1), -inf)
+    l = torch.zeros(B, H, S, 1)
+    o = torch.zeros(B, H, S, 64)
+    for j0 in range(0, S, 64):
+        sb = s[..., j0:j0 + 64].clone()
+        if drop_block is not None and j0 == 64 * drop_block:
+            sb[:, :, 128:] = -inf
+        mn = torch.maximum(m, sb.amax(-1, keepdim=True))
+        base = torch.where(mn == -inf, torch.zeros_like(mn), mn)
+        c = torch.exp(m - base)
+        e = torch.exp(sb - base)
+        l = l * c + e.sum(-1, keepdim=True)
+        o = (o * c if rescale else o) + e.to(torch.bfloat16).float() @ v[..., j0:j0 + 64, :]
+        m = mn
+    out.copy_((o / torch.where(l > 0, l, torch.ones_like(l))).transpose(1, 2).reshape(B * S, H * 64).to(torch.bfloat16))
+    lse.copy_(torch.where(l > 0, m + torch.log(l), torch.full_like(l, -inf)).reshape(-1))
+
+
+def _fwd_no_rescale(qkv, out, lse, B, S, H, causal, scale):
+    _online_attn_fwd(qkv, out, lse, B, S, H, causal, scale, rescale=False)
+
+
+def _fwd_drops_block_past_first_tile(qkv, out, lse, B, S, H, causal, scale):
+    _online_attn_fwd(qkv, out, lse, B, S, H, causal, scale, drop_block=1)
+
+
+def _fwd_causal_off_by_one(qkv, out, lse, B, S, H, causal, scale):
+    _online_attn_fwd(qkv, out, lse, B, S, H, causal, scale, diag=1)
+
+
+def _fwd_kmask_ignored_in_last_block(qkv, out, lse, kmask, B, S, H, causal, scale):
+    _online_attn_fwd(qkv, out, lse, B, S, H, causal, scale, kmask, kmask_last_block=False)
+
+
+def _bwd_dkdv_skip_last_partial_tile(qkv, out, dout, lse, dqkv, B, S, H, causal, scale):
+    emu_ops.attention_bwd(qkv, out, dout, lse, dqkv, B, S, H, causal, scale)
+    if S % 128:   # dK / dV without the query rows of the last, partial 128-row tile (their dO and dS set to zero)
+        d = dout.clone().view(B, S, -1)
+        d[:, S // 128 * 128:] = 0
+        part = torch.empty_like(dqkv)
+        emu_ops.attention_bwd(qkv, out, d.view(B * S, -1), lse, part, B, S, H, causal, scale)
+        dqkv[:, H * 64:] = part[:, H * 64:]
+
+
+def _dq_f32_assigned(*args, dq_f32=None, **kw):
+    if dq_f32 is not None:
+        dq_f32.zero_()
+    emu_ops.attention_bwd_generic(*args, dq_f32=dq_f32, **kw)
+
+
+def _decode_combine_unscaled(q, k, v, out, *, B, Sq, Skv, H, head_dim, bsq, bsk, bsv, bso, scale, mask=None, mask_bs=0,
+                             mask_qs=0, causal=False):
+    """The decode kernel's schedule: each key split keeps its own running max m_s, sum l_s and unnormalised O_s; the
+    combine adds them without rescaling each to the common max, O = sum O_s / sum l_s."""
+    from multimodal_b200 import _lib
+
+    full = None if mask is None else torch.as_strided(mask, (B, Sq, Skv), (mask_bs, mask_qs, 1)).contiguous()
+    s, vh = emu_ops._gen_scores(q.float(), k.float(), v.float(), B, Sq, Skv, H, head_dim, bsq, scale, full, causal)
+    n = _lib.lib().mmb_attention_decode_splits(B, H, Skv)
+    per = -(-(-(-Skv // 64)) // n) * 64
+    o = torch.zeros(B, H, Sq, head_dim)
+    l = torch.zeros(B, H, Sq, 1)
+    for j0 in range(0, Skv, per):
+        sb = s[..., j0:j0 + per]
+        m = sb.amax(-1, keepdim=True)
+        e = torch.exp(sb - torch.where(m == float("-inf"), torch.zeros_like(m), m))
+        o = o + e.to(torch.bfloat16).float() @ vh[..., j0:j0 + per, :]
+        l = l + e.sum(-1, keepdim=True)
+    r = o / torch.where(l > 0, l, torch.ones_like(l))
+    out.copy_(r.transpose(1, 2).reshape(B * Sq, H * head_dim).to(torch.bfloat16))
+
+
+def _probs_next_row_lse(qkv, lse, kmask, probs, B, S, H, causal, scale):
+    l = lse.view(B, H, S)
+    emu_ops.attention_probs(qkv, torch.cat([l[..., 1:], l[..., -1:]], -1).reshape(-1), kmask, probs, B, S, H, causal,
+                            scale)
+
+
 MUTANTS = {
     "cast truncates instead of rounding": ("cast_bf16", "cast_bf16", _truncating_cast_bf16),
     "LayerNorm backward skips the last row": ("layernorm_bwd", "layernorm_bwd", _ln_bwd_skips_last_row),
@@ -138,6 +227,18 @@ MUTANTS = {
     "colsum drops the last partial 256-column block": ("colsum_bf16", "colsum_bf16", _colsum_drops_partial_block),
     "bf16 output of fp32 math rounds toward zero": ("l2norm_fwd", "l2norm_fwd", _l2norm_truncating_bf16),
     "batch_sum drops the last batch row": ("batch_sum", "batch_sum", _batch_sum_skips_last),
+    "online softmax does not rescale O when the running max moves": ("attention_fwd", "attention_fwd", _fwd_no_rescale),
+    "one 64-key block dropped for query rows past the first 128-row tile":
+        ("attention_fwd", "attention_fwd", _fwd_drops_block_past_first_tile),
+    "causal diagonal off by one": ("attention_fwd", "attention_fwd", _fwd_causal_off_by_one),
+    "key mask ignored in the last partial key block":
+        ("attention_fwd_kmask", "attention_fwd_kmask", _fwd_kmask_ignored_in_last_block),
+    "dK / dV skip the query rows of the last partial 128-row tile":
+        ("attention_bwd", "attention_bwd", _bwd_dkdv_skip_last_partial_tile),
+    "dq_f32 assigned instead of accumulated": ("attention_bwd_generic", "attention_bwd_generic", _dq_f32_assigned),
+    "decode splits combined without rescaling to the common max":
+        ("attention_fwd_decode", "attention_fwd_decode", _decode_combine_unscaled),
+    "attention_probs uses the lse of the next row": ("attention_probs", "attention_probs", _probs_next_row_lse),
 }
 
 
@@ -154,6 +255,31 @@ def test_broken_emulation_fails_its_contract(what):
         except AssertionError:
             caught += 1
     assert caught > 0, f"no CPU case of {op} rejects the mutant '{what}'"
+
+
+def test_online_softmax_restatement_meets_the_contract():
+    """The blockwise restatement the attention mutants are built on passes every CPU case when no defect is on, so
+    each mutant fails for its defect alone."""
+    impl = types.SimpleNamespace(**vars(KC.emulation()))
+    impl.attention_fwd = lambda *a: _online_attn_fwd(*a)
+    impl.attention_fwd_kmask = lambda qkv, out, lse, kmask, *a: _online_attn_fwd(qkv, out, lse, *a, kmask)
+    for op in ("attention_fwd", "attention_fwd_kmask"):
+        for case in KC.CASES[op]:
+            if not case.get("gpu"):
+                KC.CHECKS[op](impl, "cpu", case)
+
+
+def test_attention_cases_sit_where_they_say():
+    """The general cases lie on the side of the resident / streamed switch the case list names, and every decode
+    case runs the number of key splits it was built for."""
+    from multimodal_b200 import _lib
+
+    lib = _lib.lib()
+    for c in KC.CASES["attention_fwd_generic"]:
+        assert lib.mmb_attention_generic_streamed(c["Sq"], c["Skv"], c["hd"]) == KC._STREAMED[(c["Sq"], c["Skv"], c["hd"])], c
+    assert set(KC._STREAMED.values()) == {0, 1}
+    for c in KC.CASES["attention_fwd_decode"]:
+        assert lib.mmb_attention_decode_splits(c["B"], c["H"], c["Skv"]) == c.get("splits", 1), c
 
 
 # ---- zero-size calls ---------------------------------------------------------------------------------------------------
