@@ -36,8 +36,10 @@ class ContrastiveFunction(torch.autograd.Function):
     def forward(ctx, a, b, logit_scale, smoothing, backprop_type, want_logits, mask=None):
         if a.shape != b.shape or a.dim() != 2:
             raise MMBError(f"contrastive loss expects two [B, E] tensors, got {tuple(a.shape)} and {tuple(b.shape)}")
-        if not (a.is_cuda and b.is_cuda and logit_scale.is_cuda):
-            raise MMBError("contrastive loss: embeddings and logit_scale must be CUDA tensors (no CPU path)")
+        from .engine import _require_cuda
+
+        for t in (a, b, logit_scale):    # the one device guard of the runtimes (no CPU path)
+            _require_cuda(t.device)
         world, rank = _dist_state()
         a32 = a.detach().contiguous().float()
         b32 = b.detach().contiguous().float()

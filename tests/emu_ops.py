@@ -438,6 +438,167 @@ def argmax_tokens(tokens, idx, B, S):
     idx.copy_(tokens.argmax(-1).to(torch.int32))
 
 
+_LOG2E32 = torch.tensor(1.4426950408889634, dtype=F32)
+_LN2_32 = torch.tensor(0.6931471805599453, dtype=F32)
+
+
+def _temperature(log_scale):
+    return torch.exp(log_scale.detach().reshape(-1)[:1].float())
+
+
+def contrastive_ce_stats(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, row_loss, lse_out,
+                         dscale_accum, logits_out=None, row_w=None):
+    T = _temperature(logit_scale)
+    l = T * sims[:rows, :N].float()
+    ar = torch.arange(rows)
+    lab = label_offset + ar
+    mx = l.amax(1, keepdim=True)
+    lse = mx.squeeze(1) + torch.log(torch.exp(l - mx).sum(1))
+    xl = l[ar, lab]
+    mean = l.sum(1) / N
+    loss = (1 - smoothing) * (lse - xl) + smoothing * (lse - mean)
+    wrow = row_w[:rows].float() if row_w is not None else torch.full((rows,), 1.0 / rows)
+    if row_loss is not None:
+        row_loss[:rows] = loss * wrow * rows if row_w is not None else loss
+    if lse_out is not None:
+        lse_out[:rows] = lse
+    if logits_out is not None:
+        logits_out[:rows, :N] = l
+    if dscale_accum is not None:
+        gl = torch.exp(l - lse[:, None]) - torch.tensor(smoothing, dtype=F32) / N
+        gl[ar, lab] -= 1 - smoothing
+        dscale_accum.view(-1)[:1] += ((gl * l).sum(1) * loss_weight * wrow).sum()
+
+
+def contrastive_ce_grad(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, lse_row, lse_col, col_lo,
+                        col_hi, dsims_bf16, dsims_f32, row_w=None, col_w=None):
+    T = _temperature(logit_scale)
+    l = T * sims[:rows, :N].float()
+    ar = torch.arange(rows)
+    t = torch.full((rows, N), smoothing / N, dtype=F32)
+    t[ar, label_offset + ar] += 1 - smoothing
+    gs = loss_weight * T * (row_w[:rows].float() if row_w is not None else torch.full((rows,), 1.0 / rows))
+    g = gs[:, None] * (torch.exp(l - lse_row[:rows, None]) - t)
+    lo, hi = max(col_lo, 0), min(col_hi, N)
+    if lse_col is not None and hi > lo:
+        j = slice(lo, hi)
+        wc = loss_weight * T * (col_w[j].float() if col_w is not None else torch.full((hi - lo,), 1.0 / rows))
+        add = wc * (torch.exp(l[:, j] - lse_col[j]) - t[:, j])
+        g[:, j] += torch.where(wc != 0, add, torch.zeros_like(add))   # zero-weight rows may carry a non-finite LSE
+    if dsims_bf16 is not None:
+        dsims_bf16[:rows, :N] = g.to(BF)
+    if dsims_f32 is not None:
+        dsims_f32[:rows, :N] = g
+
+
+def _merge_lanes(a, b):
+    """One __shfl_xor level of the EPI_CE_STATS quad merge: (m2, se, sex, sx) of two lanes, m2 in log2 units."""
+    (m, se, sex, sx), (mo, seo, sexo, sxo) = a, b
+    mn = torch.maximum(m, mo)
+    f = torch.where(m == float("-inf"), torch.zeros_like(m), torch.exp2(m - mn))
+    fo = torch.where(mo == float("-inf"), torch.zeros_like(mo), torch.exp2(mo - mn))
+    return mn, se * f + seo * fo, sex * f + sexo * fo, sx + sxo
+
+
+def _ce_stats_epilogue(acc, T, lab, part, part0, xlabel):
+    """EPI_CE_STATS over one launch's fp32 accumulators acc [M, N]: per 128-column part, lane tq of a quad reduces the
+    32 columns c with (c % 8) // 2 == tq (max, then sum 2^(a T2 - m2), sum 2^(...) x, sum x with x = a T), the four
+    lanes merge as lanes 0+1 and 2+3, then the two pairs; part p gets {m2 ln2, se, sex, sx}.  xlabel[r] = x[r, lab[r]]
+    where lab[r] is a column of this launch."""
+    M, N = acc.shape
+    P = (N + 127) // 128
+    T2 = T * _LOG2E32
+    a = torch.zeros(M, P * 128)
+    a[:, :N] = acc
+    ok = torch.zeros(M, P * 128, dtype=torch.bool)
+    ok[:, :N] = True
+    a, ok = a.view(M, P, 16, 4, 2), ok.view(M, P, 16, 4, 2)     # column 128 p + 8 j + 2 tq + e
+    x = a * T
+    m2 = torch.where(ok, a, torch.full_like(a, float("-inf"))).amax((2, 4), keepdim=True) * T2
+    pe = torch.where(ok, torch.exp2(a * T2 - torch.where(m2 == float("-inf"), torch.zeros_like(m2), m2)),
+                     torch.zeros_like(a))
+    zx = torch.where(ok, x, torch.zeros_like(x))
+    lane = (m2[:, :, 0, :, 0], pe.sum((2, 4)), (pe * zx).sum((2, 4)), zx.sum((2, 4)))     # [M, P, 4 lanes] each
+    q = [tuple(t[..., k] for t in lane) for k in range(4)]
+    m, se, sex, sx = _merge_lanes(_merge_lanes(q[0], q[1]), _merge_lanes(q[2], q[3]))
+    part[:M, part0:part0 + P] = torch.stack([m * _LN2_32, se, sex, sx], -1)
+    r = torch.arange(M)
+    hit = (lab >= 0) & (lab < N)
+    xlabel[r[hit]] = (acc[r[hit], lab[hit]] * T)
+
+
+def gemm_ce_stats(A, B, log_scale, label0, part, part0, xlabel):
+    acc = A.float() @ B.float().t()
+    _ce_stats_epilogue(acc, _temperature(log_scale), label0 + torch.arange(A.shape[0]), part, part0, xlabel)
+
+
+def ce_stats_reduce(part, n_parts, xlabel, rows, n_total, smoothing, loss_weight, row_w, row_loss, lse_out,
+                    dscale_accum):
+    m, y, z, w = part[:rows, :n_parts].float().unbind(-1)
+    ok = y > 0
+    mx = torch.where(ok, m, torch.full_like(m, float("-inf"))).amax(1, keepdim=True)
+    f = torch.where(ok, torch.exp(m - mx), torch.zeros_like(m))
+    se = torch.where(ok, y * f, torch.zeros_like(y)).sum(1)
+    sex = torch.where(ok, z * f, torch.zeros_like(z)).sum(1)
+    lse = mx.squeeze(1) + torch.log(se)
+    xl = xlabel[:rows].float()
+    mean = w.sum(1) / n_total
+    loss = (1 - smoothing) * (lse - xl) + smoothing * (lse - mean)
+    wrow = row_w[:rows].float() if row_w is not None else torch.full((rows,), 1.0 / rows)
+    if row_loss is not None:
+        row_loss[:rows] = loss * wrow * rows if row_w is not None else loss
+    if lse_out is not None:
+        lse_out[:rows] = lse
+    if dscale_accum is not None:
+        dscale_accum.view(-1)[:1] += ((sex / se - (1 - smoothing) * xl - smoothing * mean) * loss_weight * wrow).sum()
+
+
+def gemm_ce_grad(A, B, log_scale, label0, n_total, rows_total, smoothing, loss_weight, lse_row, row_w, lse_col, col_w,
+                 col_lo, col_hi, dsims):
+    from multimodal_b200._lib import MMBError
+
+    M, N = A.shape[0], B.shape[0]
+    if N % 8:
+        raise MMBError("gemm_ce_grad: a bf16 output needs N % 8 == 0")
+    assert tuple(dsims.shape) == (M, N) and dsims.dtype == BF
+    acc = A.float() @ B.float().t()
+    T = _temperature(log_scale)
+    T2 = T * _LOG2E32
+    r = torch.arange(M)
+    t = (torch.tensor(smoothing, dtype=F32) / float(n_total)).expand(M, N).clone()
+    lab = label0 + r
+    hit = (lab >= 0) & (lab < N)
+    t[r[hit], lab[hit]] += 1 - smoothing
+    gs = torch.tensor(loss_weight, dtype=F32) / float(rows_total)
+    gsT = T * (loss_weight * row_w[:M].float() if row_w is not None else gs.expand(M))
+    g = gsT[:, None] * (torch.exp2(acc * T2 - (lse_row[:M] * _LOG2E32)[:, None]) - t)
+    lo, hi = max(col_lo, 0), min(col_hi, N)
+    if lse_col is not None and hi > lo:
+        j = slice(lo, hi)
+        wc = (loss_weight * T * col_w[j].float()) if col_w is not None else (T * gs).expand(hi - lo)
+        add = wc * (torch.exp2(acc[:, j] * T2 - lse_col[j] * _LOG2E32) - t[:, j])
+        g[:, j] += torch.where(wc != 0, add, torch.zeros_like(add))
+    dsims.copy_(g.to(BF))
+
+
+def linear_cross_entropy(hidden_bf16, weight_bf16, labels_i32, ignore_index, accum, row_loss=None):
+    M, V = hidden_bf16.shape[0], weight_bf16.shape[0]
+    P = (V + 127) // 128
+    part = torch.zeros(M, P, 4)
+    xlabel = torch.zeros(M)
+    lab = labels_i32.reshape(-1).long()
+    _ce_stats_epilogue(hidden_bf16.float() @ weight_bf16.float().t(), torch.ones(1), lab, part, 0, xlabel)
+    m, y = part[..., 0], part[..., 1]
+    mx = m.amax(1, keepdim=True)
+    loss = mx.squeeze(1) + torch.log((y * torch.exp(m - mx)).sum(1)) - xlabel
+    keep = lab != ignore_index
+    loss = torch.where(keep, loss, torch.zeros_like(loss))
+    if row_loss is not None:
+        row_loss[:M] = loss
+    accum.view(-1)[0] += loss.sum()
+    accum.view(-1)[1] += keep.sum()
+
+
 _real_wgrad_splits = None
 
 

@@ -25,6 +25,7 @@ kernel leaves unwritten fails.
 CASES maps every checked op to its shape cases.  A case with ``"gpu": True`` is sized for the GPU (grid caps, real
 vocabularies, long sequences) and is skipped by the CPU run of the emulation.
 """
+import contextlib
 import math
 
 import torch
@@ -197,6 +198,14 @@ TIGHTENED = {
     "attention_fwd.lse": 0.11,               # 0.037 / 0.025
     "attention_fwd_kmask.lse": 0.1,          # 0.033 / 0.027
     "attention_bwd_generic.dq_f32": 0.063,   # 0.021 / 0.00047
+    "contrastive_ce_stats.dscale": 0.14,     # 0.046 / 0.046
+    "gemm_ce_stats.sum_e": 0.16,             # 0.051 / 0.035
+    "gemm_ce_stats.sum_ex": 0.16,            # 0.051 / 0.034
+    "gemm_ce_stats.sum_x": 0.17,             # 0.056 / 0.022
+    "gemm_ce_stats.xlabel": 0.3,             # 0.097 / 0.037
+    "ce_stats_reduce.dscale": 0.12,          # 0.018 / 0.040
+    "linear_cross_entropy.row_loss": 0.15,   # 0.048 / 0.048
+    "linear_cross_entropy.accum": 0.1,       # 0.033 / 0.024
 }
 
 
@@ -1565,6 +1574,559 @@ _PROBS = [
     {"B": 1, "S": 1025, "H": 1, "causal": True, "scale": 0.3, "inputs": "falling", "gpu": True},
 ]
 
+# ---- temperature-scaled cross-entropy: materialised (loss.cu) and fused into the similarity GEMM (gemm.cu) ---------------
+# The references are written from include/mmb200.h and contrastive_loss_with_temperature.py:81-107: logits
+# x = exp(log_scale) * sims (T64 = exp(log_scale) in float64), row loss (1 - eps) (lse - x_label) + eps (lse - mean x),
+# d loss / d sims = w T (softmax - t), t = (1 - eps) onehot(label) + eps / N, plus the other direction's transposed term
+# on [col_lo, col_hi); d loss / d log_scale = sum (p - t) x = E_p[x] - (1 - eps) x_label - eps mean(x).
+# Error terms of the bounds, each built from the row's (or element's) own values:
+#   T       __expf(log_scale): (2 + floor(1.173 |log_scale|)) ulp (CUDA C++ Programming Guide, intrinsic functions);
+#   x       the fp32 GEMM accumulation (K + 3) U sum|a||b| (as check_gemm) times T, plus x's own roundings;
+#   exp     __expf(z) in loss.cu: (2 + floor(1.173 |z|)) ulp; ex2.approx in the GEMM epilogues: EX2, with the fmaf
+#           argument a T2 - m2 (T2 = T log2e rounded) rounded once;
+#   log     logf: 1 ulp (no fast-math);
+#   merges  32 columns per lane and the two-level quad merge in EPI_CE_STATS (each level rescales by one ex2), the
+#           ceil(n_parts / 32) + 5 chain of ce_stats_reduce, 256-thread block sums of ceil(N / 256) + 5 + 8 in loss.cu,
+#           reduce_partials' ceil(rows / 8) + 8 + 1 for the scalar accumulators;
+#   dscale  formed by cancellation: bounded with sum |terms|, never with the result.
+_LS_CLIP, _LS_MAX = math.log(1 / 0.07), math.log(100.0)     # the initial logit scale and its clamp
+
+
+def _expf_rel(z):
+    """Relative error of __expf(z): the CUDA C++ Programming Guide bounds it by 2 + floor(1.173 |z|) ulp, and one ulp is
+    at most 2^-23 of the value."""
+    z = torch.as_tensor(z, dtype=F64)
+    return (2 + torch.floor(1.173 * z.abs())) * 2 * U
+
+
+def _f32(v):
+    return float(torch.tensor(v, dtype=F32))
+
+
+@contextlib.contextmanager
+def _gemm_mode(impl, case):
+    """Forces the GEMM kernel variant of case["gemm_mode"] (0: one CTA per 128 x 256 tile, 1: 2-CTA clusters) for the
+    real kernels; the automatic choice takes clusters only at M >= 512 with enough tiles.  The emulation has one path."""
+    if "gemm_mode" not in case or getattr(impl, "__name__", None) != "multimodal_b200.ops":
+        yield
+        return
+    from multimodal_b200 import _lib
+
+    assert _lib.lib().mmb_gemm_set_mode(case["gemm_mode"], 8) == 0
+    try:
+        yield
+    finally:
+        _lib.lib().mmb_gemm_set_mode(-1, 0)
+
+
+def _pair(case, g, M, N, K, lab):
+    """bf16 operands of a similarity GEMM, A [M, K] and B [N, K], of the kind case["inputs"]:
+      norm  unit rows (the loss's L2-normalised embeddings);
+      raw   N(0, 1) rows: logits of several hundred at the clamped temperature;
+      peak  unit rows, A_i a noisy copy of B's row lab[i] (where that is a row of B): one column dominates its row;
+      flat  unit rows, A scaled by 1e-3: a row's logits all but equal."""
+    kind = case.get("inputs", "norm")
+    A, Bm = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g)
+    if kind != "raw":
+        A, Bm = A / A.norm(dim=1, keepdim=True), Bm / Bm.norm(dim=1, keepdim=True)
+    if kind == "peak":
+        ok = (lab >= 0) & (lab < N)
+        A[ok] = Bm[lab[ok]] + 0.1 * A[ok]
+        A = A / A.norm(dim=1, keepdim=True)
+    elif kind == "flat":
+        A = A * 1e-3
+    else:
+        assert kind in ("norm", "raw"), kind
+    return A.to(BF), Bm.to(BF)
+
+
+def _mask_weights(g, n, zero=(), one=()):
+    """Masked-mean weights mask_i / count(mask) of a boolean row mask (contrastive_loss_with_temperature.py:97-100),
+    ~70 % of the rows kept, the rows in `zero` dropped (weight 0) and those in `one` kept."""
+    m = torch.rand(n, generator=g) < 0.7
+    m[list(zero)] = False
+    m[list(one)] = True
+    return (m.to(F64) / m.sum()).to(F32)
+
+
+def _gemm64(A, Bm):
+    """float64 A B^T of bf16 operands and its fp32-accumulation bound (K + 3) U sum|a||b|, on the CPU."""
+    dev = _refdev()
+    a, b = d64(A).to(dev), d64(Bm).to(dev)
+    return (a @ b.t()).cpu(), ((A.shape[1] + 3) * U * (a.abs() @ b.abs().t())).cpu()
+
+
+def _exp_term_err(Wt, x, ex, L, e, t):
+    """Error of one W (2^(a T2 - L log2e) - t) term of the EPI_CE_GRAD epilogue (or of W (__expf(x - L) - t) in
+    loss.cu with ex = x's error): e = exp(x - L) in float64; the fmaf argument and L log2e round once each; W = lw T w
+    carries T's error and two products."""
+    rho = ex + 2 * U * L.abs() + U * (x - L).abs() + EX2 + _expf_rel(x - L)
+    return Wt.abs() * (e * rho + U * (e + t) + TINY_P) + Wt.abs() * 3 * U * (e - t).abs()
+
+
+def _sims(case, g, rows, N, off):
+    """fp32 similarity rows [rows, ld] (the columns past N NaN: the kernels must not read them) of bf16 embeddings of
+    width 64 in the case's input kind, the label column of row i at off + i."""
+    A, Bm = _pair(case, g, rows, N, 64, off + torch.arange(rows))
+    s = torch.full((rows, case.get("ld", N)), NAN)
+    s[:, :N] = (d64(A) @ d64(Bm).t()).to(F32)
+    return s
+
+
+def _lse_stats(x, ex, k):
+    """Row log-sum-exp of loss.cu over the fp32 logits with errors ex: the row max cancels (the same max enters the
+    exponent and the result), each __expf(x - max) has its own relative error, the block sum k roundings, logf 1 ulp,
+    the final add."""
+    lse = torch.logsumexp(x, 1)
+    p = torch.exp(x - lse[:, None])
+    z = x - x.amax(1, keepdim=True)
+    b = (p * (ex + U * z.abs() + _expf_rel(z))).sum(1) + k * U + 2 * U * (lse - x.amax(1)).abs() + U * lse.abs() \
+        + x.shape[1] * TINY_P
+    return lse, p, b
+
+
+def check_contrastive_ce_stats(impl, device, case):
+    o = _Out("contrastive_ce_stats")
+    g = _gen(case)
+    rows, N, off, eps, lw = case["rows"], case["N"], case.get("off", 0), _f32(case.get("eps", 0.0)), 0.5
+    sims = _sims(case, g, rows, N, off)
+    ls = torch.tensor([case.get("ls", _LS_CLIP)], dtype=F32)
+    rw = _mask_weights(g, rows, zero=(0,), one=(rows - 1,)) if case.get("rw") else None
+    d0 = torch.tensor([0.375])
+    row_loss, lse = torch.full((rows,), NAN, device=device), torch.full((rows,), NAN, device=device)
+    dscale = d0.to(device, copy=True)
+    logits = torch.full(sims.shape, NAN, device=device) if case.get("logits") else None
+    impl.contrastive_ce_stats(sims.to(device, copy=True), ls.to(device, copy=True), rows, N, off, eps, lw, row_loss,
+                              lse, dscale, logits, None if rw is None else rw.to(device, copy=True))
+    T64, eT = math.exp(ls.item()), _expf_rel(ls.item()).item()
+    x = T64 * d64(sims)[:, :N]
+    ex = (eT + 2 * U) * x.abs()                       # T's error and the product's rounding
+    k = _cdiv(N, 256) + 5 + 8
+    ar = torch.arange(rows)
+    lab = off + ar
+    lse64, p, b_lse = _lse_stats(x, ex, k)
+    xl, mean = x[ar, lab], x.mean(1)
+    b_mean = ex.mean(1) + (k + 1) * U * x.abs().mean(1)
+    loss = (1 - eps) * (lse64 - xl) + eps * (lse64 - mean)
+    b_loss = b_lse + ex[ar, lab] + eps * b_mean + 3 * U * (lse64.abs() + xl.abs() + mean.abs()) + U * loss.abs()
+    wrow = d64(rw) if rw is not None else torch.full((rows,), 1.0 / rows, dtype=F64)
+    if rw is not None:
+        o.bound("row_loss", row_loss, loss * wrow * rows, b_loss * wrow * rows + 3 * U * (loss * wrow * rows).abs())
+    else:
+        o.bound("row_loss", row_loss, loss, b_loss)
+    o.bound("lse", lse, lse64, b_lse)
+    if logits is not None:
+        got = logits.cpu()
+        o.bound("logits", got[:, :N], x, ex)
+        o.exact("logits_pad", got[:, N:], torch.full((rows, sims.shape[1] - N), NAN))
+    # d loss / d log_scale: per row sum_j (p - t) x over the block chain, * lw * wrow, then reduce_partials and the +=
+    t = torch.full((rows, N), eps / N, dtype=F64)
+    t[ar, lab] += 1 - eps
+    gl = p - t
+    e_gl = p * (ex + b_lse[:, None] + U * (x - lse64[:, None]).abs() + _expf_rel(x - lse64[:, None])) + 2 * U * (p + t)
+    part = (gl * x).sum(1) * lw * wrow
+    b_part = ((e_gl * x.abs() + gl.abs() * ex).sum(1) + (k + 2) * U * (gl * x).abs().sum(1)) * lw * wrow \
+        + 3 * U * part.abs()
+    kr = _cdiv(rows, 8) + 8 + 1
+    o.bound("dscale", dscale, d64(d0) + part.sum(), b_part.sum() + kr * U * (part.abs().sum() + abs(d0.item())))
+    return o.rec
+
+
+def check_contrastive_ce_grad(impl, device, case):
+    """lse_row is the fp32-rounded float64 row LSE; lse_col that of the other direction's rows (here: the column's LSE
+    over these rows, widened to N rows); col_w-weight-0 columns carry a non-finite lse_col when case["bad"]."""
+    o = _Out("contrastive_ce_grad")
+    g = _gen(case)
+    rows, N, off, eps, lw = case["rows"], case["N"], case.get("off", 0), _f32(case.get("eps", 0.0)), 0.5
+    sims = _sims(case, g, rows, N, off)
+    ld = sims.shape[1]
+    ls = torch.tensor([case.get("ls", _LS_CLIP)], dtype=F32)
+    T64, eT = math.exp(ls.item()), _expf_rel(ls.item()).item()
+    x = T64 * d64(sims)[:, :N]
+    lse_row = torch.logsumexp(x, 1).to(F32)
+    lse_col = (torch.logsumexp(x, 0) + math.log(N / rows)).to(F32)
+    cw = rw = None
+    if case.get("rw"):
+        cw = _mask_weights(g, N, zero=(0, off), one=(off + rows - 1,))
+        rw = cw[off:off + rows].clone()
+        if case.get("bad"):
+            z = (cw == 0).nonzero().view(-1)
+            lse_col[z] = torch.tensor([NAN, float("-inf"), float("inf")])[torch.arange(z.numel()) % 3]
+    lo, hi = {"none": (0, 0), "local": (off, off + rows), "global": (0, N),
+              "inner": (off // 2 + 3, N - 5)}[case.get("mode", "global")]
+    want = case.get("out", "both")
+    dbf = torch.full((rows, ld), NAN, dtype=BF, device=device) if want != "f32" else None
+    d32 = torch.full((rows, ld), NAN, device=device) if want != "bf16" else None
+    tod = lambda t: None if t is None else t.to(device, copy=True)  # noqa: E731
+    impl.contrastive_ce_grad(tod(sims), tod(ls), rows, N, off, eps, lw, tod(lse_row),
+                             None if hi <= lo else tod(lse_col), lo, hi, dbf, d32, tod(rw), tod(cw))
+    ar = torch.arange(rows)
+    t = torch.full((rows, N), eps / N, dtype=F64)
+    t[ar, off + ar] += 1 - eps
+    ex = (eT + 2 * U) * x.abs()
+    L1 = d64(lse_row)[:, None]
+    W1 = (lw * T64 * (d64(rw) if rw is not None else torch.full((rows,), 1.0 / rows, dtype=F64)))[:, None]
+    e1 = torch.exp(x - L1)
+    ref = W1 * (e1 - t)
+    err = _exp_term_err(W1, x, ex, L1, e1, t)
+    j = torch.arange(N)
+    W2 = lw * T64 * (d64(cw) if cw is not None else torch.full((N,), 1.0 / rows, dtype=F64))
+    W2 = torch.where((j >= lo) & (j < hi), W2, torch.zeros((), dtype=F64))[None, :]
+    L2 = torch.where(W2 != 0, d64(lse_col)[None, :], torch.zeros((), dtype=F64))
+    e2 = torch.exp(x - L2)
+    on = W2 != 0
+    ref = ref + torch.where(on, W2 * (e2 - t), torch.zeros((), dtype=F64))
+    err = err + torch.where(on, _exp_term_err(W2, x, ex, L2, e2, t), torch.zeros((), dtype=F64)) + U * ref.abs()
+    if dbf is not None:
+        got = dbf.cpu()
+        o.bf16("dsims_bf16", got[:, :N], ref, err=err)
+        o.exact("dsims_bf16_pad", got[:, N:], torch.full((rows, ld - N), NAN, dtype=BF))
+    if d32 is not None:
+        got = d32.cpu()
+        o.bound("dsims_f32", got[:, :N], ref, err)
+        o.exact("dsims_f32_pad", got[:, N:], torch.full((rows, ld - N), NAN))
+    return o.rec
+
+
+def _stats_launches(case, M):
+    """The launches of one fused-statistics case: (first B row, label0, part0) each over N = case["N"] columns.  World 1:
+    one launch with case["label0"] (default 0) at case["part0"] (default 0).  World W > 1 restates
+    engine_loss.contrastive_schedule on rank `rank` (B = M = N): one launch per peer r over its column block,
+    label0 = rank*B - r*B (negative, or >= N, when the label lies in another block), part0 = r * npp."""
+    N, W = case["N"], case.get("world", 1)
+    if W == 1:
+        return [(0, case.get("label0", 0), case.get("part0", 0))]
+    assert M == N
+    rank, npp = case["rank"], _cdiv(N, 128)
+    return [(r * N, rank * M - r * N, r * npp) for r in range(W)]
+
+
+def check_gemm_ce_stats(impl, device, case):
+    """Every float4 part {max, sum e^(x - max), sum e^(x - max) x, sum x} of every launch, the sums re-expressed
+    relative to the float64 part maximum (the kernel's own maximum is checked first, so a part is compared at the scale
+    it was formed at); parts no launch owns and xlabel entries whose label column no launch holds stay NaN."""
+    from multimodal_b200 import _lib
+
+    o = _Out("gemm_ce_stats")
+    g = _gen(case)
+    M, N, K, W = case["M"], case["N"], case["K"], case.get("world", 1)
+    npp = _cdiv(N, 128)
+    assert _lib.lib().mmb_gemm_ce_num_parts(N) == npp
+    launches = _stats_launches(case, M)
+    glab = torch.arange(M) + (case["rank"] * M if W > 1 else case.get("label0", 0))
+    A, Bfull = _pair(case, g, M, W * N, K, glab)
+    ls = torch.tensor([case.get("ls", _LS_CLIP)], dtype=F32)
+    P = max(p0 for _, _, p0 in launches) + npp + 1                 # one spare part past the last launch's
+    part = torch.full((M, P, 4), NAN, device=device)
+    xlabel = torch.full((M,), NAN, device=device)
+    Ad, lsd = A.to(device, copy=True), ls.to(device, copy=True)
+    with _gemm_mode(impl, case):
+        for b0, label0, part0 in launches:
+            impl.gemm_ce_stats(Ad, Bfull[b0:b0 + N].to(device, copy=True), lsd, label0, part, part0, xlabel)
+    got = part.cpu()
+    g64 = got.to(F64)
+    T64, eT = math.exp(ls.item()), _expf_rel(ls.item()).item()
+    written = torch.zeros(M, P, dtype=torch.bool)
+    cols = {k: ([], [], []) for k in ("max", "sum_e", "sum_ex", "sum_x")}    # got, ref, bound per part
+    xl_ref, xl_b = torch.full((M,), NAN, dtype=F64), torch.zeros(M, dtype=F64)
+    ar = torch.arange(M)
+    for b0, label0, part0 in launches:
+        acc, eacc = _gemm64(A, Bfull[b0:b0 + N])
+        x = T64 * acc
+        ex = T64 * eacc + (eT + 3 * U) * x.abs()
+        for p in range(npp):
+            xs, es = x[:, 128 * p:128 * (p + 1)], ex[:, 128 * p:128 * (p + 1)]
+            q = g64[:, part0 + p]
+            written[:, part0 + p] = True
+            mref, m = xs.amax(1), q[:, 0]
+            R = xs.abs().amax(1)
+            cols["max"][0].append(m), cols["max"][1].append(mref)
+            cols["max"][2].append(es.amax(1) + 5 * U * mref.abs())
+            e = torch.exp(xs - m[:, None])
+            rho = es + U * (xs - m[:, None]).abs() + 3 * U * m.abs()[:, None] + EX2
+            merge = 32 * U + 2 * (EX2 + 3 * U + 2 * U * R)
+            shift = torch.exp(m - mref)
+            eref = torch.exp(xs - mref[:, None])
+            for name, val, ref, b in (
+                    ("sum_e", q[:, 1], eref.sum(1), (e * rho).sum(1) + merge * e.sum(1) + 128 * TINY_P),
+                    ("sum_ex", q[:, 2], (eref * xs).sum(1),
+                     (e * (rho * xs.abs() + es)).sum(1) + (merge + U) * (e * xs.abs()).sum(1) + 128 * TINY_P * R)):
+                cols[name][0].append(val * shift), cols[name][1].append(ref), cols[name][2].append(b * shift)
+            cols["sum_x"][0].append(q[:, 3]), cols["sum_x"][1].append(xs.sum(1))
+            cols["sum_x"][2].append(es.sum(1) + 34 * U * xs.abs().sum(1))
+        lab = label0 + ar
+        hit = (lab >= 0) & (lab < N)
+        xl_ref[hit], xl_b[hit] = x[ar[hit], lab[hit]], ex[ar[hit], lab[hit]]
+    for name, (gv, rv, bv) in cols.items():
+        o.bound(name, torch.stack(gv, 1), torch.stack(rv, 1), torch.stack(bv, 1))
+    o.exact("untouched", got[~written], torch.full((int((~written).sum()), 4), NAN))
+    has = ~torch.isnan(xl_ref)
+    gx = xlabel.cpu()
+    o.bound("xlabel", gx[has], xl_ref[has], xl_b[has])
+    o.exact("xlabel_untouched", gx[~has], torch.full((int((~has).sum()),), NAN))
+    return o.rec
+
+
+def _logit_rows(case, g, rows, N, lab):
+    """float64 logits [rows, N] of the kind case["inputs"]: norm (the clamped-free CLIP scale times cosine similarities
+    of 64-wide unit rows), raw (N(0, 30^2)), peak (norm plus 60 at the label column), flat (14.3 + 1e-3 N(0, 1))."""
+    kind = case.get("inputs", "norm")
+    z = torch.randn(rows, N, generator=g, dtype=F64)
+    if kind == "raw":
+        return 30 * z
+    if kind == "flat":
+        return 14.3 + 1e-3 * z
+    x = z / 8 / 0.07
+    if kind == "peak":
+        x[torch.arange(rows), lab] += 60
+    else:
+        assert kind == "norm", kind
+    return x
+
+
+def check_ce_stats_reduce(impl, device, case):
+    """Parts formed in float64 per 128 columns of each of `world` launches of B columns (n_parts = world * npp,
+    n_total = world * B), rounded to fp32: the reduce's own contract, apart from the GEMM's.  A spare part past n_parts
+    is NaN and must not be read."""
+    o = _Out("ce_stats_reduce")
+    g = _gen(case)
+    rows, B, W, eps, lw = case["rows"], case["B"], case.get("world", 1), _f32(case.get("eps", 0.0)), 0.5
+    N, npp = W * B, _cdiv(B, 128)
+    n_parts = W * npp
+    ar = torch.arange(rows)
+    lab = (min(1, W - 1) * rows + ar) % N
+    x = _logit_rows(case, g, rows, N, lab)
+    parts = []
+    for r in range(W):
+        for p in range(npp):
+            xs = x[:, r * B + 128 * p:r * B + min(128 * (p + 1), B)]
+            m = xs.amax(1)
+            e = torch.exp(xs - m[:, None])
+            parts.append(torch.stack([m, e.sum(1), (e * xs).sum(1), xs.sum(1)], -1))
+    part = torch.full((rows, n_parts + 1, 4), NAN)
+    part[:, :n_parts] = torch.stack(parts, 1).to(F32)
+    xl = x[ar, lab].to(F32)
+    rw = _mask_weights(g, rows, zero=(0,), one=(rows - 1,)) if case.get("rw") else None
+    d0 = torch.tensor([0.375])
+    row_loss, lse = torch.full((rows,), NAN, device=device), torch.full((rows,), NAN, device=device)
+    dscale = d0.to(device, copy=True)
+    tod = lambda t: None if t is None else t.to(device, copy=True)  # noqa: E731
+    impl.ce_stats_reduce(tod(part), n_parts, tod(xl), rows, N, eps, lw, tod(rw), row_loss, lse, dscale)
+    m, y, z, w = d64(part[:, :n_parts]).unbind(-1)
+    mx = m.amax(1, keepdim=True)
+    f = torch.exp(m - mx)
+    S = (y * f).sum(1)
+    lse64 = mx.squeeze(1) + torch.log(S)
+    Ex = (z * f).sum(1) / S
+    mean = w.sum(1) / N
+    xl64 = d64(xl)
+    kc = _cdiv(n_parts, 32) + 5
+    eta = _expf_rel(m - mx) + U * (m - mx).abs() + U
+    rel_S = (y * f * eta).sum(1) / S + kc * U
+    b_lse = rel_S + 2 * U * torch.log(S).abs() + U * lse64.abs()
+    ez = z.abs() * f
+    b_E = ((ez * eta).sum(1) + kc * U * ez.sum(1)) / S + Ex.abs() * rel_S + 2 * U * Ex.abs()
+    b_mean = (kc + 1) * U * w.abs().sum(1) / N
+    loss = (1 - eps) * (lse64 - xl64) + eps * (lse64 - mean)
+    b_loss = b_lse + eps * b_mean + 3 * U * (lse64.abs() + xl64.abs() + mean.abs()) + U * loss.abs()
+    wrow = d64(rw) if rw is not None else torch.full((rows,), 1.0 / rows, dtype=F64)
+    if rw is not None:
+        o.bound("row_loss", row_loss, loss * wrow * rows, b_loss * wrow * rows + 3 * U * (loss * wrow * rows).abs())
+    else:
+        o.bound("row_loss", row_loss, loss, b_loss)
+    o.bound("lse", lse, lse64, b_lse)
+    dpart = (Ex - (1 - eps) * xl64 - eps * mean) * lw * wrow
+    b_dp = (b_E + eps * b_mean + 3 * U * (Ex.abs() + xl64.abs() + mean.abs())) * lw * wrow + 3 * U * dpart.abs()
+    kr = _cdiv(rows, 8) + 8 + 1
+    o.bound("dscale", dscale, d64(d0) + dpart.sum(), b_dp.sum() + kr * U * (dpart.abs().sum() + abs(d0.item())))
+    return o.rec
+
+
+def check_gemm_ce_grad(impl, device, case):
+    """engine_loss.contrastive_schedule's gradient launches on rank `rank` of `world` (B rows, N = world * B): one per
+    peer block r with label0 = rank*B - r*B, the transposed range clipped to the block and lse_col / col_w sliced to
+    it, each writing a column slice of one NaN-filled dsims buffer wider than [B, N] in both dimensions.  lse_row and
+    lse_col are the fp32-rounded float64 row LSEs of the two directions.  case["refused"]: a launch over an N that is
+    not a multiple of 8 (a bf16 output) raises MMBError and writes nothing."""
+    from multimodal_b200._lib import MMBError
+
+    o = _Out("gemm_ce_grad")
+    g = _gen(case)
+    B, K, W = case["B"], case["K"], case.get("world", 1)
+    rank = case.get("rank", 0)
+    N, lab = W * B, rank * B
+    eps, lw = _f32(case.get("eps", 0.0)), 0.5
+    a_all, b_all = _pair(case, g, N, N, K, torch.arange(N))
+    A = a_all[lab:lab + B]
+    ls = torch.tensor([case.get("ls", _LS_CLIP)], dtype=F32)
+    T64, eT = math.exp(ls.item()), _expf_rel(ls.item()).item()
+    acc, eacc = _gemm64(A, b_all)
+    x = T64 * acc
+    lse_row = torch.logsumexp(x, 1).to(F32)
+    lse_col = torch.logsumexp(T64 * _gemm64(b_all, a_all)[0], 1).to(F32)
+    cw = rw = None
+    if case.get("rw"):
+        cw = torch.cat([_mask_weights(g, B, zero=(0,), one=(B - 1,)) for _ in range(W)])
+        rw = cw[lab:lab + B].clone()
+        if case.get("bad"):
+            z = (cw == 0).nonzero().view(-1)
+            lse_col[z] = torch.tensor([NAN, float("-inf"), float("inf")])[torch.arange(z.numel()) % 3]
+    mode = case.get("mode", "global")
+    lo, hi = {"none": (0, 0), "local": (lab, lab + B), "global": (0, N), "inner": (lab // 2 + 3, N - 5)}[mode]
+    tod = lambda t: None if t is None else t.to(device, copy=True)  # noqa: E731
+    Ad, lsd, lrd, rwd, cwd = tod(A), tod(ls), tod(lse_row), tod(rw), tod(cw)
+    LBd = None if mode == "none" else tod(lse_col)
+    DS = torch.full((B + 3, N + 16), NAN, dtype=BF, device=device)
+    if case.get("refused"):
+        try:
+            impl.gemm_ce_grad(Ad, tod(b_all), lsd, lab, N, B, eps, lw, lrd, rwd, LBd, cwd, lo, hi, DS[:B, :N])
+        except MMBError:
+            o.exact("untouched", DS.cpu(), torch.full(DS.shape, NAN, dtype=BF))
+            return o.rec
+        raise AssertionError(f"gemm_ce_grad accepted a bf16 output of {N} columns")
+    with _gemm_mode(impl, case):
+        for r in range(W):
+            c0 = r * B
+            clo, chi = min(max(lo - c0, 0), B), min(max(hi - c0, 0), B)
+            sl = slice(c0, c0 + B)
+            impl.gemm_ce_grad(Ad, tod(b_all[sl]), lsd, lab - c0, N, B, eps, lw, lrd, rwd,
+                              LBd[sl] if (LBd is not None and chi > clo) else None,
+                              cwd[sl] if cwd is not None else None, clo, chi, DS[:B, sl])
+    ar = torch.arange(B)
+    t = torch.full((B, N), eps / N, dtype=F64)
+    t[ar, lab + ar] += 1 - eps
+    ex = T64 * eacc + (eT + 3 * U) * x.abs()
+    L1 = d64(lse_row)[:, None]
+    W1 = (lw * T64 * (d64(rw) if rw is not None else torch.full((B,), 1.0 / B, dtype=F64)))[:, None]
+    e1 = torch.exp(x - L1)
+    ref = W1 * (e1 - t)
+    err = _exp_term_err(W1, x, ex, L1, e1, t)
+    j = torch.arange(N)
+    W2 = lw * T64 * (d64(cw) if cw is not None else torch.full((N,), 1.0 / B, dtype=F64))
+    W2 = torch.where((j >= lo) & (j < hi), W2, torch.zeros((), dtype=F64))[None, :]
+    on = W2 != 0
+    L2 = torch.where(on, d64(lse_col)[None, :], torch.zeros((), dtype=F64))
+    e2 = torch.exp(x - L2)
+    ref = ref + torch.where(on, W2 * (e2 - t), torch.zeros((), dtype=F64))
+    err = err + torch.where(on, _exp_term_err(W2, x, ex, L2, e2, t), torch.zeros((), dtype=F64)) + U * ref.abs()
+    got = DS.cpu()
+    o.bf16("dsims", got[:B, :N], ref, err=err)
+    o.exact("untouched", torch.cat([got[B:].reshape(-1), got[:B, N:].reshape(-1)]),
+            torch.full((3 * (N + 16) + 16 * B,), NAN, dtype=BF))
+    return o.rec
+
+
+def check_linear_cross_entropy(impl, device, case):
+    """Linear (no bias) -> CrossEntropy(ignore_index) over a vocabulary: the fused statistics GEMM with explicit labels
+    (T = __expf(0)) and ce_labels_reduce.  Its lse carries the EPI_CE_STATS errors (per-element x and ex2 errors, the
+    max mismatch m2 ln2 vs the stored max, 32 + quad-merge roundings) and the reduce's (__expf of m_p - max, its
+    ceil(n_parts / 32) + 5 chain, logf)."""
+    o = _Out("linear_cross_entropy")
+    g = _gen(case)
+    M, V, K, ignore = case["M"], case["V"], case["K"], case.get("ignore", -100)
+    h = torch.randn(M, K, generator=g).to(BF)
+    w = (torch.randn(V, K, generator=g) * (3.0 / math.sqrt(K))).to(BF)
+    lab = torch.randint(1 if ignore == 0 else 0, V, (M,), generator=g)
+    lab[0] = V - 1
+    nig = M if case.get("n_ignored") == "all" else case.get("n_ignored", 0)
+    lab[torch.randperm(M, generator=g)[:nig]] = ignore
+    acc0 = torch.tensor([1.5, 2.0])
+    accum = acc0.to(device, copy=True)
+    row_loss = torch.full((M,), NAN, device=device)
+    with _gemm_mode(impl, case):
+        impl.linear_cross_entropy(h.to(device, copy=True), w.to(device, copy=True),
+                                  lab.to(torch.int32).to(device), ignore, accum, row_loss)
+    x, eacc = _gemm64(h, w)
+    ex = eacc + (_expf_rel(0.0).item() + 3 * U) * x.abs()
+    keep = lab != ignore
+    lse = torch.logsumexp(x, 1)
+    p = torch.exp(x - lse[:, None])
+    mx, R = x.amax(1), x.abs().amax(1)
+    span = mx - x.amin(1)
+    kc = _cdiv(_cdiv(V, 128), 32) + 5
+    b_lse = (p * ex).sum(1) + U * span + 3 * U * R + EX2 + 32 * U + 2 * (EX2 + 3 * U + 2 * U * R) \
+        + _expf_rel(span) + U * span + U + kc * U + 2 * U * (lse - mx).abs() + U * lse.abs() + V * TINY_P
+    ar = torch.arange(M)
+    lc = lab.clamp(0, V - 1)
+    xl = x[ar, lc]
+    zero = torch.zeros((), dtype=F64)
+    nll = torch.where(keep, lse - xl, zero)
+    b_row = torch.where(keep, b_lse + ex[ar, lc] + 2 * U * (lse.abs() + xl.abs()) + U * nll.abs(), zero)
+    o.bound("row_loss", row_loss, nll, b_row)
+    kr = _cdiv(M, 8) + 8 + 1
+    o.bound("accum", accum, torch.stack([d64(acc0)[0] + nll.sum(), d64(acc0)[1] + keep.sum().to(F64)]),
+            torch.stack([b_row.sum() + kr * U * (nll.abs().sum() + abs(acc0[0].item())), zero]))
+    return o.rec
+
+
+def _both_modes(cases):
+    return [dict(c, gemm_mode=m) for c in cases for m in (0, 1)]
+
+
+_CONTRASTIVE_STATS = [
+    {"rows": 7, "N": 7, "off": 0, "eps": 0.1},
+    {"rows": 5, "N": 256, "off": 251, "eps": 0.05, "rw": True, "ld": 264, "logits": True, "ls": _LS_MAX},
+    {"rows": 9, "N": 300, "off": 100, "inputs": "raw", "logits": True},
+    {"rows": 6, "N": 70, "off": 64, "eps": 0.1, "rw": True, "inputs": "peak", "ls": _LS_MAX, "ld": 77},
+    {"rows": 4, "N": 600, "off": 596, "eps": 0.05, "inputs": "flat"},
+    {"rows": 300, "N": 1024, "off": 724, "eps": 0.1},
+    {"rows": 1000, "N": 4000, "off": 3000, "eps": 0.1, "gpu": True},
+    {"rows": 257, "N": 1032, "rw": True, "inputs": "peak", "eps": 0.1, "ls": _LS_MAX, "logits": True, "gpu": True},
+]
+_CONTRASTIVE_GRAD = [
+    {"rows": 6, "N": 20, "off": 8, "mode": "none", "eps": 0.1},
+    {"rows": 6, "N": 20, "off": 8, "mode": "local", "rw": True, "out": "f32"},
+    {"rows": 5, "N": 300, "off": 295, "mode": "global", "eps": 0.05, "rw": True, "bad": True, "ld": 304,
+     "ls": _LS_MAX},
+    {"rows": 8, "N": 256, "mode": "inner", "inputs": "peak", "eps": 0.1, "out": "bf16"},
+    {"rows": 7, "N": 64, "off": 57, "mode": "global", "inputs": "raw", "rw": True, "bad": True},
+    {"rows": 4, "N": 130, "off": 3, "mode": "global", "inputs": "flat"},
+    {"rows": 300, "N": 1024, "off": 724, "mode": "global", "rw": True, "bad": True, "eps": 0.1, "gpu": True},
+]
+# M 1 .. 1000 and N 64 .. 1032 on both sides of the 128-column part and 256-column tile boundaries (N = 130: a second
+# half of one column; N = 255: one half present in the last tile), K tails shorter than one 64-deep k-block, world 2 / 3
+# launch sets, and a 2000 x 2600 case with more tiles than SMs in either mode (the persistent grid loops).
+_GEMM_CE_STATS = _both_modes([
+    {"M": 1, "N": 64, "K": 8},
+    {"M": 127, "N": 130, "K": 72, "inputs": "raw", "label0": 3, "part0": 1},
+    {"M": 129, "N": 255, "K": 136, "inputs": "peak", "ls": _LS_MAX},
+    {"M": 64, "N": 64, "K": 72, "world": 3, "rank": 1, "inputs": "peak"},
+    {"M": 130, "N": 130, "K": 8, "world": 2, "rank": 1, "inputs": "flat", "ls": _LS_MAX},
+    {"M": 255, "N": 256, "K": 768, "gpu": True},
+    {"M": 257, "N": 600, "K": 136, "inputs": "raw", "label0": -100, "gpu": True},
+    {"M": 1000, "N": 1032, "K": 768, "inputs": "peak", "ls": _LS_MAX, "gpu": True},
+    {"M": 264, "N": 264, "K": 136, "world": 3, "rank": 2, "gpu": True},
+    {"M": 2000, "N": 2600, "K": 136, "gpu": True},
+])
+_CE_STATS_REDUCE = [
+    {"rows": 5, "B": 200, "world": 3, "eps": 0.1},
+    {"rows": 8, "B": 130, "world": 2, "rw": True, "inputs": "raw"},
+    {"rows": 3, "B": 64, "eps": 0.05, "inputs": "peak"},
+    {"rows": 6, "B": 1032, "world": 4, "eps": 0.1, "rw": True, "inputs": "flat"},       # 36 parts: two per lane
+    {"rows": 1000, "B": 1032, "world": 2, "eps": 0.1, "gpu": True},
+    {"rows": 300, "B": 4096, "world": 2, "rw": True, "eps": 0.05, "inputs": "raw", "gpu": True},
+]
+_GEMM_CE_GRAD = _both_modes([
+    {"B": 64, "K": 72, "mode": "global", "eps": 0.1, "rw": True, "bad": True},
+    {"B": 64, "K": 8, "world": 3, "rank": 1, "mode": "local", "eps": 0.05, "inputs": "peak"},
+    {"B": 128, "K": 136, "world": 2, "rank": 1, "mode": "inner", "eps": 0.1, "rw": True, "bad": True, "ls": _LS_MAX},
+    {"B": 136, "K": 72, "world": 2, "mode": "none", "inputs": "raw"},
+    {"B": 64, "K": 72, "world": 2, "mode": "inner", "eps": 0.05},
+    {"B": 8, "K": 8, "world": 3, "rank": 2, "mode": "global", "eps": 0.1, "inputs": "flat"},
+    {"B": 256, "K": 768, "world": 2, "rank": 1, "mode": "global", "eps": 0.1, "rw": True, "bad": True, "gpu": True},
+    {"B": 1032, "K": 136, "inputs": "peak", "ls": _LS_MAX, "gpu": True},
+    {"B": 600, "K": 136, "world": 3, "rank": 2, "mode": "inner", "eps": 0.05, "inputs": "raw", "gpu": True},
+    {"B": 2600, "K": 72, "mode": "local", "eps": 0.1, "gpu": True},
+]) + [{"B": 255, "K": 72, "refused": True}]
+_LINEAR_CE = _both_modes([
+    {"M": 6, "V": 49408, "K": 8, "ignore": 0, "n_ignored": 2},
+    {"M": 5, "V": 1001, "K": 72},
+    {"M": 4, "V": 49408, "K": 72, "n_ignored": "all"},
+    {"M": 127, "V": 255, "K": 136, "ignore": 0, "n_ignored": 20},
+    {"M": 257, "V": 49408, "K": 136, "ignore": 0, "n_ignored": 40, "gpu": True},
+    {"M": 1000, "V": 1001, "K": 768, "n_ignored": 100, "gpu": True},
+])
+
 # ---- cases -----------------------------------------------------------------------------------------------------------------
 _WIDTHS = [128 * nv for nv in range(1, 9)]
 
@@ -1664,11 +2226,18 @@ CASES = {
     "attention_fwd_generic": _GENERIC,
     "attention_bwd_generic": _GENERIC,
     "attention_fwd_decode": _DECODE,
+    "contrastive_ce_stats": _CONTRASTIVE_STATS,
+    "contrastive_ce_grad": _CONTRASTIVE_GRAD,
+    "gemm_ce_stats": _GEMM_CE_STATS,
+    "ce_stats_reduce": _CE_STATS_REDUCE,
+    "gemm_ce_grad": _GEMM_CE_GRAD,
+    "linear_cross_entropy": _LINEAR_CE,
 }
 
 # Kernels whose results DESIGN.md §4 documents as run-to-run bit-exact (no floating-point atomics).
 DETERMINISTIC = ["layernorm_bwd", "vit_embed_ln_bwd", "batch_sum", "colsum_bf16", "text_embed_bwd", "ce_labels",
-                 "sum_scale"]
+                 "sum_scale", "contrastive_ce_stats", "contrastive_ce_grad", "gemm_ce_stats", "ce_stats_reduce",
+                 "gemm_ce_grad", "linear_cross_entropy"]
 
 CHECKS = {op: globals()["check_" + op] for op in CASES}
 

@@ -16,7 +16,7 @@ def emu(monkeypatch):
 
 @pytest.mark.parametrize("name", list(CC.CASES))
 def test_coca_training_schedule_against_oracle_with_emulated_kernels(emu, name):
-    G.coca_grad_parity(torch.device("cpu"), name, "cpu_emu_" + name, with_contrastive=False)
+    G.coca_grad_parity(torch.device("cpu"), name, "cpu_emu_" + name)
 
 
 @pytest.mark.parametrize("masked", [False, True])

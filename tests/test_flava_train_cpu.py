@@ -40,9 +40,9 @@ def test_flava_mm_direct_call_and_frozen_encoder_with_emulated_kernels(emu):
 
 @pytest.mark.parametrize("name", ["unimodal", "multimodal"])
 def test_pretraining_loss_gradients_with_emulated_kernels(emu, name):
-    """Head schedules (engine_flava_heads.py) on the emulated kernels; the contrastive loss's kernels are not emulated
-    (weight 0 here), its backward is covered on the GPU."""
-    G._loss_grad_parity(torch.device("cpu"), name, 0.0, "cpu_emu_" + name)
+    """Head schedules (engine_flava_heads.py) and the global contrastive loss (engine_loss.py: the batch of 5 takes the
+    exact-fp32 SIMT schedule) on the emulated kernels."""
+    G._loss_grad_parity(torch.device("cpu"), name, 1.0, "cpu_emu_" + name)
 
 
 def test_flava_for_pretraining_step_with_emulated_kernels(emu):
@@ -55,7 +55,6 @@ def test_flava_for_pretraining_step_with_emulated_kernels(emu):
     from multimodal_b200.modules.losses.flava import FLAVAPretrainingLoss
 
     m = PC.build_model(flava_model, FLAVAForPreTraining, FLAVAPretrainingLoss).train()
-    m.loss.contrastive_loss_weight = 0.0      # its kernels are not emulated; covered on the GPU
     inp, _ = PC.model_inputs()
     out = m(**inp)
     total = sum(v for v in out.losses.values() if v is not None)
@@ -72,8 +71,12 @@ def test_flava_for_pretraining_step_with_emulated_kernels(emu):
     img_m = FO.image_encoder(inp["image"], msd, cfg, keep)
     txt_m = FO.text_encoder(inp["text_masked"], msd, cfg)
     mm = FO.mm_encoder(img_m["hidden_states"][-1], txt_m["hidden_states"][-1], msd, cfg)["last_hidden_state"]
-    kw = dict(multimodal_masked_sequence=mm, mlm_labels=inp["mlm_labels"], mim_labels=mim, itm_labels=inp["itm_labels"])
-    ref_total, parts = G._oracle_loss_total(lsd, kw, dict(contrastive=0.0))
+    img = FO.image_encoder(inp["image"], msd, cfg)["last_hidden_state"][:, 0]
+    txt = FO.text_encoder(inp["text"], msd, cfg)["last_hidden_state"][:, 0]
+    kw = dict(multimodal_masked_sequence=mm, mlm_labels=inp["mlm_labels"], mim_labels=mim, itm_labels=inp["itm_labels"],
+              projected_image_embeddings=FO._lin(img, msd, "image_projection"),
+              projected_text_embeddings=FO._lin(txt, msd, "text_projection"))
+    ref_total, parts = G._oracle_loss_total(lsd, kw, dict(contrastive=m.loss.contrastive_loss_weight))
     ref_total.backward()
     assert abs(total.item() - ref_total.item()) < 2e-2 * max(1.0, abs(ref_total.item())), (total.item(), ref_total.item())
     n = 0

@@ -149,28 +149,3 @@ def test_f32_output_not_16_byte_aligned(dev, gemm_mode):
     assert _rel(out, 2 * ref) < 2e-5 * math.sqrt(K) + 1e-5
     assert full[:, 0].abs().max().item() == 0 and full[:, N + 1:].abs().max().item() == 0
 
-
-@pytest.mark.parametrize("M,N", [(300, 264), (513, 520), (1024, 1032)])
-def test_ce_stats_parts_per_128_columns(dev, gemm_mode, M, N):
-    """The fused cross-entropy statistics keep one part per 128 columns although a tile is 256 columns wide."""
-    from multimodal_b200 import ops
-
-    K = 136
-    A2, B2, _, _ = _operands(dev, M, N, K, 0, 0, seed=7)
-    log_scale = torch.tensor([math.log(10.0)], device=dev)
-    parts = ops.gemm_ce_num_parts(N)
-    assert parts == (N + 127) // 128
-    part = torch.full((M, parts + 1, 4), 7.0, device=dev)   # one spare part: must stay untouched
-    xlabel = torch.zeros(M, device=dev)
-    ops.gemm_ce_stats(A2, B2, log_scale, 0, part, 0, xlabel)
-    torch.cuda.synchronize()
-    logits = 10.0 * (A2.float() @ B2.float().t())
-    for p in range(parts):
-        blk = logits[:, 128 * p:128 * (p + 1)]
-        mx = blk.max(1).values
-        torch.testing.assert_close(part[:, p, 0], mx, rtol=1e-5, atol=1e-3)
-        torch.testing.assert_close(part[:, p, 1], torch.exp(blk - mx[:, None]).sum(1), rtol=1e-3, atol=1e-4)
-        torch.testing.assert_close(part[:, p, 3], blk.sum(1), rtol=1e-4, atol=1e-2 * blk.abs().sum(1).max().item() / 128)
-    assert (part[:, parts] == 7.0).all()
-    diag = torch.arange(min(M, N), device=dev)
-    torch.testing.assert_close(xlabel[diag], logits[diag, diag], rtol=1e-5, atol=1e-3)

@@ -26,17 +26,11 @@ ALLOWLIST = {
     "self_attention": "test_attention_router_cpu.py",
     "clip_image_transform": "test_gpu_clip_transform.py",
     "clip_image_transform_max_taps": "test_clip_transform_cpu.py",
-    "gemm_ce_stats": "test_gpu_gemm_wide.py",
-    "gemm_ce_grad": "test_gpu_gemm_wide.py",
-    "linear_cross_entropy": "test_gpu_coca_train.py",
-    "ce_stats_reduce": "test_gpu_parity.py",
-    "contrastive_ce_stats": "test_gpu_parity.py",
-    "contrastive_ce_grad": "test_gpu_parity.py",
     "adamw_step": "test_gpu_optim.py",
     "anyprecision_adamw_step": "test_gpu_optim.py",
     # pure host helpers
     "wgrad_splits": "test_abi_cpu.py",
-    "gemm_ce_num_parts": "test_gpu_gemm_wide.py",
+    "gemm_ce_num_parts": "test_kernel_contracts_cpu.py",   # asserted by check_gemm_ce_stats
     "attention_decode_splits": "test_gpu_decoder_cache.py",
     "decode_attention_wins": "test_decoder_cache_cpu.py",
 }
@@ -216,6 +210,80 @@ def _probs_next_row_lse(qkv, lse, kmask, probs, B, S, H, causal, scale):
                             scale)
 
 
+def _reduce_without_rescale(part, n_parts, xlabel, rows, n_total, smoothing, loss_weight, row_w, row_loss, lse_out,
+                            dscale_accum):
+    """ce_stats_reduce adding every part's sums as they are, without rescaling them to the row's common maximum."""
+    q = part.clone()
+    mx = q[:rows, :n_parts, 0].amax(1, keepdim=True)
+    q[:rows, :n_parts, 0] = mx
+    emu_ops.ce_stats_reduce(q, n_parts, xlabel, rows, n_total, smoothing, loss_weight, row_w, row_loss, lse_out,
+                            dscale_accum)
+
+
+def _grad_smoothing_over_launch_n(A, B, log_scale, label0, n_total, *rest):
+    emu_ops.gemm_ce_grad(A, B, log_scale, label0, B.shape[0], *rest)
+
+
+def _grad_transposed_range_inclusive(A, B, log_scale, label0, n_total, rows_total, smoothing, loss_weight, lse_row,
+                                     row_w, lse_col, col_w, col_lo, col_hi, dsims):
+    emu_ops.gemm_ce_grad(A, B, log_scale, label0, n_total, rows_total, smoothing, loss_weight, lse_row, row_w, lse_col,
+                         col_w, col_lo, col_hi + 1, dsims)
+
+
+def _grad_transposed_row_weights(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, lse_row, lse_col,
+                                 col_lo, col_hi, dsims_bf16, dsims_f32, row_w=None, col_w=None):
+    """contrastive_ce_grad weighting the transposed term of element (i, j) with row i's weight instead of column j's."""
+    g = torch.zeros(rows, N)
+    emu_ops.contrastive_ce_grad(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, lse_row, None, 0, 0,
+                                None, g, row_w, None)
+    if lse_col is not None and col_hi > col_lo and row_w is not None:
+        T = torch.exp(logit_scale.reshape(-1)[:1])
+        j = slice(col_lo, col_hi)
+        t = torch.full((rows, N), smoothing / N)
+        t[torch.arange(rows), label_offset + torch.arange(rows)] += 1 - smoothing
+        wc = (loss_weight * T * row_w[:rows])[:, None]
+        add = wc * (torch.exp(T * sims[:rows, j] - lse_col[j]) - t[:, j])
+        g[:, j] += torch.where(wc != 0, add, torch.zeros_like(add))
+    elif lse_col is not None:
+        emu_ops.contrastive_ce_grad(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, lse_row, lse_col,
+                                    col_lo, col_hi, None, g, row_w, col_w)
+    if dsims_bf16 is not None:
+        dsims_bf16[:rows, :N] = g.to(torch.bfloat16)
+    if dsims_f32 is not None:
+        dsims_f32[:rows, :N] = g
+
+
+def _stats_xlabel_at_row(A, B, log_scale, label0, part, part0, xlabel):
+    """gemm_ce_stats taking row r's label at this launch's column r instead of label0 + r."""
+    x = xlabel.clone()
+    emu_ops.gemm_ce_stats(A, B, log_scale, label0, part, part0, x)
+    emu_ops.gemm_ce_stats(A, B, log_scale, 0, part.clone(), part0, xlabel)
+
+
+def _stats_drops_second_half(A, B, log_scale, label0, part, part0, xlabel):
+    """gemm_ce_stats leaving the second 128-column part of a partial last tile unwritten."""
+    N = B.shape[0]
+    keep = part.clone()
+    emu_ops.gemm_ce_stats(A, B, log_scale, label0, part, part0, xlabel)
+    if N % 256 > 128:
+        p = part0 + 2 * (N // 256) + 1
+        part[:, p] = keep[:, p]
+
+
+def _stats_dscale_unweighted(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, row_loss, lse_out,
+                             dscale_accum, logits_out=None, row_w=None):
+    """contrastive_ce_stats weighting every row's d loss / d log_scale share by 1 / rows whatever row_w says."""
+    emu_ops.contrastive_ce_stats(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, row_loss, lse_out,
+                                 None, logits_out, row_w)
+    emu_ops.contrastive_ce_stats(sims, logit_scale, rows, N, label_offset, smoothing, loss_weight, None, None,
+                                 dscale_accum, None, None)
+
+
+def _linear_ce_counts_ignored(hidden, weight, labels, ignore_index, accum, row_loss=None):
+    emu_ops.linear_cross_entropy(hidden, weight, labels, ignore_index, accum, row_loss)
+    accum[1] += (labels == ignore_index).sum()
+
+
 MUTANTS = {
     "cast truncates instead of rounding": ("cast_bf16", "cast_bf16", _truncating_cast_bf16),
     "LayerNorm backward skips the last row": ("layernorm_bwd", "layernorm_bwd", _ln_bwd_skips_last_row),
@@ -239,6 +307,19 @@ MUTANTS = {
     "decode splits combined without rescaling to the common max":
         ("attention_fwd_decode", "attention_fwd_decode", _decode_combine_unscaled),
     "attention_probs uses the lse of the next row": ("attention_probs", "attention_probs", _probs_next_row_lse),
+    "ce_stats_reduce sums the parts without rescaling them to the common max":
+        ("ce_stats_reduce", "ce_stats_reduce", _reduce_without_rescale),
+    "smoothing term divided by the launch's N instead of n_total":
+        ("gemm_ce_grad", "gemm_ce_grad", _grad_smoothing_over_launch_n),
+    "transposed term applied on [col_lo, col_hi]": ("gemm_ce_grad", "gemm_ce_grad", _grad_transposed_range_inclusive),
+    "transposed term weighted by row_w instead of col_w":
+        ("contrastive_ce_grad", "contrastive_ce_grad", _grad_transposed_row_weights),
+    "gemm_ce_stats writes xlabel at column r instead of label0 + r":
+        ("gemm_ce_stats", "gemm_ce_stats", _stats_xlabel_at_row),
+    "gemm_ce_stats drops the second 128-column part of a partial tile":
+        ("gemm_ce_stats", "gemm_ce_stats", _stats_drops_second_half),
+    "contrastive_ce_stats ignores row_w in dscale": ("contrastive_ce_stats", "contrastive_ce_stats", _stats_dscale_unweighted),
+    "linear_cross_entropy counts ignored rows": ("linear_cross_entropy", "linear_cross_entropy", _linear_ce_counts_ignored),
 }
 
 
