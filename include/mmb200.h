@@ -226,6 +226,24 @@ int mmb_bert_embed_ln_bwd(const long long* ids, const long long* type_ids, const
  * patch-projection weight gradient), dmask_token += sum of the masked rows' g.  dcls / dpos: mmb_batch_sum of g. */
 int mmb_vit_assemble_bwd(const float* g, const unsigned char* patch_mask, void* dpatch_bf16, float* dmask_token, int B,
                          int S, int d, int has_cls, void* stream);
+/* ---- Random patch dropping (FLIP: PatchEmbeddings(patch_drop_rate=...), modules/layers/patch_embedding.py:104-154,
+ * modules/masking/random_masking.py).  keep: int32 [B, L], per sample L distinct patch indices in [0, P) in the order
+ * the tokens take (an index outside [0, P) traps).  P = (H/ps)*(W/ps); off = 1 with a CLS token, else 0. */
+/* mmb_im2col_patches on the kept patches only: out row b*L+j = patch keep[b,j] of image b (same K order and pitch). */
+int mmb_im2col_patches_gather(const float* img, const int* keep, void* out_bf16, long long ld_out, int B, int H, int W,
+                              int ps, int L, void* stream);
+/* x [B, off+L, d] fp32: x[b,0] = cls + pos[0] (cls != NULL); x[b,off+j] = (mask[b,p] ? mask_token : patch_out[b*L+j])
+ * + pos[off+p], p = keep[b,j]; patch_out bf16 [B*L, d], patch_mask uint8 [B, P] (optional, indexed by patch). */
+int mmb_vit_assemble_gather_fwd(const void* patch_out_bf16, const float* cls, const float* pos, const float* mask_token,
+                                const unsigned char* patch_mask, const int* keep, float* x, int B, int L, int P, int d,
+                                void* stream);
+/* Backward of mmb_vit_assemble_gather_fwd from g fp32 [B, off+L, d]: dpatch[b*L+j] = bf16(mask ? 0 : g[b,off+j]);
+ * dmask_token += sum of the masked kept rows; dcls += sum_b g[b,0]; dpos[0] += sum_b g[b,0] (with cls) and
+ * dpos[off+p] += sum over the samples b that kept p of g[b, off+j(b,p)] (+= 0 for a patch no sample kept).  dmask_token,
+ * dcls and dpos may each be NULL.  No atomics: the sums run in a fixed order, run-to-run bit-identical. */
+int mmb_vit_assemble_gather_bwd(const float* g, const unsigned char* patch_mask, const int* keep, void* dpatch_bf16,
+                                float* dmask_token, float* dcls, float* dpos, int B, int L, int P, int d, int has_cls,
+                                void* stream);
 /* Inverse of mmb_concat_tokens for gradients: g [B, cls+Sa+Sb, d] fp32 -> bf16 [B*Sa, d] and [B*Sb, d]. */
 int mmb_split_tokens_cast(const float* g, void* a_bf16, void* b_bf16, int B, int Sa, int Sb, int d, int has_cls,
                           void* stream);

@@ -38,9 +38,10 @@ void* scratch(int slot, size_t bytes, cudaStream_t stream);
 // SCR_ATTN_D: rowsum(dO * O) of the streamed attention backward, fp32 [B*H*S], written by its dQ kernel and read by its
 // dK / dV kernel.  SCR_ATTN_DQ: fp32 per-batch-chunk sums of dQ of the streamed general attention backward
 // (attention_generic_stream.cu), added into dq_f32 in chunk order.  SCR_ATTN_DEC: fp32 per-split partials (O, m, l) of
-// the split-KV decode attention (attention_decode.cu), added in split order by its combine kernel
+// the split-KV decode attention (attention_decode.cu), added in split order by its combine kernel.  SCR_PATCH_DROP: the
+// keep-index inverse map and the position / mask-token partials of the gathered token-assembly backward (patch_drop.cu)
 enum ScratchSlot { SCR_GEMM_SPLITK = 0, SCR_GEMM_COLSUM, SCR_LN_BWD, SCR_COLSUM, SCR_BATCH_SUM, SCR_LOSS, SCR_ATTN_D,
-                   SCR_ATTN_DQ, SCR_ATTN_DEC, SCR_COUNT };
+                   SCR_ATTN_DQ, SCR_ATTN_DEC, SCR_PATCH_DROP, SCR_COUNT };
 // out[n] (+)= sum_{p = 0..P-1} part[p * ldp + n] for n < N, summed in increasing p (accumulate = 0: out is overwritten).
 int reduce_partials(const float* part, int P, int N, long long ldp, float* out, int accumulate, cudaStream_t stream);
 }  // namespace mmb

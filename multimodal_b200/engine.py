@@ -253,23 +253,29 @@ def wants_grad(*mods: Optional[nn.Module]) -> bool:
 
 def patch_embed_fwd(image: torch.Tensor, conv: nn.Module, wconv: torch.Tensor, cls: Optional[torch.Tensor],
                     pos: torch.Tensor, mask_token: Optional[torch.Tensor], image_patches_mask: Optional[torch.Tensor],
-                    ws: Workspace, save: Workspace, prefix: str):
+                    ws: Workspace, save: Workspace, prefix: str, keep: Optional[torch.Tensor] = None):
     """Patch front end of a ViT (patch_embedding.py:104-154, image_encoder.py:139-175): im2col + conv GEMM (+ bias), then
     [cls |] patch or mask token, + position embeddings, in one assembly kernel.  wconv: bf16 [d, 3*ps*ps] conv weight.
+    keep (int32 [B, L], random patch dropping): only the kept patches are embedded, token off+j being patch keep[b, j].
     The im2col matrix goes to `save` (the conv weight gradient reads it), the rest of the scratch to `ws`.
-    Returns (X0 fp32 [B*S, d], allocated per call; B, S, P; the uint8 [B, P] patch mask or None)."""
+    Returns (X0 fp32 [B*S, d], allocated per call; B, S = off + L (L = P without keep), P; the uint8 [B, P] patch mask
+    or None)."""
     d, ps = conv.weight.shape[0], conv.weight.shape[2]
     image = image.contiguous().float()
     B, _, Hh, Ww = image.shape
     P = (Hh // ps) * (Ww // ps)
-    S = P + (1 if cls is not None else 0)
+    L = P if keep is None else keep.shape[1]
+    S = L + (1 if cls is not None else 0)
     K = 3 * ps * ps
     Kp = -(-K // 8) * 8   # row pitch: bf16 rows must be 16 B multiples for TMA (K = 588 -> 592 for 14x14 patches)
     bf = torch.bfloat16
-    PATCH = save.get(f"{prefix}.PATCH", (B * P, Kp), bf)[:, :K]
-    PO = ws.get(f"{prefix}.PO", (B * P, d), bf)
+    PATCH = save.get(f"{prefix}.PATCH", (B * L, Kp), bf)[:, :K]
+    PO = ws.get(f"{prefix}.PO", (B * L, d), bf)
     X0 = torch.empty((B * S, d), device=image.device, dtype=torch.float32)
-    ops.im2col(image, ps, PATCH)
+    if keep is None:
+        ops.im2col(image, ps, PATCH)
+    else:
+        ops._im2col_gather(image, keep, ps, PATCH)
     if Kp != K:   # re-pitch the (tiny) conv weight shadow the same way
         wp = ws.get(f"{prefix}.WCONV", (d, Kp), bf)[:, :K]
         wp.copy_(wconv)
@@ -278,26 +284,37 @@ def patch_embed_fwd(image: torch.Tensor, conv: nn.Module, wconv: torch.Tensor, c
     pm = None
     if image_patches_mask is not None and mask_token is not None:
         pm = image_patches_mask.reshape(B, P).to(torch.uint8).contiguous()
-    ops.vit_assemble_fwd(PO, cls, pos, mask_token if pm is not None else None, pm, X0, B, S, d)
+    mt = mask_token if pm is not None else None
+    if keep is None:
+        ops.vit_assemble_fwd(PO, cls, pos, mt, pm, X0, B, S, d)
+    else:
+        ops._vit_assemble_gather_fwd(PO, cls, pos, mt, pm, keep, X0, P, d)
     return X0, B, S, P, pm
 
 
 def patch_embed_bwd(G: torch.Tensor, conv: nn.Module, cls: Optional[torch.Tensor], pos: torch.Tensor,
                     mask_token: Optional[torch.Tensor], pm: Optional[torch.Tensor], B: int, S: int, P: int,
-                    st: "ParamStore", ws: Workspace, save: Workspace, prefix: str) -> None:
-    """Parameter gradients of patch_embed_fwd from G = d X0 (fp32 [B*S, d])."""
+                    st: "ParamStore", ws: Workspace, save: Workspace, prefix: str,
+                    keep: Optional[torch.Tensor] = None) -> None:
+    """Parameter gradients of patch_embed_fwd from G = d X0 (fp32 [B*S, d]); keep as given to the forward."""
     d, ps = conv.weight.shape[0], conv.weight.shape[2]
     K = 3 * ps * ps
-    ops.batch_sum(G, st.grad(pos), B, S * d, S * d)
-    if cls is not None:
-        ops.batch_sum(G, st.grad(cls), B, S * d, d)
-    DP = ws.get(f"{prefix}.DP", (B * P, d), torch.bfloat16)
-    ops.vit_assemble_bwd(G, pm, DP, st.grad(mask_token) if pm is not None else None, B, S, d, cls is not None)
-    PATCH = save.get(f"{prefix}.PATCH", (B * P, -(-K // 8) * 8), torch.bfloat16)[:, :K]
+    rows = B * (P if keep is None else keep.shape[1])
+    DP = ws.get(f"{prefix}.DP", (rows, d), torch.bfloat16)
+    dmask = st.grad(mask_token) if pm is not None else None
+    if keep is None:
+        ops.batch_sum(G, st.grad(pos), B, S * d, S * d)
+        if cls is not None:
+            ops.batch_sum(G, st.grad(cls), B, S * d, d)
+        ops.vit_assemble_bwd(G, pm, DP, dmask, B, S, d, cls is not None)
+    else:
+        ops._vit_assemble_gather_bwd(G, pm, keep, DP, dmask, st.grad(cls) if cls is not None else None, st.grad(pos),
+                                    P, d, cls is not None)
+    PATCH = save.get(f"{prefix}.PATCH", (rows, -(-K // 8) * 8), torch.bfloat16)[:, :K]
     ops.gemm(DP, PATCH, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad2d(conv.weight),
-             splits=ops.wgrad_splits(d, K, B * P), accumulate=True)
+             splits=ops.wgrad_splits(d, K, rows), accumulate=True)
     if conv.bias is not None:
-        ops.colsum_bf16(DP, st.grad(conv.bias), B * P, d, d)
+        ops.colsum_bf16(DP, st.grad(conv.bias), rows, d, d)
 
 
 class TransformerStack:

@@ -137,12 +137,15 @@ class VisionRuntime:
 
     def forward(self, images: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None):
         from .modules.layers.transformer import TransformerOutput
+        from .modules.masking.random_masking import patch_keep_indices
 
         emb, st = self.mod.embeddings, self.stack
         d, conv = st.d, emb.conv_projection
+        drop = patch_keep_indices(emb, images.shape[0], images.device)   # training with patch_drop_rate
         X0, B, S, _, _ = patch_embed_fwd(images, conv, st.sh.get("conv.w", [conv.weight.view(d, -1)]),
                                          emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
-                                         emb.mask_token, image_patches_mask, st.ws, st.ws, "vit")   # hidden_states[0]
+                                         emb.mask_token, image_patches_mask, st.ws, st.ws, "vit",
+                                         keep=drop[0] if drop is not None else None)   # hidden_states[0]
         hidden = st.run(X0, B, S, keep_hidden=True)
         fln = self.mod.encoder.final_layer_norm
         XF, LAST, _ = st.finish(B, S, fln)

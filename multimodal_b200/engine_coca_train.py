@@ -31,6 +31,7 @@ from torch import nn
 from . import ops
 from ._lib import MMBError
 from .engine import ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run
+from .modules.masking.random_masking import patch_keep_indices
 
 
 def _qkv_first(layers) -> List[nn.Parameter]:
@@ -150,12 +151,14 @@ class VisionTrainRuntime:
         d, conv = s.d, emb.conv_projection
         st.refresh()
         save = Workspace(s.device)
+        drop = patch_keep_indices(emb, images.shape[0], images.device)   # the same draw as VisionRuntime.forward
+        keep = drop[0] if drop is not None else None
         X0, B, S, P, pm = patch_embed_fwd(images, conv, st.shadow2d(conv.weight),
                                           emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
-                                          emb.mask_token, image_patches_mask, s.ws, save, "cvit")
+                                          emb.mask_token, image_patches_mask, s.ws, save, "cvit", keep=keep)
         XM, Y = s.stack.forward(X0, B, S, True, save=save)
         XF, LAST = s.finish(XM, Y, B * S, self.mod.encoder.final_layer_norm, save)
-        save.B, save.S, save.P, save.pm = B, S, P, pm
+        save.B, save.S, save.P, save.pm, save.keep = B, S, P, pm, keep
         self.last_hidden = ([X0.view(B, S, d)] + [save.bufs[f"cvit.XA.{l}"].view(B, S, d) for l in range(1, s.L)]
                             + [XF.view(B, S, d)])
         return ((LAST if LAST is not None else XF),), save
@@ -169,7 +172,8 @@ class VisionTrainRuntime:
         G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
         G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
         patch_embed_bwd(G, emb.conv_projection, emb.cls_token if emb.include_cls_embed else None,
-                        emb.position_embeddings, emb.mask_token, save.pm, B, S, save.P, self.store, s.ws, save, "cvit")
+                        emb.position_embeddings, emb.mask_token, save.pm, B, S, save.P, self.store, s.ws, save, "cvit",
+                        keep=save.keep)
         return ()
 
 

@@ -213,9 +213,12 @@ def encoder_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask:
 
 
 def patch_embeddings_forward(mod: nn.Module, image: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None):
-    """PatchEmbeddings.forward (patch_embedding.py:104-154) without random patch dropping: conv projection as
-    im2col + wgmma GEMM, [cls |] patches (mask-token substitution) + position embeddings in one assembly kernel."""
+    """PatchEmbeddings.forward (patch_embedding.py:104-154): conv projection as im2col + wgmma GEMM, [cls |] patches
+    (mask-token substitution) + position embeddings in one assembly kernel.  In training with a patch_drop_rate, only
+    the kept patches are embedded (gathered im2col and assembly) and random_mask / ids_restore are returned as the
+    reference returns them (float rate; None for a (rate_h, rate_w) tuple)."""
     from .modules.layers.patch_embedding import PatchEmbeddingsOutput
+    from .modules.masking.random_masking import patch_keep_indices
 
     forward_only_guard(mod, "PatchEmbeddings")
     _cuda(image, "PatchEmbeddings")
@@ -225,10 +228,13 @@ def patch_embeddings_forward(mod: nn.Module, image: torch.Tensor, image_patches_
         raise ValueError(f"Input image shape {tuple(image.shape)} doesn't match the model's 3 x {mod.image_size}")
     rt = _rt(mod, image.device)
     d = conv.weight.shape[0]
+    drop = patch_keep_indices(mod, image.shape[0], image.device)
+    keep, random_mask, ids_restore = drop if drop is not None else (None, None, None)
     X, B, S, _, _ = patch_embed_fwd(image, conv, rt.sh.get("conv.w", [conv.weight.view(d, -1)]),
                                     mod.cls_token if mod.include_cls_embed else None, mod.position_embeddings,
-                                    mod.mask_token, image_patches_mask, rt.ws, rt.ws, "pe")
-    return PatchEmbeddingsOutput(embeddings=X.view(B, S, d).to(image.dtype))
+                                    mod.mask_token, image_patches_mask, rt.ws, rt.ws, "pe", keep=keep)
+    return PatchEmbeddingsOutput(embeddings=X.view(B, S, d).to(image.dtype), random_mask=random_mask,
+                                 ids_restore=ids_restore)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

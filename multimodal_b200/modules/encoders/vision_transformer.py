@@ -1,7 +1,9 @@
 """`VisionTransformer` — drop-in for torchmultimodal/modules/encoders/vision_transformer.py:19-203 (constructor,
 `vision_transformer` builder and the vit_* presets).  Forward = `engine_coca.VisionRuntime`.  ``attentions`` is None
 (flash-style attention); a custom ``pooler`` module, if given, is applied to ``last_hidden_state`` as in the reference.
-`GlobalAveragePooler` (MAE fine-tuning head) is outside SURVEY.md §8."""
+`GlobalAveragePooler` (MAE fine-tuning head) is outside SURVEY.md §8.  With `patch_drop_rate` the module drops patches in
+training only (either grad mode, the same random draws as the reference): `hidden_states` and `last_hidden_state` are
+then [B, off + L, d] for the L kept patches (off = 1 with a CLS token)."""
 import warnings
 from typing import Any, Callable, Optional, Tuple, Union
 

@@ -1,7 +1,11 @@
 """`PatchEmbeddings` — parameter container mirroring torchmultimodal/modules/layers/patch_embedding.py:25-157
 (conv projection with truncated-normal init, optional CLS token, position embeddings, optional mask token).  Executed
 by `engine_coca.VisionRuntime` as im2col + wgmma GEMM + one token-assembly kernel.  Random patch dropping
-(`patch_drop_rate`, training-time augmentation) is not on the accelerated path."""
+(`patch_drop_rate`: a float drops that share of the patches per sample, a (rate_h, rate_w) tuple drops whole patch rows
+and columns; FLIP, arXiv 2212.00794) applies in training only: the keep indices come from
+`modules/masking/random_masking.py` with the reference's random draws, and only the kept patches are embedded, by
+gathered im2col and token-assembly kernels, so the encoder runs on the shortened sequence.  `hidden_dropout_prob` must
+be 0."""
 import math
 from typing import Any, NamedTuple, Optional, Tuple, Union
 
@@ -29,8 +33,8 @@ class PatchEmbeddings(nn.Module):
             raise ValueError("Image size needs to be divisible by patch size")
         if num_channels != 3:
             raise NotImplementedError("the im2col kernel is specialised for 3-channel images")
-        if hidden_dropout_prob != 0.0 or patch_drop_rate is not None:
-            raise NotImplementedError("dropout / patch dropping are not on the accelerated path")
+        if hidden_dropout_prob != 0.0:
+            raise NotImplementedError("dropout is not on the accelerated path")
         self.num_patches_h = image_size[0] // patch_size
         self.num_patches_w = image_size[1] // patch_size
         num_patches = self.num_patches_h * self.num_patches_w
@@ -57,7 +61,8 @@ class PatchEmbeddings(nn.Module):
         nn.init.zeros_(self.conv_projection.bias)
 
     def forward(self, image: Tensor, image_patches_mask: Optional[Tensor] = None) -> PatchEmbeddingsOutput:
-        """Standalone forward (values only): im2col + wgmma GEMM + token assembly, as inside VisionTransformer."""
+        """Standalone forward (values only): im2col + wgmma GEMM + token assembly, as inside VisionTransformer; with
+        patch dropping in training, random_mask / ids_restore as the reference returns them."""
         from ...engine_layers import patch_embeddings_forward
 
         return patch_embeddings_forward(self, image, image_patches_mask)

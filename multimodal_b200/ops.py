@@ -167,6 +167,27 @@ def im2col(img: torch.Tensor, ps: int, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# Patch dropping (csrc/patch_drop.cu): called by engine.patch_embed_fwd / patch_embed_bwd only; their kernel contracts
+# are held in tests/test_gpu_patch_drop.py.
+def _check_keep(keep: torch.Tensor) -> torch.Tensor:
+    _chk(keep, torch.int32, "keep")
+    if keep.dim() != 2 or not keep.is_contiguous():
+        raise MMBError(f"keep: expected a contiguous int32 [B, L] tensor, got shape {tuple(keep.shape)}")
+    return keep
+
+
+def _im2col_gather(img: torch.Tensor, keep: torch.Tensor, ps: int, out: torch.Tensor) -> torch.Tensor:
+    """im2col of the kept patches: out row b*L+j = patch keep[b, j] of image b (keep int32 [B, L])."""
+    _chk(img, torch.float32, "img"); _chk(out, torch.bfloat16, "out"); _check_keep(keep)
+    B, C, H, W = img.shape
+    _rowmajor(out, "out")
+    if keep.shape[0] != B or out.shape[0] != keep.numel():
+        raise MMBError(f"im2col_gather: keep {tuple(keep.shape)} / out {tuple(out.shape)} do not match batch {B}")
+    _lib.check(_lib.lib().mmb_im2col_patches_gather(_p(img), _p(keep), _p(out), out.stride(0), B, H, W, ps,
+                                                    keep.shape[1], _stream()), "mmb_im2col_patches_gather")
+    return out
+
+
 def add_layernorm_fwd(x_in, y, x_out, ln_bf16, ln_f32, gamma, beta, mean, rstd, M, d, eps, row_idx=None,
                       rows_per_group=0):
     nbytes = M * d * (4 + (2 if y is not None else 0) + (4 if x_out is not None else 0) +
@@ -399,6 +420,15 @@ def vit_assemble_fwd(patch_out, cls, pos, mask_token, patch_mask, x, B, S, d):
                                                d, _stream()), "mmb_vit_assemble_fwd")
 
 
+def _vit_assemble_gather_fwd(patch_out, cls, pos, mask_token, patch_mask, keep, x, P, d):
+    """x [B*(off+L), d] from the kept patches' projections patch_out [B*L, d] (keep int32 [B, L], P patches)."""
+    _check_keep(keep)
+    B, L = keep.shape
+    _lib.check(_lib.lib().mmb_vit_assemble_gather_fwd(_p(patch_out), _p(cls), _p(pos), _p(mask_token), _p(patch_mask),
+                                                      _p(keep), _p(x), B, L, P, d, _stream()),
+               "mmb_vit_assemble_gather_fwd")
+
+
 def gather_rows_cast(x, out, B, rows_per_group, row, d):
     _lib.check(_lib.lib().mmb_gather_rows_cast(_p(x), _p(out), B, rows_per_group, row, d, _stream()), "mmb_gather_rows_cast")
 
@@ -553,6 +583,15 @@ def vit_assemble_bwd(g, patch_mask, dpatch, dmask_token, B, S, d, has_cls=True):
     _chk(g, torch.float32, "g"); _chk(dpatch, torch.bfloat16, "dpatch")
     _lib.check(_lib.lib().mmb_vit_assemble_bwd(_p(g), _p(patch_mask), _p(dpatch), _p(dmask_token), B, S, d, int(has_cls),
                                                _stream()), "mmb_vit_assemble_bwd")
+
+
+def _vit_assemble_gather_bwd(g, patch_mask, keep, dpatch, dmask_token, dcls, dpos, P, d, has_cls=True):
+    """Backward of vit_assemble_gather_fwd; dmask_token / dcls / dpos are added into (+=), each may be None."""
+    _chk(g, torch.float32, "g"); _chk(dpatch, torch.bfloat16, "dpatch"); _check_keep(keep)
+    B, L = keep.shape
+    _lib.check(_lib.lib().mmb_vit_assemble_gather_bwd(_p(g), _p(patch_mask), _p(keep), _p(dpatch), _p(dmask_token),
+                                                      _p(dcls), _p(dpos), B, L, P, d, int(has_cls), _stream()),
+               "mmb_vit_assemble_gather_bwd")
 
 
 def split_tokens_cast(g, a, b, B, Sa, Sb, d, has_cls=True):
