@@ -92,6 +92,11 @@ int mmb_gemm_ce_grad(const void* A, long long lda, const void* B, long long ldb,
 int mmb_cast_f32_to_bf16(const float* src, void* dst_bf16, long long n, void* stream);
 /* bf16 -> fp32 (result of the optional bf16-compressed gradient all-reduce back into the optimizer's fp32 input). */
 int mmb_cast_bf16_to_f32(const void* src, float* dst, long long n, void* stream);
+/* mmb_cast_f32_to_bf16 with a per-sample stochastic-depth factor: dst[i] = bf16(fl32(scale[i / per_scale] * src[i]));
+ * per_scale (elements per factor, e.g. S*d) > 0 and a multiple of 4.  The gradient entering the last layer's MLP branch
+ * of a stack without a final LayerNorm (StochasticDepth(p, "row"), modules/layers/transformer.py:63-70). */
+int mmb_cast_f32_to_bf16_scaled(const float* src, void* dst_bf16, long long n, const float* scale, long long per_scale,
+                                void* stream);
 
 /* Patch im2col + cast: img fp32 [B,3,H,W] -> bf16 [B*(H/ps)*(W/ps), 3*ps*ps] with row pitch ld_out elements (>= 3*ps*ps;
  * a multiple of 8 keeps the rows TMA-addressable, e.g. 592 for 14x14 patches), K order (c,kh,kw), patches row-major.
@@ -106,6 +111,13 @@ int mmb_im2col_patches(const float* img, void* out_bf16, long long ld_out, int B
 int mmb_add_layernorm_fwd(const float* x_in, const void* y_bf16, float* x_out, void* ln_bf16, float* ln_f32,
                           const float* gamma, const float* beta, float* mean, float* rstd, const int* row_idx,
                           int rows_per_group, int M, int d, float eps, void* stream);
+/* mmb_add_layernorm_fwd with stochastic depth on the added branch (torchvision stochastic_depth(y, p, "row") as
+ * TransformerEncoderLayer(drop_path_rate=...) applies it, modules/layers/transformer.py:63-70,95-129):
+ * x_out = x_in + fl32(scale[m / rows_per_scale] * y) for row m; scale fp32 [M / rows_per_scale] holds the drawn noise
+ * (0 or 1/(1-p)); the LayerNorm is unchanged.  y and scale required, rows_per_scale > 0, no row gather. */
+int mmb_add_layernorm_fwd_scaled(const float* x_in, const void* y_bf16, float* x_out, void* ln_bf16, float* ln_f32,
+                                 const float* gamma, const float* beta, float* mean, float* rstd, const float* scale,
+                                 int rows_per_scale, int M, int d, float eps, void* stream);
 
 /* CLIP ViT token assembly + ln_pre: x0 = LN(cat(cls, patch_out) + pos) (models/clip/image_encoder.py:94-106). */
 int mmb_vit_embed_ln_fwd(const void* patch_out_bf16, const float* cls, const float* pos, const float* gamma,
@@ -121,6 +133,13 @@ int mmb_vit_embed_ln_fwd(const void* patch_out_bf16, const float* cls, const flo
 int mmb_layernorm_bwd(const float* x, const void* dy_bf16, const float* dy_f32, const float* mean, const float* rstd,
                       const float* gamma, const float* g_in, float* g_out, void* g_bf16, float* dgamma, float* dbeta,
                       const int* row_idx, int rows_per_group, int M, int d, float* gsum, void* stream);
+/* mmb_layernorm_bwd for a residual stream whose next branch was scaled by stochastic depth: g_out is unchanged,
+ * g_bf16 = bf16(fl32(scale[m / rows_per_scale] * g_out)) (the gradient that enters the branch) and gsum sums those
+ * scaled bf16 values.  g_bf16 and scale required, rows_per_scale > 0, no row scatter. */
+int mmb_layernorm_bwd_scaled(const float* x, const void* dy_bf16, const float* dy_f32, const float* mean,
+                             const float* rstd, const float* gamma, const float* g_in, float* g_out, void* g_bf16,
+                             float* dgamma, float* dbeta, const float* scale, int rows_per_scale, int M, int d,
+                             float* gsum, void* stream);
 
 /* Backward of mmb_vit_embed_ln_fwd: dt = d/d(cat+pos) fp32 [B,S,d]; dpatch = bf16 copy of rows s>=1, compact. */
 int mmb_vit_embed_ln_bwd(const void* patch_out_bf16, const float* cls, const float* pos, const float* dy_f32,

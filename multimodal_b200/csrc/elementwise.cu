@@ -77,17 +77,28 @@ static inline int grid_for(long long n_items, int per_block) {
 
 // ---------------------------------------------------------------------------------------------
 // fp32 -> bf16 cast (weights, once per optimizer step)
+// SCALED: dst[i] = bf16(fl32(scale[i / per_scale] * src[i])), per_scale % 4 == 0 (the stochastic-depth factor of a
+// residual-stream gradient entering the last layer's MLP branch when no final LayerNorm produces it)
 // ---------------------------------------------------------------------------------------------
-__global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
+template <bool SCALED>
+__global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n,
+                                     const float* __restrict__ scale, long long per_scale) {
   const long long n4 = n >> 2;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(reinterpret_cast<const float4*>(src) + i);
+    float4 v = __ldg(reinterpret_cast<const float4*>(src) + i);
+    if (SCALED) {
+      const float sc = __ldg(scale + (i << 2) / per_scale);
+      v.x = __fmul_rn(sc, v.x); v.y = __fmul_rn(sc, v.y); v.z = __fmul_rn(sc, v.z); v.w = __fmul_rn(sc, v.w);
+    }
     uint2 o;
     o.x = pack_bf16x2(v.x, v.y);
     o.y = pack_bf16x2(v.z, v.w);
     reinterpret_cast<uint2*>(dst)[i] = o;
   }
-  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) dst[(n4 << 2) + threadIdx.x] = __float2bfloat16(src[(n4 << 2) + threadIdx.x]);
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const long long e = (n4 << 2) + threadIdx.x;
+    dst[e] = __float2bfloat16(SCALED ? __fmul_rn(__ldg(scale + e / per_scale), src[e]) : src[e]);
+  }
 }
 
 // bf16 -> fp32 (the bf16-compressed gradient all-reduce hands its result back to the fp32 optimizer input)
@@ -153,20 +164,25 @@ __device__ __forceinline__ void ln_stats(const LnRow& r, int nv, int d, float ep
 //   x_in : fp32 [M,d] or nullptr;  y : bf16 [M,d] or nullptr;  x_out : fp32 [M,d] or nullptr (may alias x_in)
 //   ln_bf16 : bf16 [M,d] or nullptr; ln_f32 : fp32 [M,d] or nullptr; mean/rstd : fp32 [M] or nullptr
 //   row_idx : optional gather: logical row m reads physical row (m*rows_per_group + row_idx[m]) (row_idx null -> +0)
+//   SCALED  : stochastic depth (torchvision stochastic_depth, mode "row"): x_out = x_in + fl32(s * y) with
+//             s = scale[m / rows_per_scale] (0 or 1/(1-p) per sample, drawn on the host side); no gather mode.
 // Replaces F.layer_norm + residual add (torch/nn/modules/transformer.py:946-951) and Fp32LayerNorm
 // (torchmultimodal/modules/layers/normalizations.py:17-25).
+template <bool SCALED>
 __global__ void add_ln_fwd_kernel(const float* __restrict__ x_in, const __nv_bfloat16* __restrict__ y,
                                   float* __restrict__ x_out, __nv_bfloat16* __restrict__ ln_bf16,
                                   float* __restrict__ ln_f32, const float* __restrict__ gamma,
                                   const float* __restrict__ beta, float* __restrict__ mean_out,
                                   float* __restrict__ rstd_out, const int* __restrict__ row_idx, int rows_per_group,
-                                  int M, int d, float eps) {
+                                  int M, int d, float eps, const float* __restrict__ scale, int rows_per_scale) {
   const int nv = d >> 7;
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   for (int m = blockIdx.x * wpb + (threadIdx.x >> 5); m < M; m += gridDim.x * wpb) {
     long long src = m;
     if (rows_per_group > 0) src = (long long)m * rows_per_group + (row_idx ? row_idx[m] : 0);
+    float s = 1.f;
+    if (SCALED) s = __ldg(scale + m / rows_per_scale);
     LnRow r;
 #pragma unroll
     for (int i = 0; i < LN_MAX_NV; ++i)
@@ -176,7 +192,12 @@ __global__ void add_ln_fwd_kernel(const float* __restrict__ x_in, const __nv_bfl
         if (x_in) a = *reinterpret_cast<const float4*>(x_in + src * d + c);
         if (y) {
           const uint2 u = *reinterpret_cast<const uint2*>(y + src * d + c);
-          a.x += bf16_lo(u.x); a.y += bf16_hi(u.x); a.z += bf16_lo(u.y); a.w += bf16_hi(u.y);
+          if (SCALED) {  // the product is rounded on its own (no FMA), as input * noise is in the reference
+            a.x += __fmul_rn(s, bf16_lo(u.x)); a.y += __fmul_rn(s, bf16_hi(u.x));
+            a.z += __fmul_rn(s, bf16_lo(u.y)); a.w += __fmul_rn(s, bf16_hi(u.y));
+          } else {
+            a.x += bf16_lo(u.x); a.y += bf16_hi(u.x); a.z += bf16_lo(u.y); a.w += bf16_hi(u.y);
+          }
         }
         r.v[i] = a;
         if (x_out) *reinterpret_cast<float4*>(x_out + (long long)m * d + c) = a;  // compact in gather mode
@@ -475,6 +496,8 @@ __global__ void concat_tokens_kernel(const float* __restrict__ cls, const float*
 //   xhat = (x - mean) * rstd;  dyg = dy * gamma
 //   dx   = rstd * (dyg - mean_d(dyg) - xhat * mean_d(dyg * xhat))
 //   g_out = (g_in ? g_in : 0) + dx         (fp32 [M,d], may alias g_in)     and/or  g_bf16 = bf16(g_out)
+//   SCALED (stochastic depth of the branch that reads g_bf16): g_bf16 = bf16(fl32(s * g_out)),
+//   s = scale[m / rows_per_scale]; gsum sums those scaled bf16 values; g_out is unscaled (the residual path)
 //   dgamma += sum_rows dy * xhat ; dbeta += sum_rows dy      (fp32 atomics, one per column per block)
 // Input modes for x:  MODE_X      : x fp32 [M,d]
 //                     MODE_VIT    : x is re-assembled from patch_out/cls/pos (token assembly, see above)
@@ -491,13 +514,14 @@ struct LnBwdArgs {
   float* part;  // [3][gridDim.x][d] per-CTA column partials of dgamma / dbeta / gsum (reduced in a fixed order)
   const int* row_idx; int rows_per_group;
   int M, d;
+  const float* scale; int rows_per_scale;  // SCALED only: per-sample factor of g_bf16
 };
 
 // One CTA of NV warps per row (one float4 of the row per thread): ~20 live registers per thread, so 10-16 CTAs are
 // resident per SM and 60+ warps hide the HBM latency (a warp-per-row layout would keep the whole row plus three
 // per-lane column accumulators in ~170 registers and leave only 12 warps per SM to hide it).
 // The two row reductions cross the NV warps through a double-buffered smem slot: one __syncthreads per row.
-template <bool VIT, int NV>
+template <bool VIT, int NV, bool SCALED>
 __global__ void __launch_bounds__(NV * 32, (1536 / (NV * 32) > 32 ? 32 : 1536 / (NV * 32))) ln_bwd_kernel(const LnBwdArgs a) {
   constexpr int d = NV * 128;
   __shared__ float part[2][NV][2];
@@ -528,6 +552,8 @@ __global__ void __launch_bounds__(NV * 32, (1536 / (NV * 32) > 32 ? 32 : 1536 / 
     else           dy = *reinterpret_cast<const float4*>(a.dy_f32 + (long long)m * d + c);
     if (a.g_in) gi = *reinterpret_cast<const float4*>(a.g_in + phys * d + c);
     const float mean = a.mean[m], rstd = a.rstd[m];
+    float sc = 1.f;
+    if (SCALED) sc = __ldg(a.scale + m / a.rows_per_scale);
     if (VIT) {
       if (s == 0) { x.x += cl.x; x.y += cl.y; x.z += cl.z; x.w += cl.w; }
       else { x.x += bf16_lo(pu.x); x.y += bf16_hi(pu.x); x.z += bf16_lo(pu.y); x.w += bf16_hi(pu.y); }
@@ -558,8 +584,13 @@ __global__ void __launch_bounds__(NV * 32, (1536 / (NV * 32) > 32 ? 32 : 1536 / 
     if (a.g_out) *reinterpret_cast<float4*>(a.g_out + phys * d + c) = o;
     if (a.g_bf16) {
       uint2 u;
-      u.x = pack_bf16x2(o.x, o.y);
-      u.y = pack_bf16x2(o.z, o.w);
+      if (SCALED) {
+        u.x = pack_bf16x2(__fmul_rn(sc, o.x), __fmul_rn(sc, o.y));
+        u.y = pack_bf16x2(__fmul_rn(sc, o.z), __fmul_rn(sc, o.w));
+      } else {
+        u.x = pack_bf16x2(o.x, o.y);
+        u.y = pack_bf16x2(o.z, o.w);
+      }
       if (want_gsum) {  // sums the ROUNDED values: identical to a column sum over the stored bf16 tensor
         accs.x += bf16_lo(u.x); accs.y += bf16_hi(u.x); accs.z += bf16_lo(u.y); accs.w += bf16_hi(u.y);
       }
@@ -579,7 +610,7 @@ __global__ void __launch_bounds__(NV * 32, (1536 / (NV * 32) > 32 ? 32 : 1536 / 
   if (want_gsum) *reinterpret_cast<float4*>(pp + 2 * plane) = accs;
 }
 
-template <bool VIT>
+template <bool VIT, bool SCALED = false>
 static int launch_ln_bwd(LnBwdArgs a, cudaStream_t st) {
   const int nv = a.d >> 7;
   const int threads = nv * 32;
@@ -594,7 +625,7 @@ static int launch_ln_bwd(LnBwdArgs a, cudaStream_t st) {
     if (!a.part) return (int)cudaErrorMemoryAllocation;
   }
   switch (nv) {
-#define LNB(NVV) case NVV: ln_bwd_kernel<VIT, NVV><<<grid, threads, 0, st>>>(a); break;
+#define LNB(NVV) case NVV: ln_bwd_kernel<VIT, NVV, SCALED><<<grid, threads, 0, st>>>(a); break;
     LNB(1) LNB(2) LNB(3) LNB(4) LNB(5) LNB(6) LNB(7) LNB(8)
 #undef LNB
     default: return MMB_ERR_UNSUPPORTED;
@@ -894,7 +925,18 @@ using namespace mmb;
 extern "C" int mmb_cast_f32_to_bf16(const float* src, void* dst, long long n, void* stream) {
   if (n <= 0) return MMB_OK;
   if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(dst) & 7)) return MMB_ERR_ARG;
-  cast_f32_bf16_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(src, (__nv_bfloat16*)dst, n);
+  cast_f32_bf16_kernel<false><<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(src, (__nv_bfloat16*)dst, n,
+                                                                                 nullptr, 0);
+  return LAUNCH_RC();
+}
+
+extern "C" int mmb_cast_f32_to_bf16_scaled(const float* src, void* dst, long long n, const float* scale,
+                                           long long per_scale, void* stream) {
+  if (n <= 0) return MMB_OK;
+  if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(dst) & 7)) return MMB_ERR_ARG;
+  if (!scale || per_scale <= 0 || (per_scale & 3)) return MMB_ERR_ARG;
+  cast_f32_bf16_kernel<true><<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(src, (__nv_bfloat16*)dst, n, scale,
+                                                                                per_scale);
   return LAUNCH_RC();
 }
 
@@ -920,9 +962,22 @@ extern "C" int mmb_add_layernorm_fwd(const float* x_in, const void* y_bf16, floa
                                      const int* row_idx, int rows_per_group, int M, int d, float eps, void* stream) {
   if (!ln_dim_ok(d)) return MMB_ERR_UNSUPPORTED;
   if (M <= 0) return MMB_OK;
-  add_ln_fwd_kernel<<<grid_for(M, 8), 256, 0, ST(stream)>>>(x_in, (const __nv_bfloat16*)y_bf16, x_out,
-                                                             (__nv_bfloat16*)ln_bf16, ln_f32, gamma, beta, mean, rstd,
-                                                             row_idx, rows_per_group, M, d, eps);
+  add_ln_fwd_kernel<false><<<grid_for(M, 8), 256, 0, ST(stream)>>>(x_in, (const __nv_bfloat16*)y_bf16, x_out,
+                                                                    (__nv_bfloat16*)ln_bf16, ln_f32, gamma, beta, mean,
+                                                                    rstd, row_idx, rows_per_group, M, d, eps, nullptr, 0);
+  return LAUNCH_RC();
+}
+
+extern "C" int mmb_add_layernorm_fwd_scaled(const float* x_in, const void* y_bf16, float* x_out, void* ln_bf16,
+                                            float* ln_f32, const float* gamma, const float* beta, float* mean,
+                                            float* rstd, const float* scale, int rows_per_scale, int M, int d,
+                                            float eps, void* stream) {
+  if (!ln_dim_ok(d)) return MMB_ERR_UNSUPPORTED;
+  if (!y_bf16 || !scale || rows_per_scale <= 0) return MMB_ERR_ARG;
+  if (M <= 0) return MMB_OK;
+  add_ln_fwd_kernel<true><<<grid_for(M, 8), 256, 0, ST(stream)>>>(x_in, (const __nv_bfloat16*)y_bf16, x_out,
+                                                                   (__nv_bfloat16*)ln_bf16, ln_f32, gamma, beta, mean,
+                                                                   rstd, nullptr, 0, M, d, eps, scale, rows_per_scale);
   return LAUNCH_RC();
 }
 
@@ -948,6 +1003,21 @@ extern "C" int mmb_layernorm_bwd(const float* x, const void* dy_bf16, const floa
   a.g_in = g_in; a.g_out = g_out; a.g_bf16 = (__nv_bfloat16*)g_bf16; a.dgamma = dgamma; a.dbeta = dbeta;
   a.row_idx = row_idx; a.rows_per_group = rows_per_group; a.M = M; a.d = d;
   return launch_ln_bwd<false>(a, ST(stream));
+}
+
+extern "C" int mmb_layernorm_bwd_scaled(const float* x, const void* dy_bf16, const float* dy_f32, const float* mean,
+                                        const float* rstd, const float* gamma, const float* g_in, float* g_out,
+                                        void* g_bf16, float* dgamma, float* dbeta, const float* scale,
+                                        int rows_per_scale, int M, int d, float* gsum, void* stream) {
+  if (!ln_dim_ok(d)) return MMB_ERR_UNSUPPORTED;
+  if (!g_bf16 || !scale || rows_per_scale <= 0) return MMB_ERR_ARG;
+  if (M <= 0) return MMB_OK;
+  LnBwdArgs a{};
+  a.gsum = gsum;
+  a.x = x; a.dy_bf16 = (const __nv_bfloat16*)dy_bf16; a.dy_f32 = dy_f32; a.mean = mean; a.rstd = rstd; a.gamma = gamma;
+  a.g_in = g_in; a.g_out = g_out; a.g_bf16 = (__nv_bfloat16*)g_bf16; a.dgamma = dgamma; a.dbeta = dbeta;
+  a.M = M; a.d = d; a.scale = scale; a.rows_per_scale = rows_per_scale;
+  return launch_ln_bwd<false, true>(a, ST(stream));
 }
 
 extern "C" int mmb_vit_embed_ln_bwd(const void* patch_out, const float* cls, const float* pos, const float* dy_f32,

@@ -244,6 +244,13 @@ def act_code(act: nn.Module) -> int:
     raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU / SiLU)")
 
 
+def scaled(scale: Optional[torch.Tensor], rows_per_scale: int) -> dict:
+    """Keyword arguments that pass a stochastic-depth factor (fp32 [M / rows_per_scale] or None) to
+    ops.add_layernorm_fwd / layernorm_bwd / cast_bf16: none without a factor, so an unscaled call is the call a stack
+    without drop path makes."""
+    return {} if scale is None else {"branch_scale": scale, "rows_per_scale": rows_per_scale}
+
+
 def wants_grad(*mods: Optional[nn.Module]) -> bool:
     """True when the caller expects an autograd graph: grad mode on and some parameter of `mods` trainable."""
     if not torch.is_grad_enabled():
@@ -337,9 +344,13 @@ class TransformerStack:
 
     def forward(self, X0: torch.Tensor, B: int, S: int, training: bool, kmask: Optional[torch.Tensor] = None,
                 save: Optional["Workspace"] = None, mask3: Optional[torch.Tensor] = None,
-                enc: Optional[torch.Tensor] = None, S_enc: int = 0):
+                enc: Optional[torch.Tensor] = None, S_enc: int = 0, scales=None):
         """X0: fp32 [B*S, d] residual stream entering layer 0.  Returns (XM_last fp32, Y bf16): the final residual
-        stream is XM_last + Y (the add is fused into whichever LayerNorm consumes it).
+        stream is XM_last + Y (the add is fused into whichever LayerNorm consumes it; with stochastic depth the caller
+        scales that add by `top_scale`).
+        scales: stochastic depth (modules/layers/stochastic_depth.drop_path_scales): per layer the (attention,
+        feed-forward) per-sample factors fp32 [B] or None; each scales its branch inside the residual add that
+        follows it, and the backward scales the gradient entering the branch.  Not with cross-attention layers.
         kmask: optional uint8 [B*S] key-padding mask (1 = attend).  mask3: optional uint8 [B, S, S] mask (general
         attention kernels).  enc / S_enc: bf16 [B*S_enc, d_kv] cross-attention source for layers that carry a
         `cross_attn` block (TransformerDecoderLayer: modules/layers/transformer.py:354-377).  save: the Workspace that receives the activations a
@@ -349,6 +360,9 @@ class TransformerStack:
         self._save.kmask = kmask if training else None
         self._save.mask3 = mask3 if training else None
         self._save.enc, self._save.S_enc = (enc, S_enc) if training else (None, 0)
+        if scales is not None and enc is not None:
+            raise MMBError("stochastic depth is applied to encoder layers only (no cross-attention)")
+        self._save.scales, self._save.rows_per_scale = scales, S
         st, d, ff, H = self.store, self.d, self.ff, self.H
         M = B * S
         bf, f32 = torch.bfloat16, torch.float32
@@ -356,6 +370,8 @@ class TransformerStack:
         XA_prev, XM_prev = X0, None
         for l, layer in enumerate(self.layers):
             at = layer.self_attn
+            s_attn = scales[l][0] if scales is not None else None
+            s_prev_ff = scales[l - 1][1] if scales is not None and l > 0 else None
             LN1 = self._buf("LN1", l, (M, d), bf, training)
             QKV = self._buf("QKV", l, (M, 3 * d), bf, training)
             O = self._buf("O", l, (M, d), bf, training)
@@ -373,7 +389,7 @@ class TransformerStack:
             else:
                 XA = self._buf("XA", l, (M, d), f32, training)
                 ops.add_layernorm_fwd(XM_prev, Y, XA, LN1, None, layer.norm1.weight, layer.norm1.bias, m1, r1, M, d,
-                                      layer.norm1.eps)
+                                      layer.norm1.eps, **scaled(s_prev_ff, S))
             ops.gemm(LN1, st.shadow(at.in_proj_weight), bias=at.in_proj_bias, out=QKV)
             ops.self_attention(QKV, O, LSE, B, S, H, 64, self.causal, self.scale, kmask=kmask, mask=mask3)
             ops.gemm(O, st.shadow(at.out_proj.weight), bias=at.out_proj.bias, out=Y)
@@ -399,7 +415,7 @@ class TransformerStack:
                 XM = XC
             else:
                 ops.add_layernorm_fwd(XA, Y, XM, LN2, None, layer.norm2.weight, layer.norm2.bias, m2, r2, M, d,
-                                      layer.norm2.eps)
+                                      layer.norm2.eps, **scaled(s_attn, S))
             ops.gemm(LN2, st.shadow(layer.linear1.weight), bias=layer.linear1.bias, epilogue=ops.EPI_BF16_ACT, out=PRE,
                      out2=HACT, act=self.act)
             ops.gemm(HACT, st.shadow(layer.linear2.weight), bias=layer.linear2.bias, out=Y)
@@ -409,13 +425,21 @@ class TransformerStack:
         self._save.X0 = self._X0
         return XM_prev, Y
 
+    @staticmethod
+    def top_scale(save: "Workspace"):
+        """(factor or None, rows_per_scale) of the last layer's MLP branch: scales the add of XM_last + Y, and the
+        gradient entering that branch at the start of the backward."""
+        scales = getattr(save, "scales", None)
+        return (scales[-1][1] if scales is not None else None), getattr(save, "rows_per_scale", 0)
+
     def top_bias_grad(self) -> torch.Tensor:
         """Gradient slot of the last layer's linear2.bias: the producer of the incoming Gb sums its columns into it."""
         return self.store.grad(self.layers[-1].linear2.bias)
 
     def backward(self, G: torch.Tensor, Gb: torch.Tensor, B: int, S: int, on_layer_done=None,
                  top_bias_done: bool = False, save: Optional["Workspace"] = None) -> torch.Tensor:
-        """G (fp32) / Gb (bf16 copy): gradient w.r.t. the final residual stream [B*S, d].  Returns G w.r.t. X0
+        """G (fp32) / Gb (bf16 copy, times the last MLP branch's stochastic-depth factor when the forward had
+        scales): gradient w.r.t. the final residual stream [B*S, d].  Returns G w.r.t. X0
         (in place).  Parameter gradients are ACCUMULATED into the ParamStore's flat fp32 buffer.
         The bias gradients of linear2 / out_proj are column sums of Gb; they are produced by the LayerNorm-backward
         kernel that writes Gb (`gsum`), not by a separate pass (top_bias_done: the caller's kernel did the top one)."""
@@ -425,6 +449,7 @@ class TransformerStack:
             save = self.ws
         X0, kmask = save.X0, getattr(save, "kmask", None)
         mask3, enc, Se = getattr(save, "mask3", None), getattr(save, "enc", None), getattr(save, "S_enc", 0)
+        scales = getattr(save, "scales", None)
         save.dENC = None
         if X0 is None:
             raise MMBError("backward called without a saved training forward")
@@ -463,7 +488,8 @@ class TransformerStack:
             ops.gemm(dPRE, st.shadow(layer.linear1.weight), b_mn=True, out=T1)
             ops.layernorm_bwd(XMID, T1, None, m2, r2, layer.norm2.weight, G, G, Gb, st.grad(layer.norm2.weight),
                               st.grad(layer.norm2.bias), M, d,
-                              gsum=st.grad(ca.out_proj.bias if ca is not None else at.out_proj.bias))
+                              gsum=st.grad(ca.out_proj.bias if ca is not None else at.out_proj.bias),
+                              **scaled(scales[l][0] if scales is not None else None, S))
             if ca is not None:
                 # ---- cross-attention branch:  x2 = x1 + Wo_c Attn(Wq LN_c(x1), Wkv enc) ----
                 lnc = layer.norm_cross
@@ -505,7 +531,8 @@ class TransformerStack:
             ops.gemm(T3, st.shadow(at.in_proj_weight), b_mn=True, out=T1)
             ops.layernorm_bwd(XA, T1, None, m1, r1, layer.norm1.weight, G, G, Gb, st.grad(layer.norm1.weight),
                               st.grad(layer.norm1.bias), M, d,
-                              gsum=st.grad(self.layers[l - 1].linear2.bias) if l > 0 else None)
+                              gsum=st.grad(self.layers[l - 1].linear2.bias) if l > 0 else None,
+                              **scaled(scales[l - 1][1] if scales is not None and l > 0 else None, S))
             if on_layer_done is not None:
                 on_layer_done(l)  # all parameter gradients of layer l are final (data-parallel all-reduce hook)
         return G

@@ -24,7 +24,7 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import Workspace, _Shadows, act_code, patch_embed_fwd
+from .engine import Workspace, _Shadows, act_code, patch_embed_fwd, scaled
 
 
 class LayerStack:
@@ -56,9 +56,11 @@ class LayerStack:
                 self.sh.cat_f32(f"{l}.bqkv", [at.q_proj.bias, at.k_proj.bias, at.v_proj.bias]))
 
     def run(self, X0: torch.Tensor, B: int, S: int, *, causal: bool = False, mask: Optional[torch.Tensor] = None,
-            enc: Optional[torch.Tensor] = None, S_enc: int = 0, keep_hidden: bool = False):
+            enc: Optional[torch.Tensor] = None, S_enc: int = 0, keep_hidden: bool = False, scales=None):
         """X0 fp32 [B*S, d].  mask: uint8 [B, S, S] (1 = attend).  enc: bf16 [B*S_enc, d_kv] cross-attention source.
-        Returns (XF fp32 [B*S, d] residual stream after the last layer, hidden_states list or None)."""
+        scales: stochastic depth, per layer the (attention, feed-forward) factors fp32 [B] or None
+        (stochastic_depth.drop_path_scales); each scales its branch in the residual add that follows it.
+        Returns the hidden_states list or None; `finish` adds the last MLP branch."""
         d, ff, H, hd, ws, sh, pfx = self.d, self.ff, self.H, self.hd, self.ws, self.sh, self.prefix
         M = B * S
         bf, f32 = torch.bfloat16, torch.float32
@@ -81,7 +83,8 @@ class LayerStack:
                 # returned as hidden_states[l] when requested: allocated per call (never aliases a later forward)
                 XA = (torch.empty((M, d), device=X0.device, dtype=f32) if keep_hidden
                       else ws.get(f"{pfx}.XA.{l % 2}", (M, d), f32))
-                ops.add_layernorm_fwd(XR, Y, XA, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
+                ops.add_layernorm_fwd(XR, Y, XA, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps,
+                                      **scaled(scales[l - 1][1] if scales is not None else None, S))
                 if keep_hidden:
                     hidden.append(XA.view(B, S, d))
             else:
@@ -91,6 +94,8 @@ class LayerStack:
             ops.gemm(O, sh.get(f"{l}.wo", [at.output_proj.weight]), bias=at.output_proj.bias, out=Y)
             XR = XM
             if getattr(layer, "use_cross_attention", False) and enc is not None:
+                if scales is not None:
+                    raise MMBError("stochastic depth is applied to encoder layers only (no cross-attention)")
                 ca, lnc = layer.cross_attention, layer.cross_attention_layernorm
                 ops.add_layernorm_fwd(XA, Y, XM, LN, None, lnc.weight, lnc.bias, None, None, M, d, lnc.eps)
                 Qc = ws.get(f"{pfx}.Qc", (M, d), bf)
@@ -104,17 +109,18 @@ class LayerStack:
                 ops.add_layernorm_fwd(XM, Y, XC, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
                 XR = XC
             else:
-                ops.add_layernorm_fwd(XA, Y, XM, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+                ops.add_layernorm_fwd(XA, Y, XM, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
+                                      **scaled(scales[l][0] if scales is not None else None, S))
             ops.gemm(LN, sh.get(f"{l}.w1", [mlp[0].weight]), bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE,
                      out2=HACT, act=self.act)
             ops.gemm(HACT, sh.get(f"{l}.w2", [mlp[-1].weight]), bias=mlp[-1].bias, out=Y)
-        self._last = (XR, Y)
+        self._last = (XR, Y, scales[-1][1] if scales is not None else None)
         return hidden
 
     def finish(self, B: int, S: int, final_ln: Optional[nn.Module], want_bf16: bool = False):
         """Adds the last MLP output to the stream (XF) and applies the optional final LayerNorm.
         Returns (XF fp32 [M,d], LAST fp32 or None, LAST bf16 or None)."""
-        XR, Y = self._last
+        XR, Y, scale = self._last
         M, d, ws, pfx = B * S, self.d, self.ws, self.prefix
         # XF / LAST are handed to the caller (last_hidden_state / hidden_states[-1] / tokens): fresh per call, as the
         # reference's outputs are; bf16 copies consumed inside the same forward stay in the workspace
@@ -122,7 +128,8 @@ class LayerStack:
         ln = final_ln if final_ln is not None else self.layers[0].attention_layernorm  # affine unused when no output
         LAST = torch.empty((M, d), device=XR.device, dtype=torch.float32) if final_ln is not None else None
         LASTb = ws.get(f"{pfx}.LASTb", (M, d), torch.bfloat16) if (final_ln is not None and want_bf16) else None
-        ops.add_layernorm_fwd(XR, Y, XF, LASTb, LAST, ln.weight, ln.bias, None, None, M, d, ln.eps)
+        ops.add_layernorm_fwd(XR, Y, XF, LASTb, LAST, ln.weight, ln.bias, None, None, M, d, ln.eps,
+                              **scaled(scale, S))
         return XF, LAST, LASTb
 
 
@@ -137,16 +144,18 @@ class VisionRuntime:
 
     def forward(self, images: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None):
         from .modules.layers.transformer import TransformerOutput
+        from .modules.layers.stochastic_depth import drop_path_scales
         from .modules.masking.random_masking import patch_keep_indices
 
         emb, st = self.mod.embeddings, self.stack
         d, conv = st.d, emb.conv_projection
         drop = patch_keep_indices(emb, images.shape[0], images.device)   # training with patch_drop_rate
+        scales = drop_path_scales(st.layers, images.shape[0], images.device)   # training with drop_path_rate
         X0, B, S, _, _ = patch_embed_fwd(images, conv, st.sh.get("conv.w", [conv.weight.view(d, -1)]),
                                          emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
                                          emb.mask_token, image_patches_mask, st.ws, st.ws, "vit",
                                          keep=drop[0] if drop is not None else None)   # hidden_states[0]
-        hidden = st.run(X0, B, S, keep_hidden=True)
+        hidden = st.run(X0, B, S, keep_hidden=True, scales=scales)
         fln = self.mod.encoder.final_layer_norm
         XF, LAST, _ = st.finish(B, S, fln)
         hidden.append(XF.view(B, S, d))

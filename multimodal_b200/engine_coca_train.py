@@ -30,7 +30,9 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run
+from .engine import (ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run,
+                     scaled)
+from .modules.layers.stochastic_depth import drop_path_scales
 from .modules.masking.random_masking import patch_keep_indices
 
 
@@ -99,36 +101,42 @@ class _Stack:
                                       ff=l0.feedforward.model[0].weight.shape[0], causal=causal,
                                       act=act_code(l0.feedforward.model[1]), prefix=prefix)
         self.prefix, self.L = prefix, len(layers)
+        self.layers = layers     # the modules themselves: their StochasticDepth (drop_path_rate), if any
 
     def finish(self, XM, Y, M: int, ln: Optional[nn.Module], save: Workspace):
-        """XF = XM + Y (the residual stream after the last layer); LAST = ln(XF) when a final LayerNorm exists."""
+        """XF = XM + Y (the residual stream after the last layer; Y times the last MLP branch's stochastic-depth
+        factor when the forward drew one); LAST = ln(XF) when a final LayerNorm exists."""
         d, pfx = self.d, self.prefix
         f32 = torch.float32
         XF = torch.empty((M, d), device=self.device, dtype=f32)
         LAST = torch.empty((M, d), device=self.device, dtype=f32) if ln is not None else None
         aff = ln if ln is not None else self.stack.layers[0].norm1   # affine terms unused when nothing is normalised
+        scale, rows = self.stack.top_scale(save)
         ops.add_layernorm_fwd(XM, Y, XF, None, LAST, aff.weight, aff.bias,
                               save.get(f"{pfx}.mF", (M,), f32) if ln is not None else None,
-                              save.get(f"{pfx}.rF", (M,), f32) if ln is not None else None, M, d, aff.eps)
+                              save.get(f"{pfx}.rF", (M,), f32) if ln is not None else None, M, d, aff.eps,
+                              **scaled(scale, rows))
         save.XF = XF
         return XF, LAST
 
     def start_backward(self, save: Workspace, M: int, ln: Optional[nn.Module], dLAST, dXF):
-        """(G fp32, Gb bf16, top_bias_done): gradient w.r.t. XF entering the stack's backward."""
+        """(G fp32, Gb bf16, top_bias_done): gradient w.r.t. XF entering the stack's backward; Gb is the gradient
+        entering the last MLP branch (scaled by its stochastic-depth factor, if any)."""
         d, pfx, st = self.d, self.prefix, self.store
         f32, bf = torch.float32, torch.bfloat16
         G = self.ws.get(f"{pfx}.G", (M, d), f32)
         Gb = self.ws.get(f"{pfx}.Gb", (M, d), bf)
+        scale, rows = self.stack.top_scale(save)
         if ln is not None and dLAST is not None:
             ops.layernorm_bwd(save.XF, None, dLAST, save.get(f"{pfx}.mF", (M,), f32), save.get(f"{pfx}.rF", (M,), f32),
                               ln.weight, dXF, G, Gb, st.grad(ln.weight), st.grad(ln.bias), M, d,
-                              gsum=self.stack.top_bias_grad())
+                              gsum=self.stack.top_bias_grad(), **scaled(scale, rows))
             return G, Gb, True
         if dXF is None:
             ops.zero_(G)
         else:
             G.copy_(dXF.view(M, d))      # the stack's backward works in place on G
-        ops.cast_bf16(G, Gb)
+        ops.cast_bf16(G, Gb, **scaled(scale, rows))
         return G, Gb, False
 
 
@@ -151,12 +159,13 @@ class VisionTrainRuntime:
         d, conv = s.d, emb.conv_projection
         st.refresh()
         save = Workspace(s.device)
-        drop = patch_keep_indices(emb, images.shape[0], images.device)   # the same draw as VisionRuntime.forward
+        drop = patch_keep_indices(emb, images.shape[0], images.device)   # the same draws as VisionRuntime.forward
         keep = drop[0] if drop is not None else None
+        scales = drop_path_scales(s.layers, images.shape[0], images.device)
         X0, B, S, P, pm = patch_embed_fwd(images, conv, st.shadow2d(conv.weight),
                                           emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
                                           emb.mask_token, image_patches_mask, s.ws, save, "cvit", keep=keep)
-        XM, Y = s.stack.forward(X0, B, S, True, save=save)
+        XM, Y = s.stack.forward(X0, B, S, True, save=save, scales=scales)
         XF, LAST = s.finish(XM, Y, B * S, self.mod.encoder.final_layer_norm, save)
         save.B, save.S, save.P, save.pm, save.keep = B, S, P, pm, keep
         self.last_hidden = ([X0.view(B, S, d)] + [save.bufs[f"cvit.XA.{l}"].view(B, S, d) for l in range(1, s.L)]
@@ -523,7 +532,8 @@ class LayersTrainRuntime:
         save = Workspace(s.device)
         X0 = torch.empty((B * S, d), device=s.device, dtype=torch.float32)
         X0.view(B, S, d).copy_(x)
-        XM, Y = s.stack.forward(X0, B, S, True, save=save, mask3=mask_u8)
+        XM, Y = s.stack.forward(X0, B, S, True, save=save, mask3=mask_u8,
+                                scales=drop_path_scales(s.layers, B, s.device))
         XF, LAST = s.finish(XM, Y, B * S, self.final_ln, save)
         save.B, save.S = B, S
         self.last_hidden = ([X0.view(B, S, d)] + [save.bufs[f"lyr.XA.{l}"].view(B, S, d) for l in range(1, s.L)]

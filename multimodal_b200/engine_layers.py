@@ -30,7 +30,7 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import Workspace, _Shadows, act_code, patch_embed_fwd
+from .engine import Workspace, _Shadows, act_code, patch_embed_fwd, scaled
 
 
 def forward_only_guard(mod: nn.Module, what: str) -> None:
@@ -132,7 +132,10 @@ def mlp_forward(mod: nn.Module, x: torch.Tensor) -> torch.Tensor:
 
 def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
                           attention_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """TransformerEncoderLayer.forward (transformer.py:95-154), pre-norm (:95-111) and post-norm (:113-128)."""
+    """TransformerEncoderLayer.forward (transformer.py:95-154), pre-norm (:95-111) and post-norm (:113-128).  With a
+    drop_path_rate in training, each branch is scaled per sample inside the residual add that follows it."""
+    from .modules.layers.stochastic_depth import drop_path_scales
+
     if _wants_graph(mod, hidden_states):
         if not mod.norm_first:
             raise MMBError("standalone post-norm TransformerEncoderLayer has no backward schedule; call it under "
@@ -162,27 +165,33 @@ def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
     wqkv, wo = sh.get("wqkv", [at.input_proj.weight]), sh.get("wo", [at.output_proj.weight])
     w1, w2 = sh.get("w1", [mlp[0].weight]), sh.get("w2", [mlp[-1].weight])
     out = torch.empty((M, d), device=X.device, dtype=f32)
+    scales = drop_path_scales([mod], B, X.device)
+    s_attn, s_ff = scales[0] if scales is not None else (None, None)
     if mod.norm_first:
         ops.add_layernorm_fwd(X, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
         ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
         ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
         ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
         XM = ws.get("l.XM", (M, d), f32)                       # x + attention(LN(x)); LN2 of it for the MLP
-        ops.add_layernorm_fwd(X, Y, XM, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+        ops.add_layernorm_fwd(X, Y, XM, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
+                              **scaled(s_attn, S))
         ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
         ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
         # out = XM + mlp: the add kernel with an identity-free LayerNorm is not needed — reuse add+LN writing only x_out
-        ops.add_layernorm_fwd(XM, Y, out, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+        ops.add_layernorm_fwd(XM, Y, out, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
+                              **scaled(s_ff, S))
     else:
         ops.cast_bf16(X.view(-1), LN.view(-1))                 # attention(x) on the raw input
         ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
         ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
         ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
         H1 = ws.get("l.H1", (M, d), f32)                       # LN1(x + attention(x)), fp32 + its bf16 operand copy
-        ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
+        ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps,
+                              **scaled(s_attn, S))
         ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
         ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
-        ops.add_layernorm_fwd(H1, Y, None, None, out, ln2.weight, ln2.bias, None, None, M, d, ln2.eps)
+        ops.add_layernorm_fwd(H1, Y, None, None, out, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
+                              **scaled(s_ff, S))
     return out.view(B, S, d).to(hidden_states.dtype)
 
 

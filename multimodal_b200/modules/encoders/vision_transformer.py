@@ -3,7 +3,9 @@
 (flash-style attention); a custom ``pooler`` module, if given, is applied to ``last_hidden_state`` as in the reference.
 `GlobalAveragePooler` (MAE fine-tuning head) is outside SURVEY.md §8.  With `patch_drop_rate` the module drops patches in
 training only (either grad mode, the same random draws as the reference): `hidden_states` and `last_hidden_state` are
-then [B, off + L, d] for the L kept patches (off = 1 with a CLS token)."""
+then [B, off + L, d] for the L kept patches (off = 1 with a CLS token).  With `drop_path_rate` the encoder layers apply
+stochastic depth in training only (either grad mode, the reference's per-layer rates and random draws, drawn after the
+patch-dropping draws)."""
 import warnings
 from typing import Any, Callable, Optional, Tuple, Union
 

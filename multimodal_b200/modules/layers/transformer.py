@@ -3,9 +3,16 @@ CoCa encoder returns) and the parameter containers `TransformerEncoderLayer` / `
 `TransformerDecoderLayer` / `TransformerDecoder` (:262-657) — same constructors, state-dict keys and creation order.
 The layers execute inside `engine_coca.LayerStack` (fused kernels), owned by VisionTransformer / CoCaTextDecoder /
 CoCaMultimodalDecoder; all four are also callable on their own (forward values, same kernels: `engine_layers.py`), the
-decoders with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive decoding."""
+decoders with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive decoding.
+
+With `drop_path_rate` an encoder layer applies stochastic depth as the reference does: one shared
+`StochasticDepth(p, "row")` (modules/layers/stochastic_depth.py) is both `attention_dropout` and `feedforward_dropout`,
+and `TransformerEncoder` gives layer i the rate `torch.linspace(0, drop_path_rate, n_layer)[i]`.  In training the
+runtimes draw the per-sample noise in the reference's order and scale each branch inside the residual-add and
+LayerNorm-backward kernels; it adds no parameters."""
 from typing import Callable, List, NamedTuple, Optional, Tuple
 
+import torch
 from torch import nn, Tensor
 
 
@@ -31,13 +38,15 @@ class TransformerEncoderLayer(nn.Module):
         from .mlp import MLP
         from .multi_head_attention import MultiHeadSelfAttention
         from .normalizations import Fp32LayerNorm
+        from .stochastic_depth import StochasticDepth
 
         _no_dropout(dropout, "TransformerEncoderLayer")
-        if drop_path_rate is not None:
-            raise NotImplementedError("stochastic depth (drop_path_rate) is not on the accelerated path")
         self.attention = MultiHeadSelfAttention(embed_dim=d_model, num_heads=n_head)
-        self.attention_dropout = nn.Dropout(dropout)
-        self.feedforward_dropout = nn.Dropout(dropout)
+        if drop_path_rate is not None:
+            self.attention_dropout = self.feedforward_dropout = StochasticDepth(drop_path_rate, mode="row")
+        else:
+            self.attention_dropout = nn.Dropout(dropout)
+            self.feedforward_dropout = nn.Dropout(dropout)
         self.feedforward = MLP(d_model, d_model, dim_feedforward, dropout=dropout, activation=activation)
         self.attention_layernorm = Fp32LayerNorm(d_model, eps=layer_norm_eps)
         self.feedforward_layernorm = Fp32LayerNorm(d_model, eps=layer_norm_eps)
@@ -57,9 +66,13 @@ class TransformerEncoder(nn.Module):
         super().__init__()
         from .normalizations import Fp32LayerNorm
 
+        if drop_path_rate is not None:
+            drop_rate = [x.item() for x in torch.linspace(0, drop_path_rate, n_layer)]
+        else:
+            drop_rate = [None for _ in range(n_layer)]
         self.layer = nn.ModuleList([
             TransformerEncoderLayer(d_model, n_head, dim_feedforward, dropout, activation, layer_norm_eps, norm_first,
-                                    drop_path_rate) for _ in range(n_layer)])
+                                    drop_rate[i]) for i in range(n_layer)])
         self.final_layer_norm = None
         if final_layer_norm_eps:
             self.final_layer_norm = Fp32LayerNorm(d_model, eps=final_layer_norm_eps)

@@ -140,15 +140,34 @@ def wgrad_splits(out_rows: int, out_cols: int, k: int, n_units: Optional[int] = 
     return best
 
 
-def cast_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+def cast_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None, branch_scale: Optional[torch.Tensor] = None,
+              rows_per_scale: int = 0) -> torch.Tensor:
+    """bf16 copy of src; with branch_scale (fp32 [rows / rows_per_scale], stochastic depth), row r of the 2-D src is
+    multiplied by branch_scale[r // rows_per_scale] first."""
     _chk(src, torch.float32, "src")
     if not src.is_contiguous():
         raise MMBError("cast_bf16: src must be contiguous")
     if out is None:
         out = torch.empty(src.shape, device=src.device, dtype=torch.bfloat16)
     _chk(out, torch.bfloat16, "out")
-    _lib.check(_lib.lib().mmb_cast_f32_to_bf16(_p(src), _p(out), src.numel(), _stream()), "mmb_cast_f32_to_bf16")
+    if branch_scale is None:
+        _lib.check(_lib.lib().mmb_cast_f32_to_bf16(_p(src), _p(out), src.numel(), _stream()), "mmb_cast_f32_to_bf16")
+        return out
+    if src.dim() != 2 or out.numel() != src.numel():
+        raise MMBError("cast_bf16: a branch_scale needs a 2-D src [rows, d] and an out of the same size")
+    _check_scale(branch_scale, src.shape[0], rows_per_scale)
+    _lib.check(_lib.lib().mmb_cast_f32_to_bf16_scaled(_p(src), _p(out), src.numel(), _p(branch_scale),
+                                                      rows_per_scale * src.shape[1], _stream()),
+               "mmb_cast_f32_to_bf16_scaled")
     return out
+
+
+def _check_scale(scale: torch.Tensor, M: int, rows_per_scale: int) -> None:
+    """Per-sample stochastic-depth factors: contiguous fp32 with one entry per rows_per_scale rows of M."""
+    _chk(scale, torch.float32, "branch_scale")
+    if rows_per_scale <= 0 or M % rows_per_scale or not scale.is_contiguous() or scale.numel() != M // rows_per_scale:
+        raise MMBError(f"branch_scale: expected a contiguous fp32 tensor of {M} / rows_per_scale = {rows_per_scale} "
+                       f"entries, got shape {tuple(scale.shape)}")
 
 
 def cast_f32(src: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
@@ -189,9 +208,21 @@ def _im2col_gather(img: torch.Tensor, keep: torch.Tensor, ps: int, out: torch.Te
 
 
 def add_layernorm_fwd(x_in, y, x_out, ln_bf16, ln_f32, gamma, beta, mean, rstd, M, d, eps, row_idx=None,
-                      rows_per_group=0):
+                      rows_per_group=0, branch_scale=None, rows_per_scale=0):
+    """x_out = x_in + y, LayerNorm of it.  branch_scale (fp32 [M / rows_per_scale], stochastic depth): row m adds
+    branch_scale[m // rows_per_scale] * y instead (not with a row gather)."""
     nbytes = M * d * (4 + (2 if y is not None else 0) + (4 if x_out is not None else 0) +
                       (2 if ln_bf16 is not None else 0) + (4 if ln_f32 is not None else 0))
+    if branch_scale is not None:
+        if rows_per_group > 0 or y is None:
+            raise MMBError("add_layernorm_fwd: a branch_scale needs y and excludes the row gather")
+        _check_scale(branch_scale, M, rows_per_scale)
+        with _timed("ln_fwd", nbytes + 4 * (M // rows_per_scale), "B"):
+            _lib.check(_lib.lib().mmb_add_layernorm_fwd_scaled(_p(x_in), _p(y), _p(x_out), _p(ln_bf16), _p(ln_f32),
+                                                               _p(gamma), _p(beta), _p(mean), _p(rstd), _p(branch_scale),
+                                                               rows_per_scale, M, d, float(eps), _stream()),
+                       "mmb_add_layernorm_fwd_scaled")
+        return
     with _timed("ln_fwd", nbytes, "B"):
         _lib.check(_lib.lib().mmb_add_layernorm_fwd(_p(x_in), _p(y), _p(x_out), _p(ln_bf16), _p(ln_f32), _p(gamma),
                                                     _p(beta), _p(mean), _p(rstd), _p(row_idx), rows_per_group, M, d,
@@ -204,9 +235,22 @@ def vit_embed_ln_fwd(patch_out, cls, pos, gamma, beta, x0, mean, rstd, B, S, d, 
 
 
 def layernorm_bwd(x, dy_bf16, dy_f32, mean, rstd, gamma, g_in, g_out, g_bf16, dgamma, dbeta, M, d, row_idx=None,
-                  rows_per_group=0, gsum=None):
+                  rows_per_group=0, gsum=None, branch_scale=None, rows_per_scale=0):
+    """LayerNorm backward + residual-gradient add.  branch_scale (fp32 [M / rows_per_scale], stochastic depth of the
+    branch that consumes g_bf16): g_bf16 = bf16(branch_scale[m // rows_per_scale] * g_out) and gsum sums it; g_out is
+    unscaled (not with a row scatter)."""
     nbytes = M * d * (4 + (2 if dy_bf16 is not None else 4) + (4 if g_in is not None else 0) +
                       (4 if g_out is not None else 0) + (2 if g_bf16 is not None else 0))
+    if branch_scale is not None:
+        if rows_per_group > 0 or g_bf16 is None:
+            raise MMBError("layernorm_bwd: a branch_scale needs g_bf16 and excludes the row scatter")
+        _check_scale(branch_scale, M, rows_per_scale)
+        with _timed("ln_bwd", nbytes + 4 * (M // rows_per_scale), "B"):
+            _lib.check(_lib.lib().mmb_layernorm_bwd_scaled(_p(x), _p(dy_bf16), _p(dy_f32), _p(mean), _p(rstd),
+                                                           _p(gamma), _p(g_in), _p(g_out), _p(g_bf16), _p(dgamma),
+                                                           _p(dbeta), _p(branch_scale), rows_per_scale, M, d, _p(gsum),
+                                                           _stream()), "mmb_layernorm_bwd_scaled")
+        return
     with _timed("ln_bwd", nbytes, "B"):
         _lib.check(_lib.lib().mmb_layernorm_bwd(_p(x), _p(dy_bf16), _p(dy_f32), _p(mean), _p(rstd), _p(gamma), _p(g_in),
                                                 _p(g_out), _p(g_bf16), _p(dgamma), _p(dbeta), _p(row_idx),
