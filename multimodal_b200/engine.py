@@ -8,6 +8,7 @@ the reference call stack (SURVEY.md §3.1):
 """
 from __future__ import annotations
 
+import math
 import os
 
 from typing import Dict, List, Optional, Sequence
@@ -49,31 +50,44 @@ def _require_cuda(dev: torch.device) -> None:
 
 
 class ParamStore:
-    """Flat bf16 shadow (tensor-core operand copies) + flat fp32 gradient buffer for a list of parameters."""
+    """Flat bf16 shadow (tensor-core operand copies) + flat fp32 gradient buffer for a list of parameters.
+    fp32_only: parameters the kernels only ever read in fp32 (embedding tables); they go last and get no bf16 shadow."""
 
-    def __init__(self, params: Sequence[nn.Parameter]):
-        self.params: List[nn.Parameter] = list(params)
+    def __init__(self, params: Sequence[nn.Parameter], fp32_only: Sequence[nn.Parameter] = ()):
+        plain = {id(p) for p in fp32_only}
+        self.params: List[nn.Parameter] = ([p for p in params if id(p) not in plain] +
+                                           [p for p in params if id(p) in plain])
         if not self.params:
             raise MMBError("ParamStore: no parameters")
         dev = self.params[0].device
         _require_cuda(dev)
         self.device = dev
         self.off: Dict[int, int] = {}
-        off = 0
+        off, n_shadow = 0, None
         for p in self.params:
             if p.dtype != torch.float32:
                 raise MMBError("parameters must be fp32 (bf16 operand copies are made internally)")
+            if id(p) in plain and n_shadow is None:
+                n_shadow = off
             self.off[id(p)] = off
             off += -(-p.numel() // _ALIGN) * _ALIGN
         self.total = off
-        self.wb = torch.empty(self.total, device=dev, dtype=torch.bfloat16)
-        self.g = torch.zeros(self.total, device=dev, dtype=torch.float32)
+        self.wb = torch.empty(off if n_shadow is None else n_shadow, device=dev, dtype=torch.bfloat16)
+        self._g: Optional[torch.Tensor] = None
         self._seen: Dict[int, tuple] = {}
         self.master: Optional[torch.Tensor] = None  # set by flatten_()
         self._shadow_fresh = False
         self._epoch = _WEIGHT_EPOCH[0]
+        self._shadowed = [p for p in self.params if self.off[id(p)] < self.wb.numel()]
         self._packs: List[list] = []   # [key tensor, parts, version seen]: fp32 concatenations kept current by refresh()
         self._keys: List[torch.Tensor] = []
+
+    @property
+    def g(self) -> torch.Tensor:
+        """The fp32 gradient buffer, allocated on first use: a store that only serves no_grad forwards never holds it."""
+        if self._g is None:
+            self._g = torch.zeros(self.total, device=self.device, dtype=torch.float32)
+        return self._g
 
     # -- views ------------------------------------------------------------------------------------------
     def shadow(self, p: nn.Parameter) -> torch.Tensor:
@@ -139,12 +153,12 @@ class ParamStore:
         """Make the bf16 shadows current (re-cast whatever changed since the last call)."""
         if self.master is not None:
             if not self._shadow_fresh or self._epoch != _WEIGHT_EPOCH[0]:
-                ops.cast_bf16(self.master, self.wb)
+                ops.cast_bf16(self.master[:self.wb.numel()], self.wb)
                 self._refresh_packs(True)
                 self._shadow_fresh = True
                 self._epoch = _WEIGHT_EPOCH[0]
             return
-        for p in self.params:
+        for p in self._shadowed:
             if p.device != self.device:
                 raise MMBError("parameter moved to another device after the runtime was created")
             key = (p._version, p.data_ptr(), _WEIGHT_EPOCH[0])
@@ -167,7 +181,7 @@ class Workspace:
     def __init__(self, device):
         self.device = device
         self.bufs: Dict[str, torch.Tensor] = {}
-        self.X0: Optional[torch.Tensor] = None      # set by TransformerStack.forward(training=True): layer-0 input
+        self.X0: Optional[torch.Tensor] = None      # set by TransformerStack.forward when saving: layer-0 input
         self.kmask: Optional[torch.Tensor] = None   # ... and the key-padding mask / [B,S,S] mask / cross-attention
         self.mask3: Optional[torch.Tensor] = None   #     source that forward used
         self.enc: Optional[torch.Tensor] = None
@@ -324,91 +338,125 @@ def patch_embed_bwd(G: torch.Tensor, conv: nn.Module, cls: Optional[torch.Tensor
         ops.colsum_bf16(DP, st.grad(conv.bias), rows, d, d)
 
 
+def require_head_dim_64(d: int, heads: int) -> None:
+    if d % heads or d // heads != 64:
+        raise MMBError(f"attention kernels support head_dim 64 only (got d={d}, heads={heads})")
+
+
 class TransformerStack:
-    """L pre-norm encoder layers (torch.nn.TransformerEncoderLayer parameter layout), QuickGELU or GELU MLP."""
+    """L pre-norm encoder / decoder layers (torch.nn.TransformerEncoderLayer parameter layout), QuickGELU or GELU MLP,
+    head_dim 64 / 96 / 128 (a forward that saves for the backward: 64)."""
+
+    # without a save Workspace, a buffer that is dead before its namesake is written shares that namesake's storage
+    _SHARED = {"LN2": "LN1", "LNC": "LN1", "OC": "O"}
 
     def __init__(self, layers: Sequence[nn.Module], store: ParamStore, ws: Workspace, *, d: int, heads: int, ff: int,
-                 causal: bool, act: int, prefix: str):
+                 act: int, prefix: str):
         self.layers = list(layers)
         self.store, self.ws = store, ws
-        self.d, self.H, self.ff, self.causal, self.act, self.prefix = d, heads, ff, causal, act, prefix
-        if d % heads or d // heads != 64:
-            raise MMBError(f"attention kernels support head_dim 64 only (got d={d}, heads={heads})")
-        self.scale = 1.0 / 8.0
+        self.d, self.H, self.ff, self.act, self.prefix = d, heads, ff, act, prefix
+        self.hd = d // heads
+        if d % heads or self.hd not in (64, 96, 128):
+            raise MMBError(f"unsupported head_dim {self.hd}")
+        self.scale = 1.0 / math.sqrt(self.hd)
         self.L = len(self.layers)
-        self.saved = False
 
-    def _buf(self, name, l, shape, dtype, training):
-        key = f"{self.prefix}.{name}.{l if training else 0}"
-        return (self._save if training else self.ws).get(key, shape, dtype)
+    def _bufs(self, save):
+        """buf(name, layer, shape, dtype): per-layer buffers in `save`, or without one the workspace's buffer of that
+        name, looked up once per forward (every layer has the same shapes)."""
+        if save is not None:
+            return lambda name, l, shape, dt: save.get(f"{self.prefix}.{name}.{l}", shape, dt)
+        got: Dict[str, torch.Tensor] = {}
 
-    def forward(self, X0: torch.Tensor, B: int, S: int, training: bool, kmask: Optional[torch.Tensor] = None,
-                save: Optional["Workspace"] = None, mask3: Optional[torch.Tensor] = None,
-                enc: Optional[torch.Tensor] = None, S_enc: int = 0, scales=None):
+        def buf(name, l, shape, dt):
+            if name not in got:
+                got[name] = self.ws.get(f"{self.prefix}.{self._SHARED.get(name, name)}.0", shape, dt)
+            return got[name]
+        return buf
+
+    def forward(self, X0: torch.Tensor, B: int, S: int, save: Optional["Workspace"], *, causal: bool = False,
+                kmask: Optional[torch.Tensor] = None, mask3: Optional[torch.Tensor] = None,
+                enc: Optional[torch.Tensor] = None, S_enc: int = 0, scales=None,
+                hidden: Optional[List[torch.Tensor]] = None, attns: Optional[List[torch.Tensor]] = None):
         """X0: fp32 [B*S, d] residual stream entering layer 0.  Returns (XM_last fp32, Y bf16): the final residual
         stream is XM_last + Y (the add is fused into whichever LayerNorm consumes it; with stochastic depth the caller
-        scales that add by `top_scale`).
+        scales that add by the last layer's feed-forward factor).
+        save: the Workspace that receives the activations (and the arguments below) the backward reads, or None: a
+        forward that keeps nothing runs in the stack's own workspace, one buffer per name for all layers.
         scales: stochastic depth (modules/layers/stochastic_depth.drop_path_scales): per layer the (attention,
         feed-forward) per-sample factors fp32 [B] or None; each scales its branch inside the residual add that
         follows it, and the backward scales the gradient entering the branch.  Not with cross-attention layers.
         kmask: optional uint8 [B*S] key-padding mask (1 = attend).  mask3: optional uint8 [B, S, S] mask (general
         attention kernels).  enc / S_enc: bf16 [B*S_enc, d_kv] cross-attention source for layers that carry a
-        `cross_attn` block (TransformerDecoderLayer: modules/layers/transformer.py:354-377).  save: the Workspace that receives the activations a
-        training forward keeps for its backward (default: the stack's own — ONE in-flight training forward; callers
-        that run the same stack several times before the backward pass a fresh Workspace per call)."""
-        self._save = save if save is not None else self.ws
-        self._save.kmask = kmask if training else None
-        self._save.mask3 = mask3 if training else None
-        self._save.enc, self._save.S_enc = (enc, S_enc) if training else (None, 0)
+        `cross_attn` block (TransformerDecoderLayer: modules/layers/transformer.py:354-377).
+        hidden: list that receives each layer's input stream [B, S, d], X0 first (without `save`, allocated per call:
+        they are returned to the user).  attns: list that receives each layer's attention probabilities fp32
+        [B, H, S, S] (ops.attention_probs, recomputed from the packed QKV and the row LSE)."""
         if scales is not None and enc is not None:
             raise MMBError("stochastic depth is applied to encoder layers only (no cross-attention)")
-        self._save.scales, self._save.rows_per_scale = scales, S
+        if save is None:
+            self.ws.X0 = None   # this forward overwrites what a saving forward into the stack's own workspace kept
+        else:
+            if self.hd != 64:
+                raise MMBError(f"training needs head_dim 64 in the layer stacks (got {self.hd}); the poolers may differ")
+            save.X0, save.causal, save.kmask, save.mask3, save.enc, save.S_enc = X0, causal, kmask, mask3, enc, S_enc
+            save.scales, save.rows_per_scale = scales, S
         st, d, ff, H = self.store, self.d, self.ff, self.H
         M = B * S
         bf, f32 = torch.bfloat16, torch.float32
+        buf = self._bufs(save)
         Y = self.ws.get(f"{self.prefix}.Y", (M, d), bf)
-        XA_prev, XM_prev = X0, None
+        if hidden is not None:
+            hidden.append(X0.view(B, S, d))
+        XA, XM_prev = X0, None
         for l, layer in enumerate(self.layers):
             at = layer.self_attn
             s_attn = scales[l][0] if scales is not None else None
             s_prev_ff = scales[l - 1][1] if scales is not None and l > 0 else None
-            LN1 = self._buf("LN1", l, (M, d), bf, training)
-            QKV = self._buf("QKV", l, (M, 3 * d), bf, training)
-            O = self._buf("O", l, (M, d), bf, training)
-            LSE = self._buf("LSE", l, (B * H * S,), f32, training)
-            XM = self._buf("XM", l, (M, d), f32, training)
-            LN2 = self._buf("LN2", l, (M, d), bf, training)
-            PRE = self._buf("PRE", l, (M, ff), bf, training)
-            HACT = self._buf("HACT", l, (M, ff), bf, training)
-            m1 = self._buf("m1", l, (M,), f32, training); r1 = self._buf("r1", l, (M,), f32, training)
-            m2 = self._buf("m2", l, (M,), f32, training); r2 = self._buf("r2", l, (M,), f32, training)
+            LN1 = buf("LN1", l, (M, d), bf)
+            QKV = buf("QKV", l, (M, 3 * d), bf)
+            O = buf("O", l, (M, d), bf)
+            LSE = buf("LSE", l, (B * H * S,), f32)
+            XM = buf("XM", l, (M, d), f32)
+            LN2 = buf("LN2", l, (M, d), bf)
+            PRE = buf("PRE", l, (M, ff), bf)
+            HACT = buf("HACT", l, (M, ff), bf)
+            m1 = buf("m1", l, (M,), f32); r1 = buf("r1", l, (M,), f32)
+            m2 = buf("m2", l, (M,), f32); r2 = buf("r2", l, (M,), f32)
             if l == 0:
                 XA = X0
                 ops.add_layernorm_fwd(XA, None, None, LN1, None, layer.norm1.weight, layer.norm1.bias, m1, r1, M, d,
                                       layer.norm1.eps)
             else:
-                XA = self._buf("XA", l, (M, d), f32, training)
+                XA = (torch.empty((M, d), device=X0.device, dtype=f32) if save is None and hidden is not None
+                      else buf("XA", l, (M, d), f32))
                 ops.add_layernorm_fwd(XM_prev, Y, XA, LN1, None, layer.norm1.weight, layer.norm1.bias, m1, r1, M, d,
                                       layer.norm1.eps, **scaled(s_prev_ff, S))
+                if hidden is not None:
+                    hidden.append(XA.view(B, S, d))
             ops.gemm(LN1, st.shadow(at.in_proj_weight), bias=at.in_proj_bias, out=QKV)
-            ops.self_attention(QKV, O, LSE, B, S, H, 64, self.causal, self.scale, kmask=kmask, mask=mask3)
+            ops.self_attention(QKV, O, LSE, B, S, H, self.hd, causal, self.scale, kmask=kmask, mask=mask3)
+            if attns is not None:
+                P = torch.empty((B, H, S, S), device=X0.device, dtype=f32)
+                ops.attention_probs(QKV, LSE, kmask, P, B, S, H, causal, self.scale)
+                attns.append(P)
             ops.gemm(O, st.shadow(at.out_proj.weight), bias=at.out_proj.bias, out=Y)
             ca = getattr(layer, "cross_attn", None)
             if ca is not None and enc is not None:
                 # x1 = x + self-attention (XM);  x2 = x1 + cross-attention(LN_c(x1), enc) (XC);  the MLP reads LN2(x2)
                 lnc = layer.norm_cross
                 Se = S_enc
-                LNC = self._buf("LNC", l, (M, d), bf, training)
-                QC = self._buf("QC", l, (M, d), bf, training)
-                KVC = self._buf("KVC", l, (B * Se, 2 * d), bf, training)
-                OC = self._buf("OC", l, (M, d), bf, training)
-                XC = self._buf("XC", l, (M, d), f32, training)
-                mc = self._buf("mc", l, (M,), f32, training); rc = self._buf("rc", l, (M,), f32, training)
+                LNC = buf("LNC", l, (M, d), bf)
+                QC = buf("QC", l, (M, d), bf)
+                KVC = buf("KVC", l, (B * Se, 2 * d), bf)
+                OC = buf("OC", l, (M, d), bf)
+                XC = buf("XC", l, (M, d), f32)
+                mc = buf("mc", l, (M,), f32); rc = buf("rc", l, (M,), f32)
                 ops.add_layernorm_fwd(XA, Y, XM, LNC, None, lnc.weight, lnc.bias, mc, rc, M, d, lnc.eps)
                 ops.gemm(LNC, st.shadow(ca.q_w), bias=ca.q_b, out=QC)
                 ops.gemm(enc, st.shadow(ca.kv_w), bias=ca.kv_b, out=KVC)
-                ops.attention_fwd_generic(QC, KVC[:, :d], KVC[:, d:], OC, B=B, Sq=S, Skv=Se, H=H, head_dim=64, bsq=S * d,
-                                          bsk=Se * 2 * d, bsv=Se * 2 * d, bso=S * d, scale=self.scale)
+                ops.attention_fwd_generic(QC, KVC[:, :d], KVC[:, d:], OC, B=B, Sq=S, Skv=Se, H=H, head_dim=self.hd,
+                                          bsq=S * d, bsk=Se * 2 * d, bsv=Se * 2 * d, bso=S * d, scale=self.scale)
                 ops.gemm(OC, st.shadow(ca.out_proj.weight), bias=ca.out_proj.bias, out=Y)
                 ops.add_layernorm_fwd(XM, Y, XC, LN2, None, layer.norm2.weight, layer.norm2.bias, m2, r2, M, d,
                                       layer.norm2.eps)
@@ -420,9 +468,6 @@ class TransformerStack:
                      out2=HACT, act=self.act)
             ops.gemm(HACT, st.shadow(layer.linear2.weight), bias=layer.linear2.bias, out=Y)
             XM_prev = XM
-        self.saved = training
-        self._X0 = X0 if training else None
-        self._save.X0 = self._X0
         return XM_prev, Y
 
     @staticmethod
@@ -436,18 +481,14 @@ class TransformerStack:
         """Gradient slot of the last layer's linear2.bias: the producer of the incoming Gb sums its columns into it."""
         return self.store.grad(self.layers[-1].linear2.bias)
 
-    def backward(self, G: torch.Tensor, Gb: torch.Tensor, B: int, S: int, on_layer_done=None,
-                 top_bias_done: bool = False, save: Optional["Workspace"] = None) -> torch.Tensor:
+    def backward(self, G: torch.Tensor, Gb: torch.Tensor, B: int, S: int, *, save: "Workspace", on_layer_done=None,
+                 top_bias_done: bool = False) -> torch.Tensor:
         """G (fp32) / Gb (bf16 copy, times the last MLP branch's stochastic-depth factor when the forward had
-        scales): gradient w.r.t. the final residual stream [B*S, d].  Returns G w.r.t. X0
-        (in place).  Parameter gradients are ACCUMULATED into the ParamStore's flat fp32 buffer.
+        scales): gradient w.r.t. the final residual stream [B*S, d]; save: the Workspace the forward saved into.
+        Returns G w.r.t. X0 (in place).  Parameter gradients are ACCUMULATED into the ParamStore's flat fp32 buffer.
         The bias gradients of linear2 / out_proj are column sums of Gb; they are produced by the LayerNorm-backward
         kernel that writes Gb (`gsum`), not by a separate pass (top_bias_done: the caller's kernel did the top one)."""
-        if save is None:
-            if not self.saved:
-                raise MMBError("backward called without a saved training forward")
-            save = self.ws
-        X0, kmask = save.X0, getattr(save, "kmask", None)
+        X0, kmask, causal = save.X0, getattr(save, "kmask", None), getattr(save, "causal", False)
         mask3, enc, Se = getattr(save, "mask3", None), getattr(save, "enc", None), getattr(save, "S_enc", 0)
         scales = getattr(save, "scales", None)
         save.dENC = None
@@ -503,7 +544,7 @@ class TransformerStack:
                 dQC = self.ws.get(f"{self.prefix}.dQC", (M, d), bf)
                 dKVC = self.ws.get(f"{self.prefix}.dKVC", (B * Se, 2 * d), bf)
                 ops.attention_bwd_generic(QC, KVC[:, :d], KVC[:, d:], T1, dKVC[:, :d], dKVC[:, d:], dq=dQC, B=B, Sq=S,
-                                          Skv=Se, H=H, head_dim=64, bsq=S * d, bsk=Se * 2 * d, bsv=Se * 2 * d, bso=S * d,
+                                          Skv=Se, H=H, head_dim=self.hd, bsq=S * d, bsk=Se * 2 * d, bsv=Se * 2 * d, bso=S * d,
                                           scale=self.scale)
                 ops.gemm(dQC, LNC, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(ca.q_w), splits=sp(d, d, M),
                          accumulate=True)
@@ -523,7 +564,7 @@ class TransformerStack:
             ops.gemm(Gb, O, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(at.out_proj.weight),
                      splits=sp(d, d, M), accumulate=True)
             ops.gemm(Gb, st.shadow(at.out_proj.weight), b_mn=True, out=T1)  # dO
-            ops.self_attention(QKV, O, LSE, B, S, H, 64, self.causal, self.scale, kmask=kmask, mask=mask3, dout=T1,
+            ops.self_attention(QKV, O, LSE, B, S, H, self.hd, causal, self.scale, kmask=kmask, mask=mask3, dout=T1,
                                dqkv=T3)
             ops.gemm(T3, LN1, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(at.in_proj_weight),
                      splits=sp(3 * d, d, M), accumulate=True)
@@ -549,9 +590,9 @@ class ViTTower:
         layer0 = mod.encoder.layers[0]
         self.d, self.ps = d, mod.conv.weight.shape[2]
         self.E = mod.projection.shape[1]
+        require_head_dim_64(d, layer0.self_attn.num_heads)
         self.stack = TransformerStack(mod.encoder.layers, self.store, self.ws, d=d, heads=layer0.self_attn.num_heads,
-                                      ff=layer0.linear1.weight.shape[0], causal=False, act=ops.ACT_QUICK_GELU,
-                                      prefix="img")
+                                      ff=layer0.linear1.weight.shape[0], act=ops.ACT_QUICK_GELU, prefix="img")
         self.gen = 0
 
     def forward(self, image: torch.Tensor, training: bool, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -581,7 +622,7 @@ class ViTTower:
         ops.gemm(PATCH, wconv, out=PO)
         ops.vit_embed_ln_fwd(PO, mod.cls_token_embedding, mod.positional_embedding, mod.ln_pre.weight, mod.ln_pre.bias,
                              X0, m0, r0, B, S, d, mod.ln_pre.eps)
-        XM, Y = self.stack.forward(X0, B, S, training)
+        XM, Y = self.stack.forward(X0, B, S, ws if training else None)
         XSEL = ws.get("img.XSEL", (B, d), f32)
         LNP = ws.get("img.LNP", (B, d), bf)
         mP = ws.get("img.mP", (B,), f32); rP = ws.get("img.rP", (B,), f32)
@@ -609,7 +650,7 @@ class ViTTower:
         ops.layernorm_bwd(XSEL, None, dLNP, ws.get("img.mP", (B,), f32), ws.get("img.rP", (B,), f32), mod.ln_post.weight, None, G, Gb,
                           st.grad(mod.ln_post.weight), st.grad(mod.ln_post.bias), B, d, row_idx=None, rows_per_group=S,
                           gsum=self.stack.top_bias_grad())
-        self.stack.backward(G, Gb, B, S, on_layer_done=getattr(self, "layer_done_cb", None), top_bias_done=True)
+        self.stack.backward(G, Gb, B, S, save=ws, on_layer_done=getattr(self, "layer_done_cb", None), top_bias_done=True)
         PO = ws.get("img.PO", (B * P, d), bf)
         DP = ws.get("img.DP", (B * P, d), bf)
         ops.vit_embed_ln_bwd(PO, mod.cls_token_embedding, mod.positional_embedding, G, ws.get("img.m0", (M,), f32), ws.get("img.r0", (M,), f32),
@@ -632,8 +673,9 @@ class TextTower:
         layer0 = mod.encoder.layers[0]
         self.d = mod.width
         self.E = mod.projection.weight.shape[0]
+        require_head_dim_64(self.d, layer0.self_attn.num_heads)
         self.stack = TransformerStack(mod.encoder.layers, self.store, self.ws, d=self.d,
-                                      heads=layer0.self_attn.num_heads, ff=layer0.linear1.weight.shape[0], causal=True,
+                                      heads=layer0.self_attn.num_heads, ff=layer0.linear1.weight.shape[0],
                                       act=ops.ACT_QUICK_GELU, prefix="txt")
         self.gen = 0
 
@@ -649,7 +691,7 @@ class TextTower:
         X0 = ws.get("txt.X0", (B * S, d), f32)
         V = mod.token_embedding.weight.shape[0]
         ops.text_embed_fwd(text, mod.token_embedding.weight, mod.positional_embedding, X0, B, S, d, V)
-        XM, Y = self.stack.forward(X0, B, S, training and not return_hidden_state)
+        XM, Y = self.stack.forward(X0, B, S, ws if training and not return_hidden_state else None, causal=True)
         if return_hidden_state:
             HS = torch.empty((B, S, d), device=text.device, dtype=f32)
             ops.add_layernorm_fwd(XM, Y, None, None, HS, mod.ln_final.weight, mod.ln_final.bias, None, None, B * S, d,
@@ -686,7 +728,7 @@ class TextTower:
         ops.layernorm_bwd(XSEL, None, dLNF, ws.get("txt.mF", (B,), f32), ws.get("txt.rF", (B,), f32), mod.ln_final.weight, None, G, Gb,
                           st.grad(mod.ln_final.weight), st.grad(mod.ln_final.bias), B, d, row_idx=IDX, rows_per_group=S,
                           gsum=self.stack.top_bias_grad())
-        self.stack.backward(G, Gb, B, S, top_bias_done=True)
+        self.stack.backward(G, Gb, B, S, save=ws, top_bias_done=True)
         ops.batch_sum(G, st.grad(mod.positional_embedding), B, S * d, S * d)
         ops.text_embed_bwd(self.tokens, G, st.grad(mod.token_embedding.weight), B, S, d)
 

@@ -1,7 +1,7 @@
-"""Training runtime of the CoCa model family (BASELINE.json config 5 / SURVEY.md §8 a14 + f3 as a training step):
-forwards that keep what the backward needs + explicit backward schedules, behind torch.autograd Functions, so that
-`CoCaModel` / `CoCaForPretraining` train with ``loss.backward()`` like the reference (models/coca/coca_model.py:69-130,
-398-454 under autograd).
+"""Runtime of the CoCa model family (BASELINE.json config 5 / SURVEY.md §8 a14 + f3 as a training step), one per module
+for both grad modes: forwards that keep what the backward needs + explicit backward schedules, behind torch.autograd
+Functions, so that `CoCaModel` / `CoCaForPretraining` train with ``loss.backward()`` like the reference
+(models/coca/coca_model.py:69-130, 398-454 under autograd); under torch.no_grad() the same forwards keep nothing.
 
 All layer stacks run on ``engine.TransformerStack`` (the CLIP towers' fused schedule and kernels):
   vision encoder      : packed `input_proj` self-attention (tensor-core fwd / bwd), erf-GELU MLP, optional final LayerNorm
@@ -49,13 +49,13 @@ def _qkv_first(layers) -> List[nn.Parameter]:
     return out
 
 
-def _store_for(owner: nn.Module, first: Sequence[nn.Parameter]) -> ParamStore:
+def _store_for(owner: nn.Module, first: Sequence[nn.Parameter], fp32_only: Sequence[nn.Parameter] = ()) -> ParamStore:
     params, seen = list(first), {id(p) for p in first}
     for p in owner.parameters():
         if id(p) not in seen:
             seen.add(id(p))
             params.append(p)
-    return ParamStore(params)
+    return ParamStore(params, fp32_only)
 
 
 def _adapters(layers, st: ParamStore):
@@ -85,38 +85,38 @@ def _adapters(layers, st: ParamStore):
 class _Stack:
     """ParamStore + TransformerStack over a list of TorchMultimodal pre-norm encoder / decoder layers."""
 
-    def __init__(self, owner: nn.Module, layers, prefix: str, causal: bool):
+    def __init__(self, owner: nn.Module, layers, prefix: str, fp32_only: Sequence[nn.Parameter] = ()):
         layers = list(layers)
         l0 = layers[0]
         if not l0.norm_first:
             raise MMBError("only pre-norm (norm_first=True) layers are on the accelerated path")
-        self.store = _store_for(owner, _qkv_first(layers))
+        self.store = _store_for(owner, _qkv_first(layers), fp32_only)
         self.device = self.store.device
         self.d = l0.attention_layernorm.normalized_shape[0]
-        H = l0.attention.num_heads
-        if self.d // H != 64:
-            raise MMBError(f"training needs head_dim 64 in the layer stacks (got {self.d // H}); the poolers may differ")
         self.ws = Workspace(self.device)
-        self.stack = TransformerStack(_adapters(layers, self.store), self.store, self.ws, d=self.d, heads=H,
-                                      ff=l0.feedforward.model[0].weight.shape[0], causal=causal,
+        self.stack = TransformerStack(_adapters(layers, self.store), self.store, self.ws, d=self.d,
+                                      heads=l0.attention.num_heads, ff=l0.feedforward.model[0].weight.shape[0],
                                       act=act_code(l0.feedforward.model[1]), prefix=prefix)
         self.prefix, self.L = prefix, len(layers)
         self.layers = layers     # the modules themselves: their StochasticDepth (drop_path_rate), if any
 
-    def finish(self, XM, Y, M: int, ln: Optional[nn.Module], save: Workspace):
+    def finish(self, XM, Y, B: int, S: int, ln: Optional[nn.Module], save: Optional[Workspace], scales,
+               LASTb: Optional[torch.Tensor] = None):
         """XF = XM + Y (the residual stream after the last layer; Y times the last MLP branch's stochastic-depth
-        factor when the forward drew one); LAST = ln(XF) when a final LayerNorm exists."""
-        d, pfx = self.d, self.prefix
+        factor when `scales` has one); LAST = ln(XF) when a final LayerNorm exists, and its bf16 copy into LASTb if
+        given.  XF / LAST are returned to the caller: allocated per call."""
+        d, pfx, M = self.d, self.prefix, B * S
         f32 = torch.float32
+        stats = save if save is not None else self.ws
         XF = torch.empty((M, d), device=self.device, dtype=f32)
         LAST = torch.empty((M, d), device=self.device, dtype=f32) if ln is not None else None
         aff = ln if ln is not None else self.stack.layers[0].norm1   # affine terms unused when nothing is normalised
-        scale, rows = self.stack.top_scale(save)
-        ops.add_layernorm_fwd(XM, Y, XF, None, LAST, aff.weight, aff.bias,
-                              save.get(f"{pfx}.mF", (M,), f32) if ln is not None else None,
-                              save.get(f"{pfx}.rF", (M,), f32) if ln is not None else None, M, d, aff.eps,
-                              **scaled(scale, rows))
-        save.XF = XF
+        ops.add_layernorm_fwd(XM, Y, XF, LASTb, LAST, aff.weight, aff.bias,
+                              stats.get(f"{pfx}.mF", (M,), f32) if ln is not None else None,
+                              stats.get(f"{pfx}.rF", (M,), f32) if ln is not None else None, M, d, aff.eps,
+                              **scaled(scales[-1][1] if scales is not None else None, S))
+        if save is not None:
+            save.XF = XF
         return XF, LAST
 
     def start_backward(self, save: Workspace, M: int, ln: Optional[nn.Module], dLAST, dXF):
@@ -145,32 +145,48 @@ def _f32(t: Optional[torch.Tensor], shape) -> Optional[torch.Tensor]:
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# One runtime per module.  `forward(data, diff) -> (outputs, save)` / `backward(save, *d outputs)` are driven by
+# engine.run under autograd; `infer(...)` is the torch.no_grad() call: the same front end, stack and finish without a
+# save Workspace (scratch in the runtime's workspace, returned tensors allocated per call), then the tails only
+# inference has.  A backward reads only its own save, so no_grad calls may run between a forward and its backward.
 class VisionTrainRuntime:
     """VisionTransformer (modules/encoders/vision_transformer.py:56-89).  Output: last_hidden_state [B*S, d]."""
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.s = _Stack(mod, mod.encoder.layer, "cvit", causal=False)
+        self.s = _Stack(mod, mod.encoder.layer, "cvit")
         self.store = self.s.store
 
-    def forward(self, data, diff):
-        images, image_patches_mask = data
+    def _forward(self, images, image_patches_mask, save: Optional[Workspace]):
         emb, s, st = self.mod.embeddings, self.s, self.store
         d, conv = s.d, emb.conv_projection
         st.refresh()
-        save = Workspace(s.device)
-        drop = patch_keep_indices(emb, images.shape[0], images.device)   # the same draws as VisionRuntime.forward
+        drop = patch_keep_indices(emb, images.shape[0], images.device)   # training with patch_drop_rate
         keep = drop[0] if drop is not None else None
-        scales = drop_path_scales(s.layers, images.shape[0], images.device)
+        scales = drop_path_scales(s.layers, images.shape[0], images.device)   # training with drop_path_rate
         X0, B, S, P, pm = patch_embed_fwd(images, conv, st.shadow2d(conv.weight),
                                           emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
-                                          emb.mask_token, image_patches_mask, s.ws, save, "cvit", keep=keep)
-        XM, Y = s.stack.forward(X0, B, S, True, save=save, scales=scales)
-        XF, LAST = s.finish(XM, Y, B * S, self.mod.encoder.final_layer_norm, save)
-        save.B, save.S, save.P, save.pm, save.keep = B, S, P, pm, keep
-        self.last_hidden = ([X0.view(B, S, d)] + [save.bufs[f"cvit.XA.{l}"].view(B, S, d) for l in range(1, s.L)]
-                            + [XF.view(B, S, d)])
-        return ((LAST if LAST is not None else XF),), save
+                                          emb.mask_token, image_patches_mask, s.ws, save if save is not None else s.ws,
+                                          "cvit", keep=keep)
+        hidden: List[torch.Tensor] = []
+        XM, Y = s.stack.forward(X0, B, S, save, scales=scales, hidden=hidden)
+        XF, LAST = s.finish(XM, Y, B, S, self.mod.encoder.final_layer_norm, save, scales)
+        hidden.append(XF.view(B, S, d))
+        return (LAST if LAST is not None else XF), hidden, (B, S, P, pm, keep)
+
+    def forward(self, data, diff):
+        images, image_patches_mask = data
+        save = Workspace(self.s.device)
+        last, self.last_hidden, (save.B, save.S, save.P, save.pm, save.keep) = self._forward(images, image_patches_mask,
+                                                                                               save)
+        return (last,), save
+
+    def infer(self, images, image_patches_mask=None):
+        from .modules.layers.transformer import TransformerOutput
+
+        last, hidden, _ = self._forward(images, image_patches_mask, None)
+        return TransformerOutput(last_hidden_state=last.view(hidden[-1].shape), pooler_output=None, hidden_states=hidden,
+                                 attentions=None)
 
     def backward(self, save, dOUT):
         emb, s = self.mod.embeddings, self.s
@@ -187,7 +203,9 @@ class VisionTrainRuntime:
 
 
 class PoolerTrainRuntime:
-    """AttentionPooler (modules/layers/attention_pooler.py:16-72).  Input x [B, S, d_in] (differentiable)."""
+    """AttentionPooler (modules/layers/attention_pooler.py:16-72): learned queries cross-attend to the LayerNorm-ed
+    input; the query projection is batch independent and computed once per call for [n_queries, d].
+    Input x [B, S, d_in] (differentiable)."""
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
@@ -205,39 +223,50 @@ class PoolerTrainRuntime:
         H = m.attn.num_heads
         return nq, dout, H, dout // H
 
-    def forward(self, data, diff):
-        (x,) = diff
+    def _forward(self, x, save: Optional[Workspace]):
         m, st = self.mod, self.store
         at = m.attn
         B, S, din = x.shape
         nq, dout, H, hd = self._dims()
-        if hd not in (64, 96, 128):
-            raise MMBError(f"unsupported pooler head_dim {hd}")
         bf, f32 = torch.bfloat16, torch.float32
         st.refresh()
-        save = Workspace(self.device)
+        keep = save if save is not None else self.ws
         x32 = x.contiguous().float().view(B * S, din)
-        xk = save.get("xk", (B * S, din), bf)
-        ops.add_layernorm_fwd(x32, None, None, xk, None, m.ln_k.weight, m.ln_k.bias, save.get("mk", (B * S,), f32),
-                              save.get("rk", (B * S,), f32), B * S, din, m.ln_k.eps)
-        qn = save.get("qn", (nq, dout), bf)
-        ops.add_layernorm_fwd(m.query.data, None, None, qn, None, m.ln_q.weight, m.ln_q.bias, save.get("mq", (nq,), f32),
-                              save.get("rq", (nq,), f32), nq, dout, m.ln_q.eps)
-        Qp = save.get("Qp", (nq, dout), bf)
+        xk = keep.get("xk", (B * S, din), bf)
+        ops.add_layernorm_fwd(x32, None, None, xk, None, m.ln_k.weight, m.ln_k.bias, keep.get("mk", (B * S,), f32),
+                              keep.get("rk", (B * S,), f32), B * S, din, m.ln_k.eps)
+        qn = keep.get("qn", (nq, dout), bf)
+        ops.add_layernorm_fwd(m.query.data, None, None, qn, None, m.ln_q.weight, m.ln_q.bias, keep.get("mq", (nq,), f32),
+                              keep.get("rq", (nq,), f32), nq, dout, m.ln_q.eps)
+        Qp = keep.get("Qp", (nq, dout), bf)
         ops.gemm(qn, st.shadow(at.q_proj.weight), bias=at.q_proj.bias, out=Qp)
-        KV = save.get("KV", (B * S, 2 * dout), bf)
+        KV = keep.get("KV", (B * S, 2 * dout), bf)
         ops.gemm(xk, st.shadow(self.kv_w), bias=self.kv_b, out=KV)
-        O = save.get("O", (B * nq, dout), bf)
+        O = keep.get("O", (B * nq, dout), bf)
         ops.attention_fwd_generic(Qp, KV[:, :dout], KV[:, dout:], O, B=B, Sq=nq, Skv=S, H=H, head_dim=hd, bsq=0,
                                   bsk=S * 2 * dout, bsv=S * 2 * dout, bso=nq * dout, scale=1.0 / math.sqrt(hd))
         Y = self.ws.get("Y", (B * nq, dout), bf)
         ops.gemm(O, st.shadow(at.output_proj.weight), bias=at.output_proj.bias, out=Y)
-        Y32 = save.get("Y32", (B * nq, dout), f32)
+        Y32 = save.get("Y32", (B * nq, dout), f32) if save is not None else None
         out = torch.empty((B * nq, dout), device=self.device, dtype=f32)
-        ops.add_layernorm_fwd(None, Y, Y32, None, out, m.ln_post.weight, m.ln_post.bias, save.get("mp", (B * nq,), f32),
-                              save.get("rp", (B * nq,), f32), B * nq, dout, m.ln_post.eps)
-        save.x32, save.B, save.S, save.din = x32, B, S, din
+        ops.add_layernorm_fwd(None, Y, Y32, None, out, m.ln_post.weight, m.ln_post.bias, keep.get("mp", (B * nq,), f32),
+                              keep.get("rp", (B * nq,), f32), B * nq, dout, m.ln_post.eps)
+        return out, x32
+
+    def forward(self, data, diff):
+        (x,) = diff
+        hd = self._dims()[3]
+        if hd not in (64, 96, 128):
+            raise MMBError(f"unsupported pooler head_dim {hd}")
+        save = Workspace(self.device)
+        out, save.x32 = self._forward(x, save)
+        save.B, save.S, save.din = x.shape
         return (out,), save
+
+    def infer(self, x: torch.Tensor) -> torch.Tensor:
+        """x fp32 [B, S, d_in] -> fp32 [B, n_queries, d_out]."""
+        nq, dout = self.mod.query.shape
+        return self._forward(x, None)[0].view(x.shape[0], nq, dout)
 
     def backward(self, save, dOUT):
         m, st = self.mod, self.store
@@ -282,21 +311,17 @@ class PoolerTrainRuntime:
 
 
 class TextDecoderTrainRuntime:
-    """CoCaTextDecoder with embed_cls=True (models/coca/text_decoder.py:66-203).
-    Outputs: pooled [B, out_dim] (projected ln_final(CLS row)) and XF [B*S, d] (tokens = XF[:, :-1])."""
+    """CoCaTextDecoder (models/coca/text_decoder.py:66-203).  Training (embed_cls=True, bias-free text_projection)
+    outputs: pooled [B, out_dim] (projected ln_final(CLS row)) and XF [B*S, d] (tokens = XF[:, :-1])."""
 
     def __init__(self, mod: nn.Module):
-        if not mod.embed_cls:
-            raise NotImplementedError("training CoCaTextDecoder(embed_cls=False) is not on the accelerated path")
-        if mod.text_projection is None or mod.text_projection.bias is not None:
-            raise NotImplementedError("training expects the bias-free text_projection of the reference builder")
         self.mod = mod
-        self.s = _Stack(mod, mod.transformer_decoder.layer, "ctxt", causal=True)
+        self.s = _Stack(mod, mod.transformer_decoder.layer, "ctxt", fp32_only=list(mod.embeddings.parameters()))
         self.store = self.s.store
         self._idx = None
 
-    def forward(self, data, diff):
-        input_ids, mask_u8, S = data
+    def _forward(self, input_ids, mask_u8, S: int, save: Optional[Workspace]):
+        """-> (pooled fp32 [B, out_dim], tokens fp32 [B, S-1 | S, d], XF fp32 [B*S, d], ids, CLS row index)."""
         m, s, st = self.mod, self.s, self.store
         d = s.d
         emb = m.embeddings
@@ -304,27 +329,60 @@ class TextDecoderTrainRuntime:
         B = ids.shape[0]
         bf, f32 = torch.bfloat16, torch.float32
         st.refresh()
-        save = Workspace(s.device)
-        X0 = torch.empty((B * S, d), device=s.device, dtype=f32)
+        keep = save if save is not None else s.ws
+        X0 = torch.empty((B * S, d), device=s.device, dtype=f32) if save is not None else s.ws.get("ctxt.X0", (B * S, d), f32)
         ops.coca_text_embed_fwd(ids, emb.token_embeddings.weight, emb.cls_embedding, emb.position_embeddings, X0, B, S, d,
                                 emb.token_embeddings.weight.shape[0])
-        s.stack.causal = mask_u8 is None      # a [B, S, S] mask already contains the causal structure
-        XM, Y = s.stack.forward(X0, B, S, True, save=save, mask3=mask_u8)
-        XF, _ = s.finish(XM, Y, B * S, None, save)
-        if self._idx is None or self._idx.numel() != B:
-            self._idx = torch.full((B,), S - 1, dtype=torch.int32, device=s.device)
+        # a [B, S, S] mask already contains the causal structure
+        XM, Y = s.stack.forward(X0, B, S, save, causal=mask_u8 is None, mask3=mask_u8)
         ln = getattr(m, "ln_final", None)
-        POOLb = save.get("ctxt.POOLb", (B, d), bf)
-        if ln is not None:    # LayerNorm of the CLS row only (:186-189): gathered rows
-            ops.add_layernorm_fwd(XF, None, save.get("ctxt.XSEL", (B, d), f32), POOLb, None, ln.weight, ln.bias,
-                                  save.get("ctxt.mL", (B,), f32), save.get("ctxt.rL", (B,), f32), B, d, ln.eps,
-                                  row_idx=self._idx, rows_per_group=S)
+        POOLb = keep.get("ctxt.POOLb", (B, d), bf)
+        idx = None
+        if m.embed_cls:
+            XF, _ = s.finish(XM, Y, B, S, None, save, None)
+            if self._idx is None or self._idx.numel() != B:
+                self._idx = torch.full((B,), S - 1, dtype=torch.int32, device=s.device)
+            idx = self._idx
+            if ln is not None:    # LayerNorm of the CLS row only (:186-189): gathered rows
+                ops.add_layernorm_fwd(XF, None, save.get("ctxt.XSEL", (B, d), f32) if save is not None else None, POOLb,
+                                      None, ln.weight, ln.bias, keep.get("ctxt.mL", (B,), f32),
+                                      keep.get("ctxt.rL", (B,), f32), B, d, ln.eps, row_idx=idx, rows_per_group=S)
+            else:
+                ops.gather_rows_cast(XF, POOLb, B, S, S - 1, d)
+            tokens = XF.view(B, S, d)[:, :-1]
+        else:   # inference only
+            if ln is None:
+                raise MMBError("CoCaTextDecoder(embed_cls=False) requires final_layer_norm_eps (reference asserts too)")
+            XF, LAST = s.finish(XM, Y, B, S, ln, save, None)
+            am = torch.empty(B, dtype=torch.int32, device=s.device)
+            ops.argmax_tokens(ids, am, B, S)
+            rows = LAST.view(B, S, d)[torch.arange(B, device=s.device), am.long()]   # [B, d] gather: plumbing
+            ops.cast_bf16(rows.contiguous().view(-1), POOLb.view(-1))
+            tokens = LAST.view(B, S, d)
+        if m.text_projection is not None:
+            pooled = torch.empty((B, m.text_projection.weight.shape[0]), device=s.device, dtype=f32)
+            ops.gemm(POOLb, st.shadow(m.text_projection.weight), bias=m.text_projection.bias, epilogue=ops.EPI_F32,
+                     out=pooled)
         else:
-            ops.gather_rows_cast(XF, POOLb, B, S, S - 1, d)
-        pooled = torch.empty((B, m.text_projection.weight.shape[0]), device=s.device, dtype=f32)
-        ops.gemm(POOLb, st.shadow(m.text_projection.weight), epilogue=ops.EPI_F32, out=pooled)
-        save.B, save.S, save.ids, save.causal = B, S, ids, mask_u8 is None
+            pooled = POOLb.float()
+        return pooled, tokens, XF, ids, idx
+
+    def forward(self, data, diff):
+        m = self.mod
+        if not m.embed_cls:
+            raise NotImplementedError("training CoCaTextDecoder(embed_cls=False) is not on the accelerated path")
+        if m.text_projection is None or m.text_projection.bias is not None:
+            raise NotImplementedError("training expects the bias-free text_projection of the reference builder")
+        input_ids, mask_u8, S = data
+        save = Workspace(self.s.device)
+        pooled, _, XF, save.ids, save.idx = self._forward(input_ids, mask_u8, S, save)
+        save.B, save.S = input_ids.shape[0], S
         return (pooled, XF), save
+
+    def infer(self, input_ids: torch.Tensor, mask_u8: Optional[torch.Tensor], S: int):
+        """input_ids int64 [B, S-1 (embed_cls) | S]; mask_u8 [B, S, S] or None (plain causal).
+        Returns (pooled fp32 [B, out_dim], tokens fp32 [B, S-1 | S, d])."""
+        return self._forward(input_ids, mask_u8, S, None)[:2]
 
     def backward(self, save, dpooled, dXF):
         m, s, st = self.mod, self.s, self.store
@@ -344,11 +402,10 @@ class TextDecoderTrainRuntime:
             if ln is not None:
                 ops.layernorm_bwd(save.get("ctxt.XSEL", (B, d), f32), None, dL, save.get("ctxt.mL", (B,), f32),
                                   save.get("ctxt.rL", (B,), f32), ln.weight, G, G, None, st.grad(ln.weight),
-                                  st.grad(ln.bias), B, d, row_idx=self._idx, rows_per_group=S)
+                                  st.grad(ln.bias), B, d, row_idx=save.idx, rows_per_group=S)
             else:
                 ops.scatter_rows_add(dL, G, B, S, S - 1, d)
             ops.cast_bf16(G, Gb)
-        s.stack.causal = save.causal
         G = s.stack.backward(G, Gb, B, S, top_bias_done=False, save=save)
         ops.batch_sum(G, st.grad(emb.position_embeddings), B, S * d, S * d)
         ops.batch_sum(G.view(-1)[(S - 1) * d:], st.grad(emb.cls_embedding), B, S * d, d)
@@ -361,30 +418,62 @@ class TextDecoderTrainRuntime:
 
 
 class MultimodalDecoderTrainRuntime:
-    """CoCaMultimodalDecoder up to its final LayerNorm (models/coca/multimodal_decoder.py:86-108); the vocabulary
-    projection + cross-entropy is ``LinearCrossEntropyFunction``.  Inputs: texts [B, S, d], images [B, Si, d_kv]."""
+    """CoCaMultimodalDecoder (models/coca/multimodal_decoder.py:15-108).  Training runs up to the final LayerNorm (the
+    vocabulary projection + cross-entropy is ``LinearCrossEntropyFunction``).  Inputs: texts [B, S, d], images
+    [B, Si, d_kv]."""
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.s = _Stack(mod, mod.transformer_decoder.layer, "cmm", causal=True)
+        self.s = _Stack(mod, mod.transformer_decoder.layer, "cmm")
         self.store = self.s.store
 
-    def forward(self, data, diff):
-        texts, images = diff
-        s, st = self.s, self.store
+    def _forward(self, texts, images, save: Optional[Workspace], want_bf16: bool = False):
+        """-> (XF, LAST or None, LASTb: bf16 copy of LAST when want_bf16 and a final LayerNorm exists, else None)."""
+        s = self.s
         d = s.d
         B, S, _ = texts.shape
         _, Si, dv = images.shape
-        st.refresh()
-        save = Workspace(s.device)
-        X0 = torch.empty((B * S, d), device=s.device, dtype=torch.float32)
-        X0.view(B, S, d).copy_(texts)
-        enc = save.get("cmm.ENC", (B * Si, dv), torch.bfloat16)
+        self.store.refresh()
+        X0 = torch.empty((B * S, d), device=s.device, dtype=torch.float32) if save is not None else s.ws.get(
+            "cmm.X0", (B * S, d), torch.float32)
+        X0.view(B, S, d).copy_(texts)                 # [B, S, d] slice of the text decoder's stream -> contiguous rows
+        enc = (save if save is not None else s.ws).get("cmm.ENC", (B * Si, dv), torch.bfloat16)
         ops.cast_bf16(images.contiguous().float().view(-1), enc.view(-1))
-        XM, Y = s.stack.forward(X0, B, S, True, save=save, enc=enc, S_enc=Si)
-        XF, LAST = s.finish(XM, Y, B * S, self.mod.transformer_decoder.final_layer_norm, save)
-        save.B, save.S, save.Si, save.dv = B, S, Si, dv
+        XM, Y = s.stack.forward(X0, B, S, save, causal=True, enc=enc, S_enc=Si)
+        fln = self.mod.transformer_decoder.final_layer_norm
+        LASTb = s.ws.get("cmm.LASTb", (B * S, d), torch.bfloat16) if (fln is not None and want_bf16) else None
+        XF, LAST = s.finish(XM, Y, B, S, fln, save, None, LASTb=LASTb)
+        return XF, LAST, LASTb
+
+    def forward(self, data, diff):
+        texts, images = diff
+        save = Workspace(self.s.device)
+        XF, LAST, _ = self._forward(texts, images, save)
+        save.B, save.S, _ = texts.shape
+        _, save.Si, save.dv = images.shape
         return ((LAST if LAST is not None else XF),), save
+
+    def infer(self, texts: torch.Tensor, images: torch.Tensor, return_hidden: bool = False):
+        """return_hidden: skip the vocabulary projection and return (hidden bf16 [B*S, d], bf16 weight [V, d]) — the
+        operands of the fused Linear -> CrossEntropy kernel (CoCaForPretraining never needs the [B, S, V] logits)."""
+        m, s = self.mod, self.s
+        B, S, _ = texts.shape
+        d = s.d
+        XF, LAST, LASTb = self._forward(texts, images, None, want_bf16=m.output_projection is not None)
+        if m.output_projection is None:
+            if return_hidden:
+                raise MMBError("return_hidden needs an output projection (the vocabulary head)")
+            return (LAST if LAST is not None else XF).view(B, S, d)
+        if LASTb is None:
+            LASTb = s.ws.get("cmm.LASTb", (B * S, d), torch.bfloat16)
+            ops.cast_bf16(XF.view(-1), LASTb.view(-1))
+        W = self.store.shadow(m.output_projection.weight)
+        if return_hidden:
+            return LASTb, W
+        V = m.output_projection.weight.shape[0]
+        out = torch.empty((B * S, V), device=s.device, dtype=torch.float32)
+        ops.gemm(LASTb, W, bias=m.output_projection.bias, epilogue=ops.EPI_F32, out=out)
+        return out.view(B, S, V)
 
     def backward(self, save, dOUT):
         s = self.s
@@ -519,7 +608,7 @@ class LayersTrainRuntime:
     on its own under autograd: hidden_states [B, S, d] in (differentiable), residual stream (and final LayerNorm) out."""
 
     def __init__(self, owner: nn.Module, layers, final_ln: Optional[nn.Module]):
-        self.s = _Stack(owner, layers, "lyr", causal=False)
+        self.s = _Stack(owner, layers, "lyr")
         self.store = self.s.store
         self.final_ln = final_ln
 
@@ -532,12 +621,12 @@ class LayersTrainRuntime:
         save = Workspace(s.device)
         X0 = torch.empty((B * S, d), device=s.device, dtype=torch.float32)
         X0.view(B, S, d).copy_(x)
-        XM, Y = s.stack.forward(X0, B, S, True, save=save, mask3=mask_u8,
-                                scales=drop_path_scales(s.layers, B, s.device))
-        XF, LAST = s.finish(XM, Y, B * S, self.final_ln, save)
+        scales = drop_path_scales(s.layers, B, s.device)
+        hidden: List[torch.Tensor] = []
+        XM, Y = s.stack.forward(X0, B, S, save, mask3=mask_u8, scales=scales, hidden=hidden)
+        XF, LAST = s.finish(XM, Y, B, S, self.final_ln, save, scales)
         save.B, save.S = B, S
-        self.last_hidden = ([X0.view(B, S, d)] + [save.bufs[f"lyr.XA.{l}"].view(B, S, d) for l in range(1, s.L)]
-                            + [XF.view(B, S, d)])
+        self.last_hidden = hidden + [XF.view(B, S, d)]
         return ((LAST if LAST is not None else XF),), save
 
     def backward(self, save, dOUT):

@@ -1,6 +1,9 @@
-"""Training runtime of the FLAVA encoders (BASELINE.json config 3 as a training step): forward that keeps what the
-backward needs + the explicit backward schedule, behind torch.autograd Functions so that the drop-in modules train
-with ``loss.backward()`` exactly like the reference's (models/flava/model.py:127-298 under autograd).
+"""Runtime of the FLAVA encoders (BASELINE.json config 3, forward and training step), one per encoder for both grad
+modes: forward that keeps what the backward needs + the explicit backward schedule, behind torch.autograd Functions so
+that the drop-in modules train with ``loss.backward()`` exactly like the reference's (models/flava/model.py:127-298
+under autograd); under torch.no_grad() the same forward keeps nothing and returns the reference's ``TransformerOutput``
+(every tensor allocated per call; ``attentions`` on request, recomputed from the packed QKV and the row LSE by one
+extra kernel per layer: DESIGN.md §10).
 
 The layer stack is the CLIP towers' ``engine.TransformerStack`` (same kernels, same fused schedule): the separate
 query / key / value Linears are presented to it as one packed in-projection (``ParamStore.pack``), the MLP activation
@@ -25,27 +28,29 @@ reference's, but they carry no autograd history (nothing in the library differen
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Optional, Sequence
 
 import torch
 from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run
+from .engine import (ParamStore, TransformerStack, Workspace, _Shadows, act_code, patch_embed_bwd, patch_embed_fwd,
+                     require_head_dim_64, run)
 from .modules.layers.transformer import TransformerOutput
 
 
 class FlavaTrainStack:
-    """ParamStore (packed q/k/v order) + TransformerStack + final LayerNorm of one FLAVA encoder."""
+    """ParamStore (packed q/k/v order) + TransformerStack + final LayerNorm (+ pooler) of one FLAVA encoder."""
 
-    def __init__(self, owner: nn.Module, encoder: nn.Module, layernorm: nn.Module, prefix: str,
-                 extra: Sequence[nn.Module] = ()):
+    def __init__(self, owner: nn.Module, encoder: nn.Module, layernorm: nn.Module, pooler: Optional[nn.Module],
+                 prefix: str, extra: Sequence[nn.Module] = (), fp32_only: Sequence[nn.Parameter] = ()):
         layers = list(encoder.layer)
         l0 = layers[0]
         if not l0.norm_first:
             raise MMBError("only pre-norm (norm_first=True) FLAVA layers are on the accelerated path")
         d, H = l0.attention.dim_q, l0.attention.n_head
+        require_head_dim_64(d, H)
         ff = l0.feedforward.model[0].weight.shape[0]
         params: List[nn.Parameter] = []
         for layer in layers:   # q / k / v weights, then biases, consecutive -> packable
@@ -57,7 +62,7 @@ class FlavaTrainStack:
                 if id(p) not in seen:
                     seen.add(id(p))
                     params.append(p)
-        self.store = ParamStore(params)
+        self.store = ParamStore(params, fp32_only)
         self.device = self.store.device
         st = self.store
         adapters = []
@@ -69,28 +74,59 @@ class FlavaTrainStack:
             adapters.append(SimpleNamespace(self_attn=attn, norm1=layer.attention_layernorm,
                                             norm2=layer.feedforward_layernorm, linear1=mlp[0], linear2=mlp[-1]))
         self.ws = Workspace(self.device)   # scratch shared by all calls (stream-ordered)
-        self.stack = TransformerStack(adapters, st, self.ws, d=d, heads=H, ff=ff, causal=False,
+        self.stack = TransformerStack(adapters, st, self.ws, d=d, heads=H, ff=ff,
                                       act=act_code(l0.feedforward.model[1]), prefix=prefix)
-        self.layernorm, self.prefix = layernorm, prefix
+        self.sh = _Shadows(self.device)    # FLAVAModel's projections of the first token (project_first_token)
+        self.layernorm, self.pooler, self.prefix = layernorm, pooler, prefix
         self.d, self.H, self.L = d, H, len(layers)
 
     def forward(self, X0: torch.Tensor, B: int, S: int, kmask: Optional[torch.Tensor], save: Workspace):
         """Returns ((LAST, XF), save): fp32 [B*S, d] each; LAST = layernorm(XF), XF = hidden_states[-1].  The list of
         hidden_states goes to `last_hidden`."""
+        LAST, XF, self.last_hidden = self._run(X0, B, S, kmask, save)
+        save.XF, save.B, save.S = XF, B, S
+        return (LAST, XF), save
+
+    def _run(self, X0, B, S, kmask, save: Optional[Workspace], attns=None):
         d, ln, pfx = self.d, self.layernorm, self.prefix
         M = B * S
         f32 = torch.float32
-        XM, Y = self.stack.forward(X0, B, S, True, kmask=kmask, save=save)
-        XF = torch.empty((M, d), device=self.device, dtype=f32)
-        LAST = torch.empty((M, d), device=self.device, dtype=f32)
-        ops.add_layernorm_fwd(XM, Y, XF, None, LAST, ln.weight, ln.bias, save.get(f"{pfx}.mF", (M,), f32),
-                              save.get(f"{pfx}.rF", (M,), f32), M, d, ln.eps)
-        save.XF, save.B, save.S = XF, B, S
-        hidden = [X0.view(B, S, d)]
-        hidden += [save.bufs[f"{pfx}.XA.{l}"].view(B, S, d) for l in range(1, self.L)]
+        stats = save if save is not None else self.ws
+        hidden: List[torch.Tensor] = []
+        XM, Y = self.stack.forward(X0, B, S, save, kmask=kmask, hidden=hidden, attns=attns)
+        XF = torch.empty((M, d), device=self.device, dtype=f32)      # hidden_states[-1] (pre-LayerNorm)
+        LAST = torch.empty((M, d), device=self.device, dtype=f32)    # layernorm(XF) == last_hidden_state
+        ops.add_layernorm_fwd(XM, Y, XF, None, LAST, ln.weight, ln.bias, stats.get(f"{pfx}.mF", (M,), f32),
+                              stats.get(f"{pfx}.rF", (M,), f32), M, d, ln.eps)
         hidden.append(XF.view(B, S, d))
-        self.last_hidden = hidden
-        return (LAST, XF), save
+        return LAST, XF, hidden
+
+    def infer(self, X0: torch.Tensor, B: int, S: int, kmask: Optional[torch.Tensor] = None,
+              want_attn: bool = False) -> TransformerOutput:
+        """want_attn: also return every layer's attention probabilities fp32 [B, H, S, S] (`attentions`), recomputed
+        from the packed QKV and the row LSE of the fused attention kernel (mmb_attention_probs)."""
+        d, st = self.d, self.store
+        attns: Optional[List[torch.Tensor]] = [] if want_attn else None
+        LAST, _, hidden = self._run(X0, B, S, kmask, None, attns)
+        pooled = None
+        if self.pooler is not None:
+            CLSb = self.ws.get(f"{self.prefix}.CLSb", (B, d), torch.bfloat16)
+            ops.gather_rows_cast(LAST, CLSb, B, S, 0, d)
+            pooled = torch.empty((B, d), device=self.device, dtype=torch.float32)
+            ops.gemm(CLSb, st.shadow(self.pooler.dense.weight), bias=self.pooler.dense.bias, epilogue=ops.EPI_F32,
+                     out=pooled)
+            ops.tanh_(pooled)
+        return TransformerOutput(last_hidden_state=LAST.view(B, S, d), pooler_output=pooled, hidden_states=hidden,
+                                 attentions=attns)
+
+    def project_first_token(self, last_hidden_state: torch.Tensor, linear: nn.Linear, key: str) -> torch.Tensor:
+        """linear(last_hidden_state[:, 0, :]) (models/flava/model.py:244-246, 261-263)."""
+        B, S, d = last_hidden_state.shape
+        CLSb = self.ws.get(f"{self.prefix}.CLSb2", (B, d), torch.bfloat16)
+        ops.gather_rows_cast(last_hidden_state.reshape(B * S, d), CLSb, B, S, 0, d)
+        out = torch.empty((B, linear.weight.shape[0]), device=self.device, dtype=torch.float32)
+        ops.gemm(CLSb, self.sh.get(key, [linear.weight]), bias=linear.bias, epilogue=ops.EPI_F32, out=out)
+        return out
 
     def backward(self, save: Workspace, dLAST: Optional[torch.Tensor], dXF: Optional[torch.Tensor]) -> torch.Tensor:
         """Gradient w.r.t. X0 (fp32 [B*S, d], scratch: consume before the next backward of this encoder); parameter
@@ -116,25 +152,31 @@ def _f32c(t: Optional[torch.Tensor], shape) -> Optional[torch.Tensor]:
     return t.contiguous().float().view(shape)
 
 
+# One runtime per encoder: `forward(data, diff)` / `backward` under autograd (engine.run), `infer(...)` under
+# torch.no_grad(): the same front end and stack without a save Workspace, then the pooler.
 class FlavaImageTrainRuntime:
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.ts = FlavaTrainStack(mod, mod.encoder, mod.layernorm, "fimg")
+        self.ts = FlavaTrainStack(mod, mod.encoder, mod.layernorm, mod.pooler, "fimg")
         self.store = self.ts.store
 
-    def diff_inputs(self, data) -> Tuple[torch.Tensor, ...]:
-        return ()
-
-    def forward(self, data, diff):
-        pixel_values, image_patches_mask = data
+    def _embed(self, pixel_values, image_patches_mask, save: Optional[Workspace]):
         emb, ts, st = self.mod.embeddings, self.ts, self.store
         conv = emb.patch_embeddings.projection
         st.refresh()
-        save = Workspace(ts.device)
-        X0, B, S, P, pm = patch_embed_fwd(pixel_values, conv, st.shadow2d(conv.weight), emb.cls_token,
-                                          emb.position_embeddings, emb.mask_token, image_patches_mask, ts.ws, save, "fimg")
-        save.pm, save.P = pm, P
-        return ts.forward(X0, B, S, None, save)
+        return patch_embed_fwd(pixel_values, conv, st.shadow2d(conv.weight), emb.cls_token, emb.position_embeddings,
+                               emb.mask_token, image_patches_mask, ts.ws, save if save is not None else ts.ws, "fimg")
+
+    def forward(self, data, diff):
+        pixel_values, image_patches_mask = data
+        save = Workspace(self.ts.device)
+        X0, B, S, save.P, save.pm = self._embed(pixel_values, image_patches_mask, save)
+        return self.ts.forward(X0, B, S, None, save)
+
+    def infer(self, pixel_values: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None,
+              want_attn: bool = False) -> TransformerOutput:
+        X0, B, S, _, _ = self._embed(pixel_values, image_patches_mask, None)   # X0 is returned as hidden_states[0]
+        return self.ts.infer(X0, B, S, want_attn=want_attn)
 
     def backward(self, save, dLAST, dXF):
         emb, ts = self.mod.embeddings, self.ts
@@ -147,14 +189,11 @@ class FlavaImageTrainRuntime:
 class FlavaTextTrainRuntime:
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.ts = FlavaTrainStack(mod, mod.encoder, mod.layernorm, "ftxt")
+        self.ts = FlavaTrainStack(mod, mod.encoder, mod.layernorm, mod.pooler, "ftxt",
+                                  fp32_only=list(mod.embeddings.parameters()))
         self.store = self.ts.store
 
-    def diff_inputs(self, data):
-        return ()
-
-    def forward(self, data, diff):
-        input_ids, attention_mask, token_type_ids = data
+    def _embed(self, input_ids, attention_mask, token_type_ids, save: Optional[Workspace]):
         emb, ts, st = self.mod.embeddings, self.ts, self.store
         d = ts.d
         ids = input_ids.long().contiguous()
@@ -162,20 +201,28 @@ class FlavaTextTrainRuntime:
         if S > emb.position_embeddings.weight.shape[0]:
             raise ValueError(f"sequence length {S} exceeds max_position_embeddings")
         st.refresh()
-        save = Workspace(ts.device)
-        X0 = torch.empty((B * S, d), device=ids.device, dtype=torch.float32)
-        KM = save.get("ftxt.KM", (B * S,), torch.uint8)
+        X0 = torch.empty((B * S, d), device=ids.device, dtype=torch.float32)   # hidden_states[0]
+        KM = (save if save is not None else ts.ws).get("ftxt.KM", (B * S,), torch.uint8)
         tt = token_type_ids.long().contiguous() if token_type_ids is not None else None
         V = emb.word_embeddings.weight.shape[0]
         ops.bert_embed_ln_fwd(ids, tt, emb.word_embeddings.weight, emb.position_embeddings.weight,
                               emb.token_type_embeddings.weight, emb.layer_norm.weight, emb.layer_norm.bias, X0, KM,
                               emb.pad_token_id, B, S, d, V, emb.layer_norm.eps)
-        if attention_mask is not None:
+        if attention_mask is not None:  # user-supplied [B,S] mask (1 = attend) overrides the pad-derived one
             if attention_mask.dim() != 2:
                 raise NotImplementedError("only [batch, seq_len] padding masks are supported on the accelerated path")
             KM = (attention_mask != 0).to(torch.uint8).contiguous().view(-1)
-        save.ids, save.tt, save.V = ids, tt, V
-        return ts.forward(X0, B, S, KM, save)
+        return X0, B, S, KM, ids, tt, V
+
+    def forward(self, data, diff):
+        save = Workspace(self.ts.device)
+        X0, B, S, KM, save.ids, save.tt, save.V = self._embed(*data, save)
+        return self.ts.forward(X0, B, S, KM, save)
+
+    def infer(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
+              token_type_ids: Optional[torch.Tensor] = None, want_attn: bool = False) -> TransformerOutput:
+        X0, B, S, KM, _, _, _ = self._embed(input_ids, attention_mask, token_type_ids, None)
+        return self.ts.infer(X0, B, S, kmask=KM, want_attn=want_attn)
 
     def backward(self, save, dLAST, dXF):
         emb, ts, st = self.mod.embeddings, self.ts, self.store
@@ -197,47 +244,59 @@ class FlavaMMTrainRuntime:
     FLAVAModel, not to the multimodal encoder; they live in this runtime's ParamStore (image_proj / text_proj None:
     the module was called directly with an already fused token sequence)."""
 
-    def __init__(self, mod: nn.Module, image_proj: Optional[nn.Linear], text_proj: Optional[nn.Linear]):
+    def __init__(self, mod: nn.Module, image_proj: Optional[nn.Linear] = None, text_proj: Optional[nn.Linear] = None):
         self.mod, self.image_proj, self.text_proj = mod, image_proj, text_proj
         extra = [m for m in (image_proj, text_proj) if m is not None]
-        self.ts = FlavaTrainStack(mod, mod.encoder, mod.layernorm, "fmm", extra=extra)
+        self.ts = FlavaTrainStack(mod, mod.encoder, mod.layernorm, mod.pooler, "fmm", extra=extra)
         self.store = self.ts.store
 
-    def forward(self, data, diff):
+    def _embed(self, diff, save: Optional[Workspace]):
+        """-> (X0, B, S, Si, St, di, dt): Si = the fused sequence length and St = 0 for a direct call."""
         ts, st = self.ts, self.store
         d = ts.d
         bf, f32 = torch.bfloat16, torch.float32
         cls = self.mod.cls_token
         off = 1 if cls is not None else 0
         st.refresh()
-        save = Workspace(ts.device)
         if self.image_proj is None:   # direct call: hidden_states [B, S, d] already fused
             (hs,) = diff
-            B, Sa, dd = hs.shape
+            B, Sa, _ = hs.shape
             hs = hs.contiguous().float()
-            S = Sa + off
-            X0 = torch.empty((B * S, d), device=hs.device, dtype=f32)
-            ops.concat_tokens(cls, hs, hs, X0, B, Sa, 0, d)
-            save.Si, save.St = Sa, 0
-        else:
-            image_hidden, text_hidden = diff
-            B, Si, di = image_hidden.shape
-            Bt, St, dt = text_hidden.shape
-            if B != Bt:
-                raise ValueError(f"batch mismatch between image ({B}) and text ({Bt}) hidden states")
-            Ib = save.get("fmm.Ib", (B * Si, di), bf)
-            Tb = save.get("fmm.Tb", (B * St, dt), bf)
-            ops.cast_bf16(image_hidden.contiguous().float().view(-1), Ib.view(-1))
-            ops.cast_bf16(text_hidden.contiguous().float().view(-1), Tb.view(-1))
-            Pi = ts.ws.get("fmm.Pi", (B * Si, d), f32)
-            Pt = ts.ws.get("fmm.Pt", (B * St, d), f32)
-            ops.gemm(Ib, st.shadow(self.image_proj.weight), bias=self.image_proj.bias, epilogue=ops.EPI_F32, out=Pi)
-            ops.gemm(Tb, st.shadow(self.text_proj.weight), bias=self.text_proj.bias, epilogue=ops.EPI_F32, out=Pt)
-            S = Si + St + off
-            X0 = torch.empty((B * S, d), device=image_hidden.device, dtype=f32)
-            ops.concat_tokens(cls, Pi, Pt, X0, B, Si, St, d)
-            save.Si, save.St, save.di, save.dt = Si, St, di, dt
-        return ts.forward(X0, B, S, None, save)
+            if cls is None and save is None:
+                return hs.view(B * Sa, d), B, Sa, Sa, 0, None, None   # hidden_states[0] is the input itself
+            X0 = torch.empty((B * (Sa + off), d), device=hs.device, dtype=f32)
+            ops.concat_tokens(cls, hs, hs, X0, B, Sa, 0, d)   # cat(cls, hidden) == concat_tokens(cls, hidden, <empty>)
+            return X0, B, Sa + off, Sa, 0, None, None
+        image_hidden, text_hidden = diff
+        B, Si, di = image_hidden.shape
+        Bt, St, dt = text_hidden.shape
+        if B != Bt:
+            raise ValueError(f"batch mismatch between image ({B}) and text ({Bt}) hidden states")
+        keep = save if save is not None else ts.ws
+        Ib = keep.get("fmm.Ib", (B * Si, di), bf)
+        Tb = keep.get("fmm.Tb", (B * St, dt), bf)
+        ops.cast_bf16(image_hidden.contiguous().float().view(-1), Ib.view(-1))
+        ops.cast_bf16(text_hidden.contiguous().float().view(-1), Tb.view(-1))
+        Pi = ts.ws.get("fmm.Pi", (B * Si, d), f32)
+        Pt = ts.ws.get("fmm.Pt", (B * St, d), f32)
+        ops.gemm(Ib, st.shadow(self.image_proj.weight), bias=self.image_proj.bias, epilogue=ops.EPI_F32, out=Pi)
+        ops.gemm(Tb, st.shadow(self.text_proj.weight), bias=self.text_proj.bias, epilogue=ops.EPI_F32, out=Pt)
+        S = Si + St + off
+        X0 = torch.empty((B * S, d), device=image_hidden.device, dtype=f32)   # hidden_states[0]
+        ops.concat_tokens(cls, Pi, Pt, X0, B, Si, St, d)
+        return X0, B, S, Si, St, di, dt
+
+    def forward(self, data, diff):
+        save = Workspace(self.ts.device)
+        X0, B, S, save.Si, save.St, save.di, save.dt = self._embed(diff, save)
+        return self.ts.forward(X0, B, S, None, save)
+
+    def infer(self, *hidden: torch.Tensor, want_attn: bool = False) -> TransformerOutput:
+        """hidden: the fused token sequence fp32 [B, S, d] (direct call), or the image and text encoders' hidden
+        states (FLAVAModel.encode_mm, models/flava/model.py:283-298: projected by two GEMMs, then [cls | image | text]
+        assembled by one kernel)."""
+        X0, B, S, _, _, _, _ = self._embed(hidden, None)
+        return self.ts.infer(X0, B, S, want_attn=want_attn)
 
     def backward(self, save, dLAST, dXF):
         ts, st = self.ts, self.store

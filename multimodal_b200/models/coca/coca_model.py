@@ -1,7 +1,7 @@
 """CoCa — drop-in for torchmultimodal/models/coca/coca_model.py:27-460 (`MultimodalOutput`, `CoCaModel`, `coca_vit`,
 `coca_vit_b_32`, `coca_vit_l_14`, `CoCaForPretraining`, `coca_for_pretraining`): same builders / kwargs / state-dict
 schema / init order.  Forward only (BASELINE.json config 5 is a parity case in this round): every submodule runs on
-the fused kernel stack (engine_coca.py); `CoCaForPretraining` returns the contrastive loss from the fused
+the fused kernel stack (engine_coca_train.py); `CoCaForPretraining` returns the contrastive loss from the fused
 `ContrastiveLossWithTemperature` and the captioning cross-entropy from `mmb_ce_labels`."""
 import math
 from typing import Any, Callable, Dict, List, NamedTuple, Optional, Tuple, Union
@@ -91,8 +91,8 @@ class CoCaModel(nn.Module):
                 self.multimodal_decoder.hidden_states(text_tokens, captioning_image_embeddings),
                 self.multimodal_decoder.output_projection)
         else:
-            multimodal_embeddings = self.multimodal_decoder._runtime().forward(text_tokens, captioning_image_embeddings,
-                                                                               return_hidden=True)
+            multimodal_embeddings = self.multimodal_decoder._runtime().infer(text_tokens, captioning_image_embeddings,
+                                                                             return_hidden=True)
         return MultimodalOutput(contrastive_image_embeddings, contrastive_text_embeddings, multimodal_embeddings)
 
     def _vision_proj(self, x: Tensor) -> Tensor:

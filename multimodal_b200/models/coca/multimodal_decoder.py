@@ -1,5 +1,5 @@
 """CoCa multimodal decoder — drop-in for torchmultimodal/models/coca/multimodal_decoder.py:15-108.  Forward =
-`engine_coca.MultimodalDecoderRuntime`: causal self-attention on the tensor-core attention kernel, cross-attention to the captioning
+`engine_coca_train.MultimodalDecoderTrainRuntime`: causal self-attention on the tensor-core attention kernel, cross-attention to the captioning
 image tokens on the general kernel, final LayerNorm + vocabulary projection GEMM (fp32 logits)."""
 from typing import Callable, Optional
 
@@ -38,7 +38,7 @@ class CoCaMultimodalDecoder(_RuntimeOwner):
                 hidden = T.linear_f32(hidden, self.output_projection)
             return hidden
         with torch.no_grad():
-            return self._runtime().forward(texts, images)
+            return self._runtime().infer(texts, images)
 
     def wants_graph(self, texts: Tensor, images: Tensor) -> bool:
         from ...engine import wants_grad
@@ -48,19 +48,13 @@ class CoCaMultimodalDecoder(_RuntimeOwner):
         """Training path: the decoder output after its final LayerNorm, [B, S, d] with autograd history (the vocabulary
         projection is applied by the caller: `forward`, or fused with the cross-entropy in CoCaForPretraining)."""
         from ...engine import run
-        (out,) = run(self._train_runtime(), None, (texts, images))
+        (out,) = run(self._runtime(), None, (texts, images))
         return out.view(texts.shape[0], texts.shape[1], -1)
 
 
 def _mm_runtime(mod):
-    from ...engine_coca import MultimodalDecoderRuntime
-    return MultimodalDecoderRuntime(mod)
-
-
-def _mm_train_runtime(mod):
     from ...engine_coca_train import MultimodalDecoderTrainRuntime
     return MultimodalDecoderTrainRuntime(mod)
 
 
 CoCaMultimodalDecoder._runtime_cls = staticmethod(_mm_runtime)
-CoCaMultimodalDecoder._train_runtime_cls = staticmethod(_mm_train_runtime)

@@ -1,6 +1,6 @@
 """CoCa text decoder — drop-in for torchmultimodal/models/coca/text_decoder.py:16-252 (`CoCaTextEmbeddings`,
 `CoCaTextDecoder`): same constructor, state-dict keys, initialisation and mask semantics.  Forward =
-`engine_coca.TextDecoderRuntime` (embedding gather + CLS append in one kernel, fused decoder stack, LayerNorm of the CLS
+`engine_coca_train.TextDecoderTrainRuntime` (embedding gather + CLS append in one kernel, fused decoder stack, LayerNorm of the CLS
 row only, projection GEMM)."""
 from typing import Any, Callable, Optional, Tuple
 
@@ -98,22 +98,16 @@ class CoCaTextDecoder(_RuntimeOwner):
             mask_u8 = (mask[:, 0] != 0).to(torch.uint8).contiguous()
         from ...engine import run, wants_grad
         if wants_grad(self):
-            pooled, XF = run(self._train_runtime(), (input_ids, mask_u8, S), ())
+            pooled, XF = run(self._runtime(), (input_ids, mask_u8, S), ())
             B = input_ids.shape[0]
             return pooled, XF.view(B, S, -1)[:, :-1]       # tokens: every row but the appended CLS one (:190-191)
         with torch.no_grad():
-            return self._runtime().forward(input_ids, mask_u8, S)
+            return self._runtime().infer(input_ids, mask_u8, S)
 
 
 def _txt_runtime(mod):
-    from ...engine_coca import TextDecoderRuntime
-    return TextDecoderRuntime(mod)
-
-
-def _txt_train_runtime(mod):
     from ...engine_coca_train import TextDecoderTrainRuntime
     return TextDecoderTrainRuntime(mod)
 
 
 CoCaTextDecoder._runtime_cls = staticmethod(_txt_runtime)
-CoCaTextDecoder._train_runtime_cls = staticmethod(_txt_train_runtime)

@@ -1,6 +1,6 @@
 """FLAVA image encoder — drop-in for torchmultimodal/models/flava/image_encoder.py:28-278 (`PatchEmbeddings`,
 `ImageEmbeddings`, `ImageTransformer`, `flava_image_encoder`).  Same constructors / state-dict keys / init; the forward
-is `engine_flava.FlavaImageRuntime` (im2col + wgmma GEMM patch embedding, fused token assembly, fused layer stack).
+is `engine_flava_train.FlavaImageTrainRuntime` (im2col + wgmma GEMM patch embedding, fused token assembly, fused layer stack).
 Position-embedding interpolation (image_encoder.py:103-137) is out of scope (fixed 224x224 pre-training resolution)."""
 import warnings
 from functools import partial
@@ -83,24 +83,18 @@ class ImageTransformer(_RuntimeOwner):
         if wants_grad(self):   # training: forward keeps activations, autograd nodes carry the explicit backward
             if getattr(self, "output_attentions", False):
                 raise NotImplementedError("attention probabilities are not produced by the training forward")
-            return T.encoder_output(self._train_runtime(), (pixel_values, image_patches_mask), (), self.pooler)
+            return T.encoder_output(self._runtime(), (pixel_values, image_patches_mask), (), self.pooler)
         with torch.no_grad():
-            return self._runtime().forward(pixel_values, image_patches_mask,
-                                           want_attn=bool(getattr(self, "output_attentions", False)))
+            return self._runtime().infer(pixel_values, image_patches_mask,
+                                         want_attn=bool(getattr(self, "output_attentions", False)))
 
 
 def _img_runtime(mod):
-    from ...engine_flava import FlavaImageRuntime
-    return FlavaImageRuntime(mod)
-
-
-def _img_train_runtime(mod):
     from ...engine_flava_train import FlavaImageTrainRuntime
     return FlavaImageTrainRuntime(mod)
 
 
 ImageTransformer._runtime_cls = staticmethod(_img_runtime)
-ImageTransformer._train_runtime_cls = staticmethod(_img_train_runtime)
 
 
 def flava_image_encoder(hidden_size: int = 768, num_attention_heads: int = 12, num_hidden_layers: int = 12,

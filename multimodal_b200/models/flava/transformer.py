@@ -3,7 +3,8 @@
 
 Same constructors, state-dict keys (``layer.{i}.attention.{query,key,value,output}``, ``feedforward.model.{0,2}``,
 ``attention_layernorm``, ``feedforward_layernorm``) and initialisation order.  The layers themselves never run as torch
-modules: the owning encoder hands the whole stack to ``engine_flava.FlavaStack`` (inference) or ``engine_flava_train`` (forward + backward under autograd; DESIGN.md §10).
+modules: the owning encoder hands the whole stack to its ``engine_flava_train`` runtime (forward + backward under
+autograd, or the forward alone under torch.no_grad(); DESIGN.md §10).
 """
 from functools import partial
 from typing import Any, Callable, Optional
@@ -71,26 +72,19 @@ def init_transformer_weights(module: nn.Module, initializer_range: float) -> Non
 
 
 class _RuntimeOwner(nn.Module):
-    """Lazily (re)builds the fused runtime when the module moves or its parameters are replaced."""
+    """Lazily (re)builds the module's fused runtime when the module moves or its parameters are replaced.  One runtime
+    serves both grad modes: forward + explicit backward under autograd, and the forward alone under torch.no_grad()."""
 
     _runtime_cls = None
 
-    def _runtime(self):
-        ids = [(id(p), p.device) for p in self.parameters()]
-        if getattr(self, "_rt", None) is None or self._rt_ids != ids:
-            object.__setattr__(self, "_rt", type(self)._runtime_cls(self))
-            object.__setattr__(self, "_rt_ids", ids)
-        return self._rt
-
-    def _train_runtime(self, *extra: Optional[nn.Module]):
-        """The training runtime (engine_flava_train): forward that keeps activations + explicit backward.  `extra`:
-        modules outside this encoder whose parameters its fused front end owns (the multimodal projections)."""
+    def _runtime(self, *extra: Optional[nn.Module]):
+        """`extra`: modules outside this one whose parameters its fused front end owns (the multimodal projections)."""
         mods = [m for m in extra if m is not None]
         ids = [(id(p), p.device) for m in (self, *mods) for p in m.parameters()]
-        if getattr(self, "_trt", None) is None or self._trt_ids != ids:
-            object.__setattr__(self, "_trt", type(self)._train_runtime_cls(self, *extra))
-            object.__setattr__(self, "_trt_ids", ids)
-        return self._trt
+        if getattr(self, "_rt", None) is None or self._rt_ids != ids:
+            object.__setattr__(self, "_rt", type(self)._runtime_cls(self, *extra))
+            object.__setattr__(self, "_rt_ids", ids)
+        return self._rt
 
 
 class FLAVATransformerWithoutEmbeddings(_RuntimeOwner):
@@ -119,20 +113,14 @@ class FLAVATransformerWithoutEmbeddings(_RuntimeOwner):
         from ... import engine_flava_train as T
         from ...engine import wants_grad
         if wants_grad(self) or (torch.is_grad_enabled() and hidden_states.requires_grad):
-            return T.encoder_output(self._train_runtime(None, None), None, (hidden_states,), self.pooler)
+            return T.encoder_output(self._runtime(), None, (hidden_states,), self.pooler)
         with torch.no_grad():
-            return self._runtime().forward(hidden_states, want_attn=bool(getattr(self, "output_attentions", False)))
+            return self._runtime().infer(hidden_states, want_attn=bool(getattr(self, "output_attentions", False)))
 
 
-def _mm_runtime(mod):
-    from ...engine_flava import FlavaMMRuntime
-    return FlavaMMRuntime(mod)
-
-
-def _mm_train_runtime(mod, image_proj=None, text_proj=None):
+def _mm_runtime(mod, image_proj=None, text_proj=None):
     from ...engine_flava_train import FlavaMMTrainRuntime
     return FlavaMMTrainRuntime(mod, image_proj, text_proj)
 
 
 FLAVATransformerWithoutEmbeddings._runtime_cls = staticmethod(_mm_runtime)
-FLAVATransformerWithoutEmbeddings._train_runtime_cls = staticmethod(_mm_train_runtime)

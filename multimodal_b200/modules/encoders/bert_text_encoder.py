@@ -1,5 +1,5 @@
 """`BERTTextEncoder` — drop-in for torchmultimodal/modules/encoders/bert_text_encoder.py:17-176.  Same constructor,
-state-dict keys and argument meaning; the forward is `engine_flava.FlavaTextRuntime` (fused embedding-sum + LayerNorm,
+state-dict keys and argument meaning; the forward is `engine_flava_train.FlavaTextTrainRuntime` (fused embedding-sum + LayerNorm,
 pad-derived key mask consumed by the tensor-core attention kernel, fused layer stack, layernorm, pooler).
 
 On the accelerated path: `input_ids` (required), `attention_mask` of shape [batch, seq_len], `token_type_ids`.
@@ -42,28 +42,21 @@ class BERTTextEncoder(_RuntimeOwner):
         if wants_grad(self):   # training: forward keeps activations, autograd nodes carry the explicit backward
             if return_attn_weights:
                 raise NotImplementedError("attention probabilities are not produced by the training forward")
-            out = T.encoder_output(self._train_runtime(), (input_ids, attention_mask, token_type_ids), (), self.pooler)
+            out = T.encoder_output(self._runtime(), (input_ids, attention_mask, token_type_ids), (), self.pooler)
         else:
             with torch.no_grad():
-                out = self._runtime().forward(input_ids, attention_mask, token_type_ids,
-                                              want_attn=bool(return_attn_weights))
+                out = self._runtime().infer(input_ids, attention_mask, token_type_ids, want_attn=bool(return_attn_weights))
         if not return_hidden_states:
             out = out._replace(hidden_states=None)
         return out
 
 
 def _txt_runtime(mod):
-    from ...engine_flava import FlavaTextRuntime
-    return FlavaTextRuntime(mod)
-
-
-def _txt_train_runtime(mod):
     from ...engine_flava_train import FlavaTextTrainRuntime
     return FlavaTextTrainRuntime(mod)
 
 
 BERTTextEncoder._runtime_cls = staticmethod(_txt_runtime)
-BERTTextEncoder._train_runtime_cls = staticmethod(_txt_train_runtime)
 
 
 def bert_text_encoder(hidden_size: int = 768, num_hidden_layers: int = 6, num_attention_heads: int = 12,

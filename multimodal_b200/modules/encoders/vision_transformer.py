@@ -1,5 +1,5 @@
 """`VisionTransformer` — drop-in for torchmultimodal/modules/encoders/vision_transformer.py:19-203 (constructor,
-`vision_transformer` builder and the vit_* presets).  Forward = `engine_coca.VisionRuntime`.  ``attentions`` is None
+`vision_transformer` builder and the vit_* presets).  Forward = `engine_coca_train.VisionTrainRuntime`.  ``attentions`` is None
 (flash-style attention); a custom ``pooler`` module, if given, is applied to ``last_hidden_state`` as in the reference.
 `GlobalAveragePooler` (MAE fine-tuning head) is outside SURVEY.md §8.  With `patch_drop_rate` the module drops patches in
 training only (either grad mode, the same random draws as the reference): `hidden_states` and `last_hidden_state` are
@@ -40,7 +40,7 @@ class VisionTransformer(_RuntimeOwner):
             warnings.warn("image_patches_mask passed but use_image_masking in init was false. Ignoring.")
         from ...engine import run, wants_grad
         if wants_grad(self):   # training: forward keeps activations, the autograd node carries the explicit backward
-            rt = self._train_runtime()
+            rt = self._runtime()
             (last,) = run(rt, (images, image_patches_mask), ())
             hidden, rt.last_hidden = rt.last_hidden, None
             B, S, d = hidden[0].shape
@@ -48,24 +48,18 @@ class VisionTransformer(_RuntimeOwner):
                                     attentions=None)
         else:
             with torch.no_grad():
-                out = self._runtime().forward(images, image_patches_mask)
+                out = self._runtime().infer(images, image_patches_mask)
         if self.pooler is not None:
             out = out._replace(pooler_output=self.pooler(out.last_hidden_state))
         return out
 
 
 def _vit_runtime(mod):
-    from ...engine_coca import VisionRuntime
-    return VisionRuntime(mod)
-
-
-def _vit_train_runtime(mod):
     from ...engine_coca_train import VisionTrainRuntime
     return VisionTrainRuntime(mod)
 
 
 VisionTransformer._runtime_cls = staticmethod(_vit_runtime)
-VisionTransformer._train_runtime_cls = staticmethod(_vit_train_runtime)
 
 
 def vision_transformer(*, patch_size: int, hidden_dim: int, dim_feedforward: int, n_layer: int, n_head: int,

@@ -1,8 +1,8 @@
 """`AttentionPooler` / `CascadedAttentionPooler` — drop-in for torchmultimodal/modules/layers/attention_pooler.py
-:16-101.  Forward = `engine_coca.PoolerRuntime`: LayerNorm-ed keys/values projected by one packed GEMM, the learned
+:16-101.  Forward = `engine_coca_train.PoolerTrainRuntime`: LayerNorm-ed keys/values projected by one packed GEMM, the learned
 queries projected once (they do not depend on the batch), cross-attention on the general attention kernel (head_dim 96
 for CoCa ViT-L/14), output projection + ln_post.  With grad mode on and trainable parameters (or an input that requires grad) the call
-runs `engine_coca_train.PoolerTrainRuntime` under autograd (the learned queries' gradient is summed over the batch)."""
+runs under autograd (the learned queries' gradient is summed over the batch)."""
 from typing import List
 
 import torch
@@ -25,24 +25,18 @@ class AttentionPooler(_RuntimeOwner):
     def forward(self, x: Tensor) -> Tensor:
         from ...engine import run, wants_grad
         if wants_grad(self) or (torch.is_grad_enabled() and x.requires_grad):
-            (out,) = run(self._train_runtime(), None, (x,))
+            (out,) = run(self._runtime(), None, (x,))
             return out.view(x.shape[0], self.query.shape[0], self.query.shape[1])
         with torch.no_grad():
-            return self._runtime().forward(x)
+            return self._runtime().infer(x)
 
 
 def _pool_runtime(mod):
-    from ...engine_coca import PoolerRuntime
-    return PoolerRuntime(mod, "pool")
-
-
-def _pool_train_runtime(mod):
     from ...engine_coca_train import PoolerTrainRuntime
     return PoolerTrainRuntime(mod)
 
 
 AttentionPooler._runtime_cls = staticmethod(_pool_runtime)
-AttentionPooler._train_runtime_cls = staticmethod(_pool_train_runtime)
 
 
 class CascadedAttentionPooler(nn.Module):

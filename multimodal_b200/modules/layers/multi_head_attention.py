@@ -1,7 +1,7 @@
 """Parameter containers mirroring torchmultimodal/modules/layers/multi_head_attention.py:19-180
 (`MultiHeadSelfAttention` with the fused ``input_proj [3d, d]``; `MultiHeadAttentionWithCache` with separate
 ``q_proj / k_proj / v_proj / output_proj``).  They execute inside the owning encoder / decoder / pooler runtime
-(engine_coca.py): packed-QKV wgmma GEMM + attention kernel; F.scaled_dot_product_attention is never called.  Both are
+(engine_coca_train.py): packed-QKV wgmma GEMM + attention kernel; F.scaled_dot_product_attention is never called.  Both are
 also callable on their own (forward values, engine_layers.py); `MultiHeadAttentionWithCache` then keeps the reference's
 key / value cache (`past_key_value` / `use_cache`) for autoregressive decoding, on the split-KV decode kernel."""
 from typing import NamedTuple, Optional, Tuple, Union

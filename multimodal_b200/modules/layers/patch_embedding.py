@@ -1,6 +1,6 @@
 """`PatchEmbeddings` — parameter container mirroring torchmultimodal/modules/layers/patch_embedding.py:25-157
 (conv projection with truncated-normal init, optional CLS token, position embeddings, optional mask token).  Executed
-by `engine_coca.VisionRuntime` as im2col + wgmma GEMM + one token-assembly kernel.  Random patch dropping
+by `engine_coca_train.VisionTrainRuntime` as im2col + wgmma GEMM + one token-assembly kernel.  Random patch dropping
 (`patch_drop_rate`: a float drops that share of the patches per sample, a (rate_h, rate_w) tuple drops whole patch rows
 and columns; FLIP, arXiv 2212.00794) applies in training only: the keep indices come from
 `modules/masking/random_masking.py` with the reference's random draws, and only the kept patches are embedded, by

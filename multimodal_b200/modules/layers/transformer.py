@@ -1,7 +1,7 @@
 """Mirror of torchmultimodal/modules/layers/transformer.py: `TransformerOutput` (:22-28, the NamedTuple every FLAVA /
 CoCa encoder returns) and the parameter containers `TransformerEncoderLayer` / `TransformerEncoder` (:31-259) and
 `TransformerDecoderLayer` / `TransformerDecoder` (:262-657) — same constructors, state-dict keys and creation order.
-The layers execute inside `engine_coca.LayerStack` (fused kernels), owned by VisionTransformer / CoCaTextDecoder /
+The layers execute inside `engine.TransformerStack` (fused kernels), owned by VisionTransformer / CoCaTextDecoder /
 CoCaMultimodalDecoder; all four are also callable on their own (forward values, same kernels: `engine_layers.py`), the
 decoders with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive decoding.
 
@@ -53,7 +53,7 @@ class TransformerEncoderLayer(nn.Module):
         self.norm_first = norm_first
 
     def forward(self, hidden_states: Tensor, attention_mask: Optional[Tensor] = None) -> Tensor:
-        """Standalone forward (values only; inside VisionTransformer the layer runs in the fused LayerStack)."""
+        """Standalone forward (values only; inside VisionTransformer the layer runs in the fused TransformerStack)."""
         from ...engine_layers import encoder_layer_forward
 
         return encoder_layer_forward(self, hidden_states, attention_mask)
@@ -79,7 +79,7 @@ class TransformerEncoder(nn.Module):
 
     def forward(self, hidden_states: Tensor, attention_mask: Optional[Tensor] = None,
                 return_hidden_states: bool = False) -> TransformerOutput:
-        """Standalone forward (values only; inside VisionTransformer the stack runs in the fused LayerStack)."""
+        """Standalone forward (values only; inside VisionTransformer the stack runs in the fused TransformerStack)."""
         from ...engine_layers import encoder_forward
 
         return encoder_forward(self, hidden_states, attention_mask, return_hidden_states)
@@ -115,7 +115,7 @@ class TransformerDecoderLayer(nn.Module):
                 attention_mask: Optional[Tensor] = None, cross_attention_mask: Optional[Tensor] = None,
                 past_key_value: Optional[Tuple[Tensor, Tensor]] = None,
                 use_cache: bool = False) -> Tuple[Tensor, Optional[Tuple[Tensor, Tensor]]]:
-        """Standalone forward (values only; inside CoCa the layer runs in the fused LayerStack)."""
+        """Standalone forward (values only; inside CoCa the layer runs in the fused TransformerStack)."""
         from ...engine_layers import decoder_layer_forward
 
         return decoder_layer_forward(self, hidden_states, encoder_hidden_states, attention_mask, cross_attention_mask,
@@ -144,7 +144,7 @@ class TransformerDecoder(nn.Module):
                 attention_mask: Optional[Tensor] = None, cross_attention_mask: Optional[Tensor] = None,
                 past_key_values: Optional[List[Tuple[Tensor, Tensor]]] = None, use_cache: bool = False,
                 return_hidden_states: bool = False) -> TransformerOutput:
-        """Standalone forward (values only; inside CoCa the stack runs in the fused LayerStack)."""
+        """Standalone forward (values only; inside CoCa the stack runs in the fused TransformerStack)."""
         from ...engine_layers import decoder_forward
 
         return decoder_forward(self, hidden_states, encoder_hidden_states, attention_mask, cross_attention_mask,

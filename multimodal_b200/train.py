@@ -32,6 +32,8 @@ class _CastBack:
 
 class _FlatAdamW:
     def __init__(self, store: ParamStore, lr, betas, eps, weight_decay):
+        if store.wb.numel() != store.total:
+            raise MMBError("the fused AdamW step writes a bf16 shadow of every parameter (no fp32_only parameters)")
         store.flatten_()
         self.store = store
         self.m = torch.zeros_like(store.master)

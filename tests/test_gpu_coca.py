@@ -24,8 +24,8 @@ def dev():
 
 @pytest.fixture(autouse=True)
 def _inference():
-    """This file pins the INFERENCE runtime (engine_coca.py); with grad mode on, trainable modules take the training
-    runtime instead (engine_coca_train.py, covered by tests/test_gpu_coca_train.py)."""
+    """This file pins the no_grad forwards of the CoCa runtimes (engine_coca_train.py); their training forwards and
+    backwards are covered by tests/test_gpu_coca_train.py."""
     with torch.no_grad():
         yield
 

@@ -24,8 +24,8 @@ def dev():
 
 @pytest.fixture(autouse=True)
 def _inference():
-    """This file pins the INFERENCE runtime (engine_flava.py); with grad mode on, trainable modules take the training
-    runtime instead (engine_flava_train.py, covered by tests/test_gpu_flava_train.py)."""
+    """This file pins the no_grad forwards of the FLAVA runtimes (engine_flava_train.py); their training forwards and
+    backwards are covered by tests/test_gpu_flava_train.py."""
     with torch.no_grad():
         yield
 

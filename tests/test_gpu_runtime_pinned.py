@@ -125,8 +125,60 @@ def _text_decoder_no_cls():
     return m.eval(), ids
 
 
+def _head_dim_modules(hd):
+    """A VisionTransformer and a CoCaTextDecoder with heads of head_dim `hd` (the general attention kernels) and a width
+    that is a multiple of 128 (the LayerNorm kernels)."""
+    from multimodal_b200.models.coca.text_decoder import CoCaTextDecoder
+    from multimodal_b200.modules.encoders.vision_transformer import vision_transformer
+
+    heads = 4 if hd == 96 else 2
+    d = heads * hd
+    torch.manual_seed(0)
+    vit = vision_transformer(patch_size=8, hidden_dim=d, dim_feedforward=2 * d, n_layer=2, n_head=heads, image_size=32)
+    txt = CoCaTextDecoder(vocab_size=300, num_positions=13, embedding_dim=d, n_layer=2, n_head=heads,
+                          dim_feedforward=2 * d, output_dim=96)
+    g = torch.Generator().manual_seed(19)
+    with torch.no_grad():
+        for p in list(vit.parameters()) + list(txt.parameters()):
+            p.add_(0.03 * torch.randn(p.shape, generator=g))
+    images = torch.randn(3, 3, 32, 32, generator=g)
+    ids = torch.randint(1, 300, (3, 12), generator=g)
+    ids[1, 7:] = 0
+    return vit.eval(), txt.eval(), images, ids
+
+
+def _vit_drop():
+    """VisionTransformer with patch dropping and stochastic depth, left in train() mode."""
+    from multimodal_b200.modules.encoders.vision_transformer import vision_transformer
+
+    torch.manual_seed(0)
+    vit = vision_transformer(patch_size=4, hidden_dim=128, dim_feedforward=256, n_layer=3, n_head=2, image_size=32,
+                             patch_drop_rate=0.25, drop_path_rate=0.5)
+    g = torch.Generator().manual_seed(23)
+    with torch.no_grad():
+        for p in vit.parameters():
+            p.add_(0.03 * torch.randn(p.shape, generator=g))
+    return vit.train(), torch.randn(4, 3, 32, 32, generator=g)
+
+
 def _case(name, dev):
     """{output name: tensor} of one pinned forward."""
+    if name in ("coca_hd96.infer", "coca_hd128.infer"):
+        vit, txt, images, ids = _head_dim_modules(96 if name == "coca_hd96.infer" else 128)
+        with torch.no_grad():
+            v = vit.to(dev)(images.to(dev))
+            pooled, tokens = txt.to(dev)(ids.to(dev))
+        res = {"vision.last_hidden_state": v.last_hidden_state, "text.pooled": pooled, "text.tokens": tokens}
+        res.update({f"vision.hidden_states.{i}": h for i, h in enumerate(v.hidden_states)})
+        return res
+    if name == "vit_drop.infer":
+        vit, images = _vit_drop()
+        vit, images = vit.to(dev), images.to(dev)
+        torch.manual_seed(29)
+        with torch.no_grad():
+            v = vit(images)
+        return {"last_hidden_state": v.last_hidden_state,
+                **{f"hidden_states.{i}": h for i, h in enumerate(v.hidden_states)}}
     if name.startswith("flava_small") or name.startswith("flava_long"):
         base, mode = name.rsplit(".", 1)
         m, inp = _flava(base)
@@ -166,7 +218,8 @@ def _case(name, dev):
 
 CASES = ["flava_small.infer", "flava_small.grad", "flava_long.infer", "flava_long.grad", "flava_attentions.infer",
          "flava_text512.infer", "flava_text512.grad", "coca_small.infer", "coca_small.grad", "coca_parallel.infer",
-         "coca_parallel.grad", "coca_l14.infer", "coca_l14.grad", "text_decoder_no_cls.infer"]
+         "coca_parallel.grad", "coca_l14.infer", "coca_l14.grad", "text_decoder_no_cls.infer", "coca_hd96.infer",
+         "coca_hd128.infer", "vit_drop.infer"]
 
 # {case: {output: sha256 of its bytes}}, recorded on an H100 80GB HBM3
 PINNED = {
@@ -350,6 +403,29 @@ PINNED = {
     'text_decoder_no_cls.infer': {
         'pooled': '(3, 96) torch.float32 4ba4cb180ee243644111ef7330578468a1c9aa52c868956c17edb35f3417bef2',
         'tokens': '(3, 20, 128) torch.float32 6f83ad91f4941ecf1021bc206d61d1806e9c8deedc50ae0c88714baf442ff723',
+    },
+    'coca_hd96.infer': {
+        'text.pooled': '(3, 96) torch.float32 df8a09f65011359bde2f795280659d297d2c7fe12c73f8a29a694a94ffd16d3d',
+        'text.tokens': '(3, 12, 384) torch.float32 578e27886854eeca0375936bedf31fae2dc9cb723dd6a0b0851934053fd33e40',
+        'vision.hidden_states.0': '(3, 17, 384) torch.float32 7ab812352e8631f0b79ddb4b0705fb109c9a7c02833a6117f60c2e76419ba894',
+        'vision.hidden_states.1': '(3, 17, 384) torch.float32 8f9a0891867fae69a5ca24b22e8c144e465ce9216c95ac1f8316f460bbd38b60',
+        'vision.hidden_states.2': '(3, 17, 384) torch.float32 a03195aeacf199b136094b98a680e68490ef1f6135a72bd3c9bf0253da2a797d',
+        'vision.last_hidden_state': '(3, 17, 384) torch.float32 ddec42f7f075a220c0915d30253e96e9addc84696991015ba35907d02e479152',
+    },
+    'coca_hd128.infer': {
+        'text.pooled': '(3, 96) torch.float32 475162f4edd175574f75a37e3663cead4e4d61e19fd37e9b6b01b8f2334faf74',
+        'text.tokens': '(3, 12, 256) torch.float32 14b1ce34bba70acb0022e9110f040ce70344fb8584690ff1857dd448b7241a82',
+        'vision.hidden_states.0': '(3, 17, 256) torch.float32 351b996edbe39c247153173c2c25a6f8fbd353942f87e81194912ed3ffaf5e33',
+        'vision.hidden_states.1': '(3, 17, 256) torch.float32 8fa35243b1d33e05758ac66ad9fa0737facf047c88b9e806be93a2ae8489c446',
+        'vision.hidden_states.2': '(3, 17, 256) torch.float32 2f5d7c34985f4e7422e2effb2e3847d66760bd1490740a91fe38a1409c2c7c41',
+        'vision.last_hidden_state': '(3, 17, 256) torch.float32 1cccd9c0d6cb73707a0f8c4b2ae8e6d4d90d3b9b232f4daccbe90b400c7c3a09',
+    },
+    'vit_drop.infer': {
+        'hidden_states.0': '(4, 49, 128) torch.float32 a72ce5802d3d2c6ff02e3a7ba80c36d535edfa4ab0d32067813bf94c382df4e3',
+        'hidden_states.1': '(4, 49, 128) torch.float32 440ce22451cf3c4a6db98f49025a01d223ceffa90f88db64fcabb7b6a7102a75',
+        'hidden_states.2': '(4, 49, 128) torch.float32 5202f2a331bb8808a3e879dd3d756a718057f0815799ff20ca43a4bc4487f704',
+        'hidden_states.3': '(4, 49, 128) torch.float32 437ca8147ac89289541a23bbfbb3f044d382965d8854a1ca9b840259343effeb',
+        'last_hidden_state': '(4, 49, 128) torch.float32 9a8695b5e151fd81289c90be6f254083b12d0c3e69e551b41920f0fe43f3d267',
     },
 }
 
