@@ -1,51 +1,11 @@
-"""torch.autograd glue: lets the explicit forward/backward runtimes (engine.py) sit behind ordinary nn.Modules so
-that ``model(x); loss.backward(); torch.optim...step()`` works exactly as with the reference modules."""
+"""torch.autograd glue beside the module runtimes (whose autograd node is engine.RuntimeFunction): the L2 normalisation
+of CLIP's embeddings and the autocast dtype convention at the module boundary."""
 from __future__ import annotations
-
-from typing import Optional
 
 import torch
 
 from . import ops
 from ._lib import MMBError
-
-
-class TowerFunction(torch.autograd.Function):
-    """Whole-encoder forward/backward.  inputs: (runtime, data, *parameters)."""
-
-    @staticmethod
-    def forward(ctx, runtime, data, *params):
-        training = any(ctx.needs_input_grad[2:])
-        emb = runtime.forward(data, training)
-        ctx.runtime, ctx.gen, ctx.n = runtime, runtime.gen, len(params)
-        ctx.need = ctx.needs_input_grad[2:]
-        return emb
-
-    @staticmethod
-    def backward(ctx, demb):
-        rt = ctx.runtime
-        if rt.gen != ctx.gen:
-            raise MMBError("the encoder ran another forward before this backward: its saved activations were "
-                           "overwritten (one in-flight training forward per encoder instance)")
-        st = rt.store
-        flat = st.master is not None
-        if not flat:
-            st.zero_grads()
-        rt.backward(demb.contiguous().float())
-        if flat:  # p.grad are views of the flat buffer: gradients were accumulated in place
-            # `optimizer.zero_grad(set_to_none=True)` (torch's default) or `p.grad = None` severs those views; re-attach
-            # them, otherwise gradients would pile up invisibly in the flat buffer while the optimizer skips the parameter
-            for p in st.params:
-                want = st.grad(p)
-                if p.grad is None or p.grad.data_ptr() != want.data_ptr():
-                    p.grad = want
-            return (None, None) + (None,) * ctx.n
-        g = st.g.clone()
-        grads = []
-        for p, need in zip(st.params, ctx.need):
-            o = st.off[id(p)]
-            grads.append(g[o:o + p.numel()].view(p.shape) if need else None)
-        return (None, None, *grads)
 
 
 class L2NormalizeFunction(torch.autograd.Function):

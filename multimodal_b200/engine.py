@@ -580,7 +580,7 @@ class TransformerStack:
 
 
 class ViTTower:
-    """CLIPViTEncoder runtime (models/clip/image_encoder.py:82-113)."""
+    """CLIPViTEncoder runtime (models/clip/image_encoder.py:82-113).  Output: the embeddings fp32 [B, E]."""
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
@@ -593,11 +593,11 @@ class ViTTower:
         require_head_dim_64(d, layer0.self_attn.num_heads)
         self.stack = TransformerStack(mod.encoder.layers, self.store, self.ws, d=d, heads=layer0.self_attn.num_heads,
                                       ff=layer0.linear1.weight.shape[0], act=ops.ACT_QUICK_GELU, prefix="img")
-        self.gen = 0
 
-    def forward(self, image: torch.Tensor, training: bool, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _forward(self, image: torch.Tensor, save: Optional[Workspace], out: Optional[torch.Tensor] = None):
         """out (optional): fp32 [B, E] destination of the embeddings (e.g. a row block of a larger buffer)."""
         mod, st, ws, d = self.mod, self.store, self.ws, self.d
+        keep = save if save is not None else ws
         if image.dtype != torch.float32:
             image = image.float()
         image = image.contiguous()
@@ -609,10 +609,10 @@ class ViTTower:
         bf, f32 = torch.bfloat16, torch.float32
         st.refresh()
         Kp = -(-K // 8) * 8   # row pitch: bf16 rows must be 16 B multiples for TMA (K = 588 -> 592 for 14x14 patches)
-        PATCH = ws.get("img.PATCH", (B * P, Kp), bf)[:, :K]
-        PO = ws.get("img.PO", (B * P, d), bf)
-        X0 = ws.get("img.X0", (B * S, d), f32)
-        m0 = ws.get("img.m0", (B * S,), f32); r0 = ws.get("img.r0", (B * S,), f32)
+        PATCH = keep.get("img.PATCH", (B * P, Kp), bf)[:, :K]
+        PO = keep.get("img.PO", (B * P, d), bf)
+        X0 = keep.get("img.X0", (B * S, d), f32)
+        m0 = keep.get("img.m0", (B * S,), f32); r0 = keep.get("img.r0", (B * S,), f32)
         ops.im2col(image, ps, PATCH)
         wconv = st.shadow2d(mod.conv.weight)
         if Kp != K:  # re-pitch the (tiny) conv weight shadow the same way
@@ -622,49 +622,60 @@ class ViTTower:
         ops.gemm(PATCH, wconv, out=PO)
         ops.vit_embed_ln_fwd(PO, mod.cls_token_embedding, mod.positional_embedding, mod.ln_pre.weight, mod.ln_pre.bias,
                              X0, m0, r0, B, S, d, mod.ln_pre.eps)
-        XM, Y = self.stack.forward(X0, B, S, ws if training else None)
-        XSEL = ws.get("img.XSEL", (B, d), f32)
-        LNP = ws.get("img.LNP", (B, d), bf)
-        mP = ws.get("img.mP", (B,), f32); rP = ws.get("img.rP", (B,), f32)
+        XM, Y = self.stack.forward(X0, B, S, save)
+        XSEL = keep.get("img.XSEL", (B, d), f32)
+        LNP = keep.get("img.LNP", (B, d), bf)
+        mP = keep.get("img.mP", (B,), f32); rP = keep.get("img.rP", (B,), f32)
         ops.add_layernorm_fwd(XM, Y, XSEL, LNP, None, mod.ln_post.weight, mod.ln_post.bias, mP, rP, B, d, mod.ln_post.eps,
                               row_idx=None, rows_per_group=S)
         EMB = out if out is not None else torch.empty((B, self.E), device=image.device, dtype=f32)
         ops.gemm(LNP, st.shadow(mod.projection), b_mn=True, epilogue=ops.EPI_F32, out=EMB)
-        self.B, self.S, self.P = B, S, P
-        self.gen += 1
+        if save is not None:
+            save.B, save.S, save.P = B, S, P
         return EMB
 
-    def backward(self, dEMB: torch.Tensor) -> None:
+    def forward(self, data, diff, save: Optional[Workspace] = None):
+        """data: (image,).  save: the Workspace that keeps what the backward reads (default: a new one)."""
+        save = Workspace(self.store.device) if save is None else save
+        return (self._forward(*data, save),), save
+
+    def infer(self, image: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        return self._forward(image, None, out)
+
+    def backward(self, save: Workspace, dEMB: torch.Tensor, on_layer_done=None):
+        """on_layer_done(l): called once every parameter gradient of layer l is final (data-parallel all-reduce)."""
         mod, st, ws, d = self.mod, self.store, self.ws, self.d
-        B, S, P = self.B, self.S, self.P
+        B, S, P = save.B, save.S, save.P
         bf, f32 = torch.bfloat16, torch.float32
         M = B * S
-        dEb = ops.cast_bf16(dEMB.contiguous())
-        LNP, XSEL = ws.get("img.LNP", (B, d), bf), ws.get("img.XSEL", (B, d), f32)
+        dEb = ops.cast_bf16(dEMB.contiguous().float())
+        LNP, XSEL = save.get("img.LNP", (B, d), bf), save.get("img.XSEL", (B, d), f32)
         ops.gemm(LNP, dEb, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(mod.projection), accumulate=True)
         dLNP = ws.get("img.dLNP", (B, d), f32)
         ops.gemm(dEb, st.shadow(mod.projection), epilogue=ops.EPI_F32, out=dLNP)
         G = ws.get("img.G", (M, d), f32)
         Gb = ws.get("img.Gb", (M, d), bf)
         ops.zero_(G); ops.zero_(Gb)
-        ops.layernorm_bwd(XSEL, None, dLNP, ws.get("img.mP", (B,), f32), ws.get("img.rP", (B,), f32), mod.ln_post.weight, None, G, Gb,
-                          st.grad(mod.ln_post.weight), st.grad(mod.ln_post.bias), B, d, row_idx=None, rows_per_group=S,
-                          gsum=self.stack.top_bias_grad())
-        self.stack.backward(G, Gb, B, S, save=ws, on_layer_done=getattr(self, "layer_done_cb", None), top_bias_done=True)
-        PO = ws.get("img.PO", (B * P, d), bf)
+        ops.layernorm_bwd(XSEL, None, dLNP, save.get("img.mP", (B,), f32), save.get("img.rP", (B,), f32),
+                          mod.ln_post.weight, None, G, Gb, st.grad(mod.ln_post.weight), st.grad(mod.ln_post.bias), B, d,
+                          row_idx=None, rows_per_group=S, gsum=self.stack.top_bias_grad())
+        self.stack.backward(G, Gb, B, S, save=save, on_layer_done=on_layer_done, top_bias_done=True)
+        PO = save.get("img.PO", (B * P, d), bf)
         DP = ws.get("img.DP", (B * P, d), bf)
-        ops.vit_embed_ln_bwd(PO, mod.cls_token_embedding, mod.positional_embedding, G, ws.get("img.m0", (M,), f32), ws.get("img.r0", (M,), f32),
-                             mod.ln_pre.weight, G, DP, st.grad(mod.ln_pre.weight), st.grad(mod.ln_pre.bias), B, S, d)
+        ops.vit_embed_ln_bwd(PO, mod.cls_token_embedding, mod.positional_embedding, G, save.get("img.m0", (M,), f32),
+                             save.get("img.r0", (M,), f32), mod.ln_pre.weight, G, DP, st.grad(mod.ln_pre.weight),
+                             st.grad(mod.ln_pre.bias), B, S, d)
         ops.batch_sum(G, st.grad(mod.positional_embedding), B, S * d, S * d)
         ops.batch_sum(G, st.grad(mod.cls_token_embedding), B, S * d, d)
         K = 3 * self.ps * self.ps
-        PATCH = ws.get("img.PATCH", (B * P, -(-K // 8) * 8), bf)[:, :K]
+        PATCH = save.get("img.PATCH", (B * P, -(-K // 8) * 8), bf)[:, :K]
         ops.gemm(DP, PATCH, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad2d(mod.conv.weight),
                  splits=ops.wgrad_splits(d, PATCH.shape[1], B * P), accumulate=True)
+        return ()
 
 
 class TextTower:
-    """CLIPTextEncoder runtime (models/clip/text_encoder.py:113-134)."""
+    """CLIPTextEncoder runtime (models/clip/text_encoder.py:113-134).  Output: the embeddings fp32 [B, E]."""
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
@@ -677,60 +688,70 @@ class TextTower:
         self.stack = TransformerStack(mod.encoder.layers, self.store, self.ws, d=self.d,
                                       heads=layer0.self_attn.num_heads, ff=layer0.linear1.weight.shape[0],
                                       act=ops.ACT_QUICK_GELU, prefix="txt")
-        self.gen = 0
 
-    def forward(self, text: torch.Tensor, training: bool, return_hidden_state: bool = False,
-                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _forward(self, text: torch.Tensor, save: Optional[Workspace], return_hidden_state: bool = False,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
         mod, st, ws, d = self.mod, self.store, self.ws, self.d
+        keep = save if save is not None else ws
         if text.dtype != torch.int64:
             text = text.long()
         text = text.contiguous()
         B, S = text.shape
         bf, f32 = torch.bfloat16, torch.float32
         st.refresh()
-        X0 = ws.get("txt.X0", (B * S, d), f32)
+        X0 = keep.get("txt.X0", (B * S, d), f32)
         V = mod.token_embedding.weight.shape[0]
         ops.text_embed_fwd(text, mod.token_embedding.weight, mod.positional_embedding, X0, B, S, d, V)
-        XM, Y = self.stack.forward(X0, B, S, ws if training and not return_hidden_state else None, causal=True)
+        XM, Y = self.stack.forward(X0, B, S, save, causal=True)
         if return_hidden_state:
             HS = torch.empty((B, S, d), device=text.device, dtype=f32)
             ops.add_layernorm_fwd(XM, Y, None, None, HS, mod.ln_final.weight, mod.ln_final.bias, None, None, B * S, d,
                                   mod.ln_final.eps)
             return HS
-        IDX = ws.get("txt.IDX", (B,), torch.int32)
+        IDX = keep.get("txt.IDX", (B,), torch.int32)
         ops.argmax_tokens(text, IDX, B, S)
-        XSEL = ws.get("txt.XSEL", (B, d), f32)
-        LNF = ws.get("txt.LNF", (B, d), bf)
-        mF = ws.get("txt.mF", (B,), f32); rF = ws.get("txt.rF", (B,), f32)
+        XSEL = keep.get("txt.XSEL", (B, d), f32)
+        LNF = keep.get("txt.LNF", (B, d), bf)
+        mF = keep.get("txt.mF", (B,), f32); rF = keep.get("txt.rF", (B,), f32)
         ops.add_layernorm_fwd(XM, Y, XSEL, LNF, None, mod.ln_final.weight, mod.ln_final.bias, mF, rF, B, d,
                               mod.ln_final.eps, row_idx=IDX, rows_per_group=S)
         EMB = out if out is not None else torch.empty((B, self.E), device=text.device, dtype=f32)
         ops.gemm(LNF, st.shadow(mod.projection.weight), epilogue=ops.EPI_F32, out=EMB)
-        self.B, self.S = B, S
-        self.tokens = text if training else None
-        self.gen += 1
+        if save is not None:
+            save.B, save.S, save.tokens = B, S, text
         return EMB
 
-    def backward(self, dEMB: torch.Tensor) -> None:
+    def forward(self, data, diff, save: Optional[Workspace] = None):
+        """data: (text,).  save: the Workspace that keeps what the backward reads (default: a new one)."""
+        save = Workspace(self.store.device) if save is None else save
+        return (self._forward(*data, save),), save
+
+    def infer(self, text: torch.Tensor, return_hidden_state: bool = False,
+              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The embeddings, or with return_hidden_state the ln_final-ed hidden states fp32 [B, S, width]."""
+        return self._forward(text, None, return_hidden_state, out)
+
+    def backward(self, save: Workspace, dEMB: torch.Tensor, on_layer_done=None):
         mod, st, ws, d = self.mod, self.store, self.ws, self.d
-        B, S = self.B, self.S
+        B, S = save.B, save.S
         bf, f32 = torch.bfloat16, torch.float32
         M = B * S
-        dEb = ops.cast_bf16(dEMB.contiguous())
-        LNF, XSEL = ws.get("txt.LNF", (B, d), bf), ws.get("txt.XSEL", (B, d), f32)
+        dEb = ops.cast_bf16(dEMB.contiguous().float())
+        LNF, XSEL = save.get("txt.LNF", (B, d), bf), save.get("txt.XSEL", (B, d), f32)
         ops.gemm(dEb, LNF, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(mod.projection.weight), accumulate=True)
         dLNF = ws.get("txt.dLNF", (B, d), f32)
         ops.gemm(dEb, st.shadow(mod.projection.weight), b_mn=True, epilogue=ops.EPI_F32, out=dLNF)
         G = ws.get("txt.G", (M, d), f32)
         Gb = ws.get("txt.Gb", (M, d), bf)
         ops.zero_(G); ops.zero_(Gb)
-        IDX = ws.get("txt.IDX", (B,), torch.int32)
-        ops.layernorm_bwd(XSEL, None, dLNF, ws.get("txt.mF", (B,), f32), ws.get("txt.rF", (B,), f32), mod.ln_final.weight, None, G, Gb,
-                          st.grad(mod.ln_final.weight), st.grad(mod.ln_final.bias), B, d, row_idx=IDX, rows_per_group=S,
-                          gsum=self.stack.top_bias_grad())
-        self.stack.backward(G, Gb, B, S, save=ws, top_bias_done=True)
+        IDX = save.get("txt.IDX", (B,), torch.int32)
+        ops.layernorm_bwd(XSEL, None, dLNF, save.get("txt.mF", (B,), f32), save.get("txt.rF", (B,), f32),
+                          mod.ln_final.weight, None, G, Gb, st.grad(mod.ln_final.weight), st.grad(mod.ln_final.bias), B,
+                          d, row_idx=IDX, rows_per_group=S, gsum=self.stack.top_bias_grad())
+        self.stack.backward(G, Gb, B, S, save=save, on_layer_done=on_layer_done, top_bias_done=True)
         ops.batch_sum(G, st.grad(mod.positional_embedding), B, S * d, S * d)
-        ops.text_embed_bwd(self.tokens, G, st.grad(mod.token_embedding.weight), B, S, d)
+        ops.text_embed_bwd(save.tokens, G, st.grad(mod.token_embedding.weight), B, S, d)
+        return ()
 
 
 class RuntimeFunction(torch.autograd.Function):
@@ -751,9 +772,19 @@ class RuntimeFunction(torch.autograd.Function):
         if save is None:
             raise MMBError("this forward was already back-propagated (its activations are freed)")
         st = rt.store
-        st.zero_grads()
+        flat = st.master is not None
+        if not flat:
+            st.zero_grads()
         in_grads = rt.backward(save, *douts)
         ctx.save = None
+        if flat:  # p.grad are views of the flat buffer: gradients were accumulated in place
+            # `optimizer.zero_grad(set_to_none=True)` (torch's default) or `p.grad = None` severs those views; re-attach
+            # them, otherwise gradients would pile up invisibly in the flat buffer while the optimizer skips the parameter
+            for p in st.params:
+                want = st.grad(p)
+                if p.grad is None or p.grad.data_ptr() != want.data_ptr():
+                    p.grad = want
+            return (None, None, None, *in_grads) + (None,) * len(st.params)
         g = st.g.clone()
         grads = []
         for p, need in zip(st.params, ctx.need):
@@ -764,3 +795,20 @@ class RuntimeFunction(torch.autograd.Function):
 
 def run(rt, data, diff: Sequence[torch.Tensor] = ()):
     return RuntimeFunction.apply(rt, data, len(diff), *diff, *rt.store.params)
+
+
+class _RuntimeOwner(nn.Module):
+    """Lazily (re)builds the module's fused runtime when the module moves or its parameters are replaced.  One runtime
+    serves both grad modes: forward + explicit backward under autograd (`run`), and `infer` under torch.no_grad()."""
+
+    _runtime_cls = None
+
+    def _runtime(self, *extra: Optional[nn.Module]):
+        """`extra`: modules outside this one whose parameters its fused front end owns (the multimodal projections)."""
+        mods = [m for m in extra if m is not None]
+        ids = [(id(p), p.device) for m in (self, *mods) for p in m.parameters()]
+        if getattr(self, "_rt", None) is None or self._rt_ids != ids:
+            object.__setattr__(self, "_rt", type(self)._runtime_cls(self, *extra))
+            object.__setattr__(self, "_rt_ids", ids)
+            watch_module(self)
+        return self._rt

@@ -8,16 +8,15 @@ fused LayerNorm / QKV / attention / MLP kernels on Hopper tensor cores (see DESI
 import torch
 from torch import nn, Tensor
 
-from ...autograd import TowerFunction
 from ...autograd import autocast_out as _autocast_out
-from ...engine import watch_module, ViTTower
+from ...engine import _RuntimeOwner, run, ViTTower, wants_grad
 from ...modules.layers.activation import SiLU
 from ...modules.layers.normalizations import Fp32LayerNorm
 
 EXPANSION = 4
 
 
-class CLIPViTEncoder(nn.Module):
+class CLIPViTEncoder(_RuntimeOwner):
     """Vision transformer encoder for CLIP.
 
     Args:
@@ -30,6 +29,8 @@ class CLIPViTEncoder(nn.Module):
 
     Inputs: x (Tensor): B x 3 x image_size x image_size, CUDA.
     """
+
+    _runtime_cls = ViTTower
 
     def __init__(self, embedding_dim: int, patch_size: int, image_size: int, width: int, heads: int, layers: int):
         super().__init__()
@@ -45,14 +46,6 @@ class CLIPViTEncoder(nn.Module):
         self.encoder = nn.TransformerEncoder(encoder_layer, num_layers=layers, enable_nested_tensor=False)
         self.ln_post = Fp32LayerNorm(width)
         self.projection = nn.Parameter(scale * torch.randn(width, embedding_dim))
-        self._rt = None
-
-    def _runtime(self) -> ViTTower:
-        ids = [id(p) for p in self.parameters()]
-        if self._rt is None or self._rt.store.device != self.projection.device or self._rt_ids != ids:
-            self._rt, self._rt_ids = ViTTower(self), ids
-            watch_module(self)
-        return self._rt
 
     def forward(self, x: Tensor) -> Tensor:
         if x.size(2) != self.image_size or x.size(3) != self.image_size:
@@ -60,6 +53,9 @@ class CLIPViTEncoder(nn.Module):
                 f"Expected input with width and height as {self.image_size}, found {x.size(2)} by {x.size(3)} ")
         if x.size(1) != 3:
             raise ValueError(f"Expected 3 channels found {x.size(1)}")
-        rt = self._runtime()
-        params = rt.store.params if torch.is_grad_enabled() else ()
-        return _autocast_out(TowerFunction.apply(rt, x, *params))
+        if wants_grad(self):   # training: forward keeps activations, the autograd node carries the explicit backward
+            (emb,) = run(self._runtime(), (x,))
+        else:
+            with torch.no_grad():
+                emb = self._runtime().infer(x)
+        return _autocast_out(emb)

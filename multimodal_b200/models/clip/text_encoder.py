@@ -9,19 +9,14 @@ import torch
 from torch import nn, Tensor
 from torch.nn import TransformerEncoder, TransformerEncoderLayer
 
-from ...autograd import TowerFunction
 from ..._lib import MMBError
 from ...autograd import autocast_out as _autocast_out
-from ...engine import watch_module, TextTower
+from ...engine import _RuntimeOwner, run, TextTower, wants_grad
 from ...modules.layers.activation import SiLU
 from ...modules.layers.normalizations import Fp32LayerNorm
 
 
-class _TextFunction(TowerFunction):
-    pass
-
-
-class CLIPTextEncoder(nn.Module):
+class CLIPTextEncoder(_RuntimeOwner):
     """CLIP text encoder (Transformer with causal attention).
 
     Args: embedding_dim, context_length, vocab_size, width, dim_feedforward, heads, layers, use_clip_init
@@ -29,6 +24,7 @@ class CLIPTextEncoder(nn.Module):
     Inputs: text (Tensor[int64] B x context_length, CUDA); return_hidden_state (bool).
     """
 
+    _runtime_cls = TextTower
     TOKEN_EMBEDDING_INIT_STD = 0.02
     POS_EMBEDDING_INIT_STD = 0.01
 
@@ -47,7 +43,6 @@ class CLIPTextEncoder(nn.Module):
         self.mask = torch.full((self.context_length, self.context_length), float("-inf")).triu(1)
         if use_clip_init:
             self.initialize_parameters()
-        self._rt = None
 
     def initialize_parameters(self) -> None:
         # text_encoder.py:82-104
@@ -66,23 +61,17 @@ class CLIPTextEncoder(nn.Module):
     def build_attention_mask(self) -> Tensor:
         return torch.full((self.context_length, self.context_length), float("-inf")).triu(1)
 
-    def _runtime(self) -> TextTower:
-        ids = [id(p) for p in self.parameters()]
-        if self._rt is None or self._rt.store.device != self.positional_embedding.device or self._rt_ids != ids:
-            self._rt, self._rt_ids = TextTower(self), ids
-            watch_module(self)
-        return self._rt
-
     def forward(self, text: Tensor, return_hidden_state: bool = False) -> Tensor:
         if text.size(1) != self.context_length:
             raise ValueError(f"length of input should be {self.context_length} but found {text.size(1)}")
-        rt = self._runtime()
-        if return_hidden_state:
-            if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if wants_grad(self):
+            if return_hidden_state:
                 # the [B, 77, width] hidden-state output is not on the contrastive path and has no backward schedule:
                 # returning a detached tensor would silently drop the gradient, so refuse instead
                 raise MMBError("CLIPTextEncoder(return_hidden_state=True) returns forward values only (no backward "
                                "schedule for the per-token output); call it under torch.no_grad()")
-            return _autocast_out(rt.forward(text, False, return_hidden_state=True))
-        params = rt.store.params if torch.is_grad_enabled() else ()
-        return _autocast_out(TowerFunction.apply(rt, text, *params))
+            (emb,) = run(self._runtime(), (text,))
+        else:
+            with torch.no_grad():
+                emb = self._runtime().infer(text, return_hidden_state=return_hidden_state)
+        return _autocast_out(emb)

@@ -6,9 +6,9 @@ from typing import Callable, Optional
 import torch
 from torch import nn, Tensor
 
+from ...engine import _RuntimeOwner
 from ...modules.layers.transformer import TransformerDecoder
 from ...utils.attention import get_causal_attention_mask
-from ..flava.transformer import _RuntimeOwner
 
 
 class CoCaMultimodalDecoder(_RuntimeOwner):

@@ -9,9 +9,9 @@ import torch.nn.functional as F
 from torch import nn, Tensor
 
 from ..._lib import MMBError
+from ...engine import _RuntimeOwner
 from ...modules.layers.transformer import TransformerDecoder
 from ...utils.attention import get_causal_attention_mask
-from ..flava.transformer import _RuntimeOwner
 
 
 class CoCaTextEmbeddings(nn.Module):

@@ -10,10 +10,11 @@ import torch
 from torch import nn, Tensor
 
 from ..._lib import MMBError
+from ...engine import _RuntimeOwner
 from ...modules.layers.normalizations import Fp32LayerNorm
 from ...modules.layers.transformer import TransformerOutput
 from ...modules.losses.flava import Pooler
-from .transformer import _RuntimeOwner, init_transformer_weights, TransformerEncoder
+from .transformer import init_transformer_weights, TransformerEncoder
 
 
 def to_2tuple(x: int) -> Tuple[int, int]:

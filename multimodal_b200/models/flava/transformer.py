@@ -13,6 +13,7 @@ import torch
 from torch import nn, Tensor
 
 from ..._lib import MMBError
+from ...engine import _RuntimeOwner
 from ...modules.layers.attention import MultiHeadAttention, SelfAttention
 from ...modules.layers.mlp import MLP
 from ...modules.layers.normalizations import Fp32LayerNorm
@@ -69,22 +70,6 @@ def init_transformer_weights(module: nn.Module, initializer_range: float) -> Non
     elif isinstance(module, nn.LayerNorm):
         module.bias.data.zero_()
         module.weight.data.fill_(1.0)
-
-
-class _RuntimeOwner(nn.Module):
-    """Lazily (re)builds the module's fused runtime when the module moves or its parameters are replaced.  One runtime
-    serves both grad modes: forward + explicit backward under autograd, and the forward alone under torch.no_grad()."""
-
-    _runtime_cls = None
-
-    def _runtime(self, *extra: Optional[nn.Module]):
-        """`extra`: modules outside this one whose parameters its fused front end owns (the multimodal projections)."""
-        mods = [m for m in extra if m is not None]
-        ids = [(id(p), p.device) for m in (self, *mods) for p in m.parameters()]
-        if getattr(self, "_rt", None) is None or self._rt_ids != ids:
-            object.__setattr__(self, "_rt", type(self)._runtime_cls(self, *extra))
-            object.__setattr__(self, "_rt_ids", ids)
-        return self._rt
 
 
 class FLAVATransformerWithoutEmbeddings(_RuntimeOwner):

@@ -11,7 +11,8 @@ from typing import Callable, Optional
 import torch
 from torch import nn, Tensor
 
-from ...models.flava.transformer import _RuntimeOwner, TransformerEncoder
+from ...engine import _RuntimeOwner
+from ...models.flava.transformer import TransformerEncoder
 from ..layers.text_embedding import BERTTextEmbeddings
 from ..layers.transformer import TransformerOutput
 

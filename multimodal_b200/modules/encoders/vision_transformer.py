@@ -12,7 +12,7 @@ from typing import Any, Callable, Optional, Tuple, Union
 import torch
 from torch import nn, Tensor
 
-from ...models.flava.transformer import _RuntimeOwner
+from ...engine import _RuntimeOwner
 from ..layers.patch_embedding import PatchEmbeddings
 from ..layers.transformer import TransformerEncoder, TransformerOutput
 

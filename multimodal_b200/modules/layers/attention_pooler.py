@@ -8,7 +8,7 @@ from typing import List
 import torch
 from torch import nn, Tensor
 
-from ...models.flava.transformer import _RuntimeOwner
+from ...engine import _RuntimeOwner
 from .multi_head_attention import MultiHeadAttentionWithCache
 
 

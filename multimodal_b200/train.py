@@ -141,9 +141,10 @@ class ContrastiveTrainer:
         # with the image tower's persistent GEMM CTAs (bound by the L2 <-> SM path) instead of queueing behind them, and
         # each tower's kernels fill the other's tails.  Only kernels without shared scratch run concurrently (the fused
         # attention backward keeps its statistics in smem; the two-pass kernels share one D buffer -> S <= 256 only).
-        par = (self.tower_streams and mb == B and getattr(img, "S", 1 << 30) <= 256 and getattr(txt, "S", 1 << 30) <= 256)   # S is known after the first step
-        main = torch.cuda.current_stream(dev)
+        S_img = (image.shape[2] // img.ps) * (image.shape[3] // img.ps) + 1   # CLS + patches
+        par = self.tower_streams and mb == B and S_img <= 256 and text.shape[1] <= 256
         if par:
+            main = torch.cuda.current_stream(dev)
             if self._side is None:
                 self._side = torch.cuda.Stream(device=dev)
             side = self._side
@@ -151,20 +152,20 @@ class ContrastiveTrainer:
             ev.record(main)                      # inputs (and the previous optimizer step) are ordered before the side stream
             with torch.cuda.stream(side):
                 side.wait_event(ev)
-                eb = txt.forward(text, True)
+                (eb,), sb = txt.forward((text,), (), save=txt.ws)
                 ev_t = torch.cuda.Event()
                 ev_t.record(side)
-            ea = img.forward(image, True)
+            (ea,), sa = img.forward((image,), (), save=img.ws)
             main.wait_event(ev_t)
         elif mb == B:
-            ea = img.forward(image, True)
-            eb = txt.forward(text, True)
+            (ea,), sa = img.forward((image,), (), save=img.ws)
+            (eb,), sb = txt.forward((text,), (), save=txt.ws)
         else:
             ea = torch.empty((B, img.E), device=dev, dtype=f32)
             eb = torch.empty((B, txt.E), device=dev, dtype=f32)
             for i in range(0, B, mb):
-                img.forward(image[i:i + mb], False, out=ea[i:i + mb])
-                txt.forward(text[i:i + mb], False, out=eb[i:i + mb])
+                img.infer(image[i:i + mb], out=ea[i:i + mb])
+                txt.infer(text[i:i + mb], out=eb[i:i + mb])
         E = ea.shape[1]
         na, nb = torch.empty_like(ea), torch.empty_like(eb)
         ia, ib = torch.empty(B, device=dev, dtype=f32), torch.empty(B, device=dev, dtype=f32)
@@ -180,11 +181,11 @@ class ContrastiveTrainer:
         self._works = []
         if mb != B:
             for i in range(0, B, mb):                     # pass 2: re-forward with saving, back-propagate the slice
-                txt.forward(text[i:i + mb], True)
-                txt.backward(deb[i:i + mb])
+                sb = txt.forward((text[i:i + mb],), (), save=txt.ws)[1]   # the slice's embeddings are not kept
+                txt.backward(sb, deb[i:i + mb])
             for i in range(0, B, mb):
-                img.forward(image[i:i + mb], True)
-                img.backward(dea[i:i + mb])
+                sa = img.forward((image[i:i + mb],), (), save=img.ws)[1]
+                img.backward(sa, dea[i:i + mb])
             self._allreduce(txt.store.g)
             self._allreduce(img.store.g)
             bounds = None
@@ -193,16 +194,16 @@ class ContrastiveTrainer:
             ev.record(main)                      # deb is ready
             with torch.cuda.stream(self._side):
                 self._side.wait_event(ev)
-                txt.backward(deb)
+                txt.backward(sb, deb)
                 ev_t = torch.cuda.Event()
                 ev_t.record(self._side)
-            img.backward(dea)
+            img.backward(sa, dea)
             main.wait_event(ev_t)
             self._allreduce(txt.store.g)
             self._allreduce(img.store.g)
             bounds = None
         else:
-            txt.backward(deb)
+            txt.backward(sb, deb)
             if self.overlap_allreduce:
                 self._allreduce(txt.store.g)              # overlaps with the image tower's backward
             bounds = self._layer_boundaries(img) if (self.world > 1 and self.overlap_allreduce) else []
@@ -222,12 +223,10 @@ class ContrastiveTrainer:
                     self._allreduce(_st.g[lo:hi])
                     _state["hi"] -= 1
 
-            img.layer_done_cb = on_layer_done
-            img.backward(dea)
-            img.layer_done_cb = None
+            img.backward(sa, dea, on_layer_done=on_layer_done)
             self._allreduce(st.g[0:cuts[0]])
         else:
-            img.backward(dea)
+            img.backward(sa, dea)
             if not self.overlap_allreduce:
                 self._allreduce(txt.store.g)
             self._allreduce(img.store.g)

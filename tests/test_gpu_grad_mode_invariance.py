@@ -1,4 +1,5 @@
-"""The FLAVA and CoCa modules compute the same forward values under torch.no_grad() and with grad mode on, bit for bit.
+"""The CLIP, FLAVA and CoCa modules compute the same forward values under torch.no_grad() and with grad mode on, bit
+for bit.
 
 The inference and training runtimes launch the same kernels on the same operands (ops.self_attention picks the
 attention kernel for both); only the buffers that keep activations for the backward differ.  The cases are those of
@@ -57,12 +58,15 @@ def _outputs(name, dev):
         assert v.last_hidden_state.shape[1] == 400
         return {"last_hidden_state": v.last_hidden_state,
                 **{f"hidden_states.{i}": h for i, h in enumerate(v.hidden_states)}}
+    if name == "clip_small":
+        m, image, text = P._clip_small()
+        return P._clip_outputs(m.to(dev), image, text, dev)
     m, images, texts = P._coca_l14() if name == "coca_l14" else P._coca(name)
     return _coca_modules(m.to(dev), images, texts, dev)
 
 
 @pytest.mark.parametrize("name", ["flava_small", "flava_long", "flava_text512", "coca_small", "coca_parallel",
-                                  "coca_l14", "coca_vision_400"])
+                                  "coca_l14", "coca_vision_400", "clip_small"])
 def test_no_grad_equals_grad_mode_forward(name):
     dev = torch.device("cuda:0")
     with torch.no_grad():

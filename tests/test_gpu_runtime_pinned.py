@@ -1,8 +1,9 @@
-"""Pins the FLAVA and CoCa module forwards bit for bit, under torch.no_grad() and with grad mode on.
+"""Pins the CLIP, FLAVA and CoCa module forwards bit for bit, under torch.no_grad() and with grad mode on.
 
 Every tensor the inference forwards return is hashed: hidden states, pooler outputs, projected embeddings, attention
-probabilities, multimodal logits and both CoCa losses.  With grad mode on, the forwards run the training path, which
-also returns the losses and last hidden states pinned here (gradients are not: some backward kernels use fp32 atomics).
+probabilities, multimodal logits, both CoCa losses and the CLIP towers' embeddings and text hidden state.  With grad
+mode on, the forwards run the training path, which also returns the losses, last hidden states and CLIP embeddings
+pinned here (gradients are not: some backward kernels use fp32 atomics).
 The digests were recorded on an H100 80GB HBM3 by ``python tests/test_gpu_runtime_pinned.py``, which prints the table
 below.  Every shape stays outside 385-512 tokens of unmasked head_dim-64 self-attention, the band where the inference
 and training paths once chose different attention kernels.
@@ -161,8 +162,45 @@ def _vit_drop():
     return vit.train(), torch.randn(4, 3, 32, 32, generator=g)
 
 
+def _clip_small():
+    """A width-128, 2-layer CLIP (head_dim 64) with perturbed weights, and a batch of 6 image / text pairs."""
+    from multimodal_b200.models.clip.image_encoder import CLIPViTEncoder
+    from multimodal_b200.models.clip.model import CLIP
+    from multimodal_b200.models.clip.text_encoder import CLIPTextEncoder
+
+    torch.manual_seed(0)
+    m = CLIP(CLIPViTEncoder(64, 16, 64, 128, 2, 2),
+             CLIPTextEncoder(embedding_dim=64, vocab_size=512, width=128, dim_feedforward=512, heads=2, layers=2))
+    g = torch.Generator().manual_seed(3)
+    with torch.no_grad():
+        for p in m.parameters():
+            p.add_(0.03 * torch.randn(p.shape, generator=g))
+    B = 6
+    image = torch.randn(B, 3, 64, 64, generator=g)
+    text = torch.randint(1, 500, (B, 77), generator=g)
+    text[torch.arange(B), torch.randint(5, 77, (B,), generator=g)] = 511          # EOT = the largest id
+    return m.train(), image, text
+
+
+def _clip_outputs(m, image, text, dev):
+    """The embeddings of both CLIP towers."""
+    return {"image.embeddings": m.encoder_a(image.to(dev)), "text.embeddings": m.encoder_b(text.to(dev))}
+
+
 def _case(name, dev):
     """{output name: tensor} of one pinned forward."""
+    if name.startswith("clip_small"):
+        m, image, text = _clip_small()
+        m = m.to(dev)
+        if name.endswith("infer"):
+            with torch.no_grad():
+                res = _clip_outputs(m, image, text, dev)
+                res["text.hidden_state"] = m.encoder_b(text.to(dev), return_hidden_state=True)
+            return res
+        with torch.enable_grad():
+            res = _clip_outputs(m, image, text, dev)
+        assert all(t.requires_grad for t in res.values())
+        return res
     if name in ("coca_hd96.infer", "coca_hd128.infer"):
         vit, txt, images, ids = _head_dim_modules(96 if name == "coca_hd96.infer" else 128)
         with torch.no_grad():
@@ -219,7 +257,7 @@ def _case(name, dev):
 CASES = ["flava_small.infer", "flava_small.grad", "flava_long.infer", "flava_long.grad", "flava_attentions.infer",
          "flava_text512.infer", "flava_text512.grad", "coca_small.infer", "coca_small.grad", "coca_parallel.infer",
          "coca_parallel.grad", "coca_l14.infer", "coca_l14.grad", "text_decoder_no_cls.infer", "coca_hd96.infer",
-         "coca_hd128.infer", "vit_drop.infer"]
+         "coca_hd128.infer", "vit_drop.infer", "clip_small.infer", "clip_small.grad"]
 
 # {case: {output: sha256 of its bytes}}, recorded on an H100 80GB HBM3
 PINNED = {
@@ -426,6 +464,15 @@ PINNED = {
         'hidden_states.2': '(4, 49, 128) torch.float32 5202f2a331bb8808a3e879dd3d756a718057f0815799ff20ca43a4bc4487f704',
         'hidden_states.3': '(4, 49, 128) torch.float32 437ca8147ac89289541a23bbfbb3f044d382965d8854a1ca9b840259343effeb',
         'last_hidden_state': '(4, 49, 128) torch.float32 9a8695b5e151fd81289c90be6f254083b12d0c3e69e551b41920f0fe43f3d267',
+    },
+    'clip_small.infer': {
+        'image.embeddings': '(6, 64) torch.float32 37cf4a55f7b872b5ac1e7d732d658d269390e051db61cb5693e2a7d23372f4c4',
+        'text.embeddings': '(6, 64) torch.float32 f9b77915bf2430ad93236172cdc3d49aff5ca3a673eefda1c8df4c2da5f894e3',
+        'text.hidden_state': '(6, 77, 128) torch.float32 7d7a81ab171634ae070490a8272ee3c60279d4e9c834556c5913e3f11d93019d',
+    },
+    'clip_small.grad': {
+        'image.embeddings': '(6, 64) torch.float32 37cf4a55f7b872b5ac1e7d732d658d269390e051db61cb5693e2a7d23372f4c4',
+        'text.embeddings': '(6, 64) torch.float32 f9b77915bf2430ad93236172cdc3d49aff5ca3a673eefda1c8df4c2da5f894e3',
     },
 }
 

@@ -1,7 +1,8 @@
-"""One runtime per FLAVA / CoCa module serves both grad modes; these tests check, WITHOUT a GPU, that its torch.no_grad()
-entry point (no save Workspace, scratch shared by the layers) and its training forward (activations saved per call)
-compute the same bits, with the kernels swapped for their torch emulation (tests/emu_ops.py, with the stochastic-depth
-variants of tests/emu_drop_path_ops.py).  The same property on the kernels proper: tests/test_gpu_grad_mode_invariance.py."""
+"""One runtime per CLIP / FLAVA / CoCa module serves both grad modes; these tests check, WITHOUT a GPU, that its
+torch.no_grad() entry point (no save Workspace, scratch shared by the layers) and its training forward (activations
+saved per call) compute the same bits, with the kernels swapped for their torch emulation (tests/emu_ops.py, with the
+stochastic-depth variants of tests/emu_drop_path_ops.py).  The same property on the kernels proper:
+tests/test_gpu_grad_mode_invariance.py."""
 import pytest
 import torch
 
@@ -31,11 +32,11 @@ def _assert_grad_modes_agree(outputs):
     assert not differ, differ
 
 
-@pytest.mark.parametrize("name", list(FC.CASES) + list(CC.CASES))
+@pytest.mark.parametrize("name", list(FC.CASES) + list(CC.CASES) + ["clip_small"])
 def test_no_grad_forward_equals_training_forward(emu, name):
     """FLAVA: the image (patch mask), text (key-padding mask) and multimodal encoders of FLAVAModel; CoCa, one module at
     a time: vision encoder, poolers, text decoder ([B, S, S] causal x padding mask), multimodal decoder
-    (cross-attention)."""
+    (cross-attention); CLIP: both towers' embeddings."""
     _assert_grad_modes_agree(lambda: GI._outputs(name, CPU))
 
 
