@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import math
 import os
-
+from types import SimpleNamespace
 from typing import Dict, List, Optional, Sequence
 
 import torch
@@ -577,6 +577,120 @@ class TransformerStack:
             if on_layer_done is not None:
                 on_layer_done(l)  # all parameter gradients of layer l are final (data-parallel all-reduce hook)
         return G
+
+
+def _attention_parts(at: nn.Module):
+    """(separate q / k / v Linears or None when already packed, output Linear, head count) of a TorchMultimodal
+    attention module: packed `input_proj` (MultiHeadSelfAttention), `q_proj` / `k_proj` / `v_proj`
+    (MultiHeadAttentionWithCache) or FLAVA's `query` / `key` / `value` / `output` (MultiHeadAttention)."""
+    if hasattr(at, "input_proj"):
+        return None, at.output_proj, at.num_heads
+    if hasattr(at, "q_proj"):
+        return (at.q_proj, at.k_proj, at.v_proj), at.output_proj, at.num_heads
+    return (at.query, at.key, at.value), at.output, at.n_head
+
+
+def as_f32(t: Optional[torch.Tensor], shape) -> Optional[torch.Tensor]:
+    return None if t is None else t.contiguous().float().view(shape)
+
+
+class ModuleStack:
+    """ParamStore + TransformerStack over a list of TorchMultimodal pre-norm encoder / decoder layers
+    (modules/layers/transformer.py, models/flava/transformer.py), plus the final residual add and the gradient entering
+    the stack's backward.  The store holds every parameter of `owner` and `extra` (modules outside the owner whose
+    parameters its runtime uses); the separate q / k / v (and cross-attention k / v) projections go first, weights then
+    biases, so that they can be packed into one operand."""
+
+    def __init__(self, owner: nn.Module, layers, prefix: str, extra: Sequence[nn.Module] = (),
+                 fp32_only: Sequence[nn.Parameter] = ()):
+        layers = list(layers)
+        l0 = layers[0]
+        if not l0.norm_first:
+            raise MMBError("only pre-norm (norm_first=True) layers are on the accelerated path")
+        params: List[nn.Parameter] = []
+        for layer in layers:
+            qkv = _attention_parts(layer.attention)[0]
+            if qkv is not None:
+                params += [p.weight for p in qkv] + [p.bias for p in qkv]
+            ca = getattr(layer, "cross_attention", None)
+            if ca is not None:
+                params += [ca.k_proj.weight, ca.v_proj.weight, ca.k_proj.bias, ca.v_proj.bias]
+        seen = {id(p) for p in params}
+        for m in (owner, *extra):
+            for p in m.parameters():
+                if id(p) not in seen:
+                    seen.add(id(p))
+                    params.append(p)
+        self.store = st = ParamStore(params, fp32_only)
+        self.device = st.device
+        self.d = l0.attention_layernorm.normalized_shape[0]
+        self.ws = Workspace(self.device)   # scratch shared by all calls (stream-ordered)
+        adapters = []
+        for layer in layers:   # the attribute names TransformerStack reads (torch.nn.TransformerEncoderLayer layout)
+            mlp = layer.feedforward.model
+            qkv, out_proj, heads = _attention_parts(layer.attention)
+            if qkv is None:
+                w, b = layer.attention.input_proj.weight, layer.attention.input_proj.bias
+            else:
+                w, b = st.pack([p.weight for p in qkv]), st.pack([p.bias for p in qkv], fp32=True)
+            attn = SimpleNamespace(in_proj_weight=w, in_proj_bias=b, out_proj=out_proj, num_heads=heads)
+            ad = SimpleNamespace(self_attn=attn, norm1=layer.attention_layernorm, norm2=layer.feedforward_layernorm,
+                                 linear1=mlp[0], linear2=mlp[-1])
+            ca = getattr(layer, "cross_attention", None)
+            if ca is not None:
+                ad.cross_attn = SimpleNamespace(q_w=ca.q_proj.weight, q_b=ca.q_proj.bias,
+                                                kv_w=st.pack([ca.k_proj.weight, ca.v_proj.weight]),
+                                                kv_b=st.pack([ca.k_proj.bias, ca.v_proj.bias], fp32=True),
+                                                out_proj=ca.output_proj)
+                ad.norm_cross = layer.cross_attention_layernorm
+            adapters.append(ad)
+        self.stack = TransformerStack(adapters, st, self.ws, d=self.d, heads=_attention_parts(l0.attention)[2],
+                                      ff=l0.feedforward.model[0].weight.shape[0], act=act_code(l0.feedforward.model[1]),
+                                      prefix=prefix)
+        self.prefix = prefix
+        self.layers = layers     # the modules themselves: their StochasticDepth (drop_path_rate), if any
+
+    def finish(self, XM, Y, B: int, S: int, ln: Optional[nn.Module], save: Optional[Workspace], scales,
+               LASTb: Optional[torch.Tensor] = None):
+        """XF = XM + Y (the residual stream after the last layer; Y times the last MLP branch's stochastic-depth
+        factor when `scales` has one); LAST = ln(XF) when a final LayerNorm exists, and its bf16 copy into LASTb if
+        given.  XF / LAST are returned to the caller: allocated per call."""
+        d, pfx, M = self.d, self.prefix, B * S
+        f32 = torch.float32
+        stats = save if save is not None else self.ws
+        XF = torch.empty((M, d), device=self.device, dtype=f32)
+        LAST = torch.empty((M, d), device=self.device, dtype=f32) if ln is not None else None
+        aff = ln if ln is not None else self.stack.layers[0].norm1   # affine terms unused when nothing is normalised
+        ops.add_layernorm_fwd(XM, Y, XF, LASTb, LAST, aff.weight, aff.bias,
+                              stats.get(f"{pfx}.mF", (M,), f32) if ln is not None else None,
+                              stats.get(f"{pfx}.rF", (M,), f32) if ln is not None else None, M, d, aff.eps,
+                              **scaled(scales[-1][1] if scales is not None else None, S))
+        if save is not None:
+            save.XF = XF
+        return XF, LAST
+
+    def start_backward(self, save: Workspace, M: int, ln: Optional[nn.Module], dLAST, dXF):
+        """(G fp32, Gb bf16, top_bias_done): gradient w.r.t. XF entering the stack's backward; Gb is the gradient
+        entering the last MLP branch (scaled by its stochastic-depth factor, if any).  With a final LayerNorm and a
+        gradient of LAST or XF, the LayerNorm backward adds both (a missing dLAST counts as zero)."""
+        d, pfx, st = self.d, self.prefix, self.store
+        f32, bf = torch.float32, torch.bfloat16
+        G = self.ws.get(f"{pfx}.G", (M, d), f32)
+        Gb = self.ws.get(f"{pfx}.Gb", (M, d), bf)
+        scale, rows = self.stack.top_scale(save)
+        if ln is not None and (dLAST is not None or dXF is not None):
+            if dLAST is None:   # only XF was used downstream
+                dLAST = torch.zeros((M, d), device=self.device, dtype=f32)
+            ops.layernorm_bwd(save.XF, None, dLAST, save.get(f"{pfx}.mF", (M,), f32), save.get(f"{pfx}.rF", (M,), f32),
+                              ln.weight, dXF, G, Gb, st.grad(ln.weight), st.grad(ln.bias), M, d,
+                              gsum=self.stack.top_bias_grad(), **scaled(scale, rows))
+            return G, Gb, True
+        if dXF is None:
+            ops.zero_(G)
+        else:
+            G.copy_(dXF.view(M, d))      # the stack's backward works in place on G
+        ops.cast_bf16(G, Gb, **scaled(scale, rows))
+        return G, Gb, False
 
 
 class ViTTower:

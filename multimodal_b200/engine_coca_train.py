@@ -3,7 +3,8 @@ for both grad modes: forwards that keep what the backward needs + explicit backw
 Functions, so that `CoCaModel` / `CoCaForPretraining` train with ``loss.backward()`` like the reference
 (models/coca/coca_model.py:69-130, 398-454 under autograd); under torch.no_grad() the same forwards keep nothing.
 
-All layer stacks run on ``engine.TransformerStack`` (the CLIP towers' fused schedule and kernels):
+All layer stacks run on ``engine.TransformerStack`` (the CLIP towers' fused schedule and kernels) through
+``engine.ModuleStack``, which also owns the parameter store, the final residual add and the backward's entry:
   vision encoder      : packed `input_proj` self-attention (tensor-core fwd / bwd), erf-GELU MLP, optional final LayerNorm
                         (modules/encoders/vision_transformer.py:56-89, patch_embedding.py:104-154)
   text decoder        : separate q / k / v projections presented as one packed operand, the [B, S, S] causal x padding
@@ -22,126 +23,16 @@ Every training forward keeps its activations in its own Workspace (held by the a
 from __future__ import annotations
 
 import math
-from types import SimpleNamespace
-from typing import List, Optional, Sequence
+from typing import List, Optional
 
 import torch
 from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import (ParamStore, TransformerStack, Workspace, act_code, patch_embed_bwd, patch_embed_fwd, run,
-                     scaled)
+from .engine import ModuleStack, ParamStore, Workspace, as_f32, patch_embed_bwd, patch_embed_fwd
 from .modules.layers.stochastic_depth import drop_path_scales
 from .modules.masking.random_masking import patch_keep_indices
-
-
-def _qkv_first(layers) -> List[nn.Parameter]:
-    """Parameter order that makes the separate q / k / v (and cross k / v) projections packable."""
-    out: List[nn.Parameter] = []
-    for layer in layers:
-        at = layer.attention
-        if not hasattr(at, "input_proj"):
-            out += [at.q_proj.weight, at.k_proj.weight, at.v_proj.weight, at.q_proj.bias, at.k_proj.bias, at.v_proj.bias]
-        ca = getattr(layer, "cross_attention", None)
-        if ca is not None:
-            out += [ca.k_proj.weight, ca.v_proj.weight, ca.k_proj.bias, ca.v_proj.bias]
-    return out
-
-
-def _store_for(owner: nn.Module, first: Sequence[nn.Parameter], fp32_only: Sequence[nn.Parameter] = ()) -> ParamStore:
-    params, seen = list(first), {id(p) for p in first}
-    for p in owner.parameters():
-        if id(p) not in seen:
-            seen.add(id(p))
-            params.append(p)
-    return ParamStore(params, fp32_only)
-
-
-def _adapters(layers, st: ParamStore):
-    out = []
-    for layer in layers:
-        at, mlp = layer.attention, layer.feedforward.model
-        if hasattr(at, "input_proj"):     # MultiHeadSelfAttention: already packed [3d, d]
-            attn = SimpleNamespace(in_proj_weight=at.input_proj.weight, in_proj_bias=at.input_proj.bias,
-                                   out_proj=at.output_proj, num_heads=at.num_heads)
-        else:
-            attn = SimpleNamespace(in_proj_weight=st.pack([at.q_proj.weight, at.k_proj.weight, at.v_proj.weight]),
-                                   in_proj_bias=st.pack([at.q_proj.bias, at.k_proj.bias, at.v_proj.bias], fp32=True),
-                                   out_proj=at.output_proj, num_heads=at.num_heads)
-        ad = SimpleNamespace(self_attn=attn, norm1=layer.attention_layernorm, norm2=layer.feedforward_layernorm,
-                             linear1=mlp[0], linear2=mlp[-1])
-        ca = getattr(layer, "cross_attention", None)
-        if ca is not None:
-            ad.cross_attn = SimpleNamespace(q_w=ca.q_proj.weight, q_b=ca.q_proj.bias,
-                                            kv_w=st.pack([ca.k_proj.weight, ca.v_proj.weight]),
-                                            kv_b=st.pack([ca.k_proj.bias, ca.v_proj.bias], fp32=True),
-                                            out_proj=ca.output_proj)
-            ad.norm_cross = layer.cross_attention_layernorm
-        out.append(ad)
-    return out
-
-
-class _Stack:
-    """ParamStore + TransformerStack over a list of TorchMultimodal pre-norm encoder / decoder layers."""
-
-    def __init__(self, owner: nn.Module, layers, prefix: str, fp32_only: Sequence[nn.Parameter] = ()):
-        layers = list(layers)
-        l0 = layers[0]
-        if not l0.norm_first:
-            raise MMBError("only pre-norm (norm_first=True) layers are on the accelerated path")
-        self.store = _store_for(owner, _qkv_first(layers), fp32_only)
-        self.device = self.store.device
-        self.d = l0.attention_layernorm.normalized_shape[0]
-        self.ws = Workspace(self.device)
-        self.stack = TransformerStack(_adapters(layers, self.store), self.store, self.ws, d=self.d,
-                                      heads=l0.attention.num_heads, ff=l0.feedforward.model[0].weight.shape[0],
-                                      act=act_code(l0.feedforward.model[1]), prefix=prefix)
-        self.prefix, self.L = prefix, len(layers)
-        self.layers = layers     # the modules themselves: their StochasticDepth (drop_path_rate), if any
-
-    def finish(self, XM, Y, B: int, S: int, ln: Optional[nn.Module], save: Optional[Workspace], scales,
-               LASTb: Optional[torch.Tensor] = None):
-        """XF = XM + Y (the residual stream after the last layer; Y times the last MLP branch's stochastic-depth
-        factor when `scales` has one); LAST = ln(XF) when a final LayerNorm exists, and its bf16 copy into LASTb if
-        given.  XF / LAST are returned to the caller: allocated per call."""
-        d, pfx, M = self.d, self.prefix, B * S
-        f32 = torch.float32
-        stats = save if save is not None else self.ws
-        XF = torch.empty((M, d), device=self.device, dtype=f32)
-        LAST = torch.empty((M, d), device=self.device, dtype=f32) if ln is not None else None
-        aff = ln if ln is not None else self.stack.layers[0].norm1   # affine terms unused when nothing is normalised
-        ops.add_layernorm_fwd(XM, Y, XF, LASTb, LAST, aff.weight, aff.bias,
-                              stats.get(f"{pfx}.mF", (M,), f32) if ln is not None else None,
-                              stats.get(f"{pfx}.rF", (M,), f32) if ln is not None else None, M, d, aff.eps,
-                              **scaled(scales[-1][1] if scales is not None else None, S))
-        if save is not None:
-            save.XF = XF
-        return XF, LAST
-
-    def start_backward(self, save: Workspace, M: int, ln: Optional[nn.Module], dLAST, dXF):
-        """(G fp32, Gb bf16, top_bias_done): gradient w.r.t. XF entering the stack's backward; Gb is the gradient
-        entering the last MLP branch (scaled by its stochastic-depth factor, if any)."""
-        d, pfx, st = self.d, self.prefix, self.store
-        f32, bf = torch.float32, torch.bfloat16
-        G = self.ws.get(f"{pfx}.G", (M, d), f32)
-        Gb = self.ws.get(f"{pfx}.Gb", (M, d), bf)
-        scale, rows = self.stack.top_scale(save)
-        if ln is not None and dLAST is not None:
-            ops.layernorm_bwd(save.XF, None, dLAST, save.get(f"{pfx}.mF", (M,), f32), save.get(f"{pfx}.rF", (M,), f32),
-                              ln.weight, dXF, G, Gb, st.grad(ln.weight), st.grad(ln.bias), M, d,
-                              gsum=self.stack.top_bias_grad(), **scaled(scale, rows))
-            return G, Gb, True
-        if dXF is None:
-            ops.zero_(G)
-        else:
-            G.copy_(dXF.view(M, d))      # the stack's backward works in place on G
-        ops.cast_bf16(G, Gb, **scaled(scale, rows))
-        return G, Gb, False
-
-
-def _f32(t: Optional[torch.Tensor], shape) -> Optional[torch.Tensor]:
-    return None if t is None else t.contiguous().float().view(shape)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -154,10 +45,11 @@ class VisionTrainRuntime:
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.s = _Stack(mod, mod.encoder.layer, "cvit")
+        self.s = ModuleStack(mod, mod.encoder.layer, "cvit")
         self.store = self.s.store
 
-    def _forward(self, images, image_patches_mask, save: Optional[Workspace]):
+    def _forward(self, images, image_patches_mask, save: Optional[Workspace], hidden: List[torch.Tensor]):
+        """hidden: receives hidden_states (X0, each layer's output, XF)."""
         emb, s, st = self.mod.embeddings, self.s, self.store
         d, conv = s.d, emb.conv_projection
         st.refresh()
@@ -168,23 +60,23 @@ class VisionTrainRuntime:
                                           emb.cls_token if emb.include_cls_embed else None, emb.position_embeddings,
                                           emb.mask_token, image_patches_mask, s.ws, save if save is not None else s.ws,
                                           "cvit", keep=keep)
-        hidden: List[torch.Tensor] = []
         XM, Y = s.stack.forward(X0, B, S, save, scales=scales, hidden=hidden)
         XF, LAST = s.finish(XM, Y, B, S, self.mod.encoder.final_layer_norm, save, scales)
         hidden.append(XF.view(B, S, d))
-        return (LAST if LAST is not None else XF), hidden, (B, S, P, pm, keep)
+        return (LAST if LAST is not None else XF), (B, S, P, pm, keep)
 
     def forward(self, data, diff):
-        images, image_patches_mask = data
+        """data: (images, image_patches_mask, the caller's list that receives hidden_states)."""
+        images, image_patches_mask, hidden = data
         save = Workspace(self.s.device)
-        last, self.last_hidden, (save.B, save.S, save.P, save.pm, save.keep) = self._forward(images, image_patches_mask,
-                                                                                               save)
+        last, (save.B, save.S, save.P, save.pm, save.keep) = self._forward(images, image_patches_mask, save, hidden)
         return (last,), save
 
     def infer(self, images, image_patches_mask=None):
         from .modules.layers.transformer import TransformerOutput
 
-        last, hidden, _ = self._forward(images, image_patches_mask, None)
+        hidden: List[torch.Tensor] = []
+        last, _ = self._forward(images, image_patches_mask, None, hidden)
         return TransformerOutput(last_hidden_state=last.view(hidden[-1].shape), pooler_output=None, hidden_states=hidden,
                                  attentions=None)
 
@@ -193,7 +85,7 @@ class VisionTrainRuntime:
         d, B, S = s.d, save.B, save.S
         M = B * S
         fln = self.mod.encoder.final_layer_norm
-        dOUT = _f32(dOUT, (M, d))
+        dOUT = as_f32(dOUT, (M, d))
         G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
         G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
         patch_embed_bwd(G, emb.conv_projection, emb.cls_token if emb.include_cls_embed else None,
@@ -210,8 +102,8 @@ class PoolerTrainRuntime:
     def __init__(self, mod: nn.Module):
         self.mod = mod
         at = mod.attn
-        self.store = _store_for(mod, [at.k_proj.weight, at.v_proj.weight, at.k_proj.bias, at.v_proj.bias])
-        st = self.store
+        kv = [at.k_proj.weight, at.v_proj.weight, at.k_proj.bias, at.v_proj.bias]   # first: packable
+        self.store = st = ParamStore(kv + [p for p in mod.parameters() if all(p is not q for q in kv)])
         self.kv_w = st.pack([at.k_proj.weight, at.v_proj.weight])
         self.kv_b = st.pack([at.k_proj.bias, at.v_proj.bias], fp32=True)
         self.ws = Workspace(st.device)
@@ -277,7 +169,7 @@ class PoolerTrainRuntime:
         n = B * nq
         g = lambda name, shape, dt: save.get(name, shape, dt)  # noqa: E731
         dYb = self.ws.get("dYb", (n, dout), bf)
-        ops.layernorm_bwd(g("Y32", (n, dout), f32), None, _f32(dOUT, (n, dout)), g("mp", (n,), f32), g("rp", (n,), f32),
+        ops.layernorm_bwd(g("Y32", (n, dout), f32), None, as_f32(dOUT, (n, dout)), g("mp", (n,), f32), g("rp", (n,), f32),
                           m.ln_post.weight, None, None, dYb, st.grad(m.ln_post.weight), st.grad(m.ln_post.bias), n, dout,
                           gsum=st.grad(at.output_proj.bias))
         O, KV = g("O", (n, dout), bf), g("KV", (B * S, 2 * dout), bf)
@@ -316,7 +208,7 @@ class TextDecoderTrainRuntime:
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.s = _Stack(mod, mod.transformer_decoder.layer, "ctxt", fp32_only=list(mod.embeddings.parameters()))
+        self.s = ModuleStack(mod, mod.transformer_decoder.layer, "ctxt", fp32_only=list(mod.embeddings.parameters()))
         self.store = self.s.store
         self._idx = None
 
@@ -390,11 +282,11 @@ class TextDecoderTrainRuntime:
         M = B * S
         bf, f32 = torch.bfloat16, torch.float32
         emb = m.embeddings
-        G, Gb, _ = s.start_backward(save, M, None, None, _f32(dXF, (M, d)))
+        G, Gb, _ = s.start_backward(save, M, None, None, as_f32(dXF, (M, d)))
         if dpooled is not None:
             ln = getattr(m, "ln_final", None)
             W = m.text_projection.weight
-            dPb = ops.cast_bf16(_f32(dpooled, (B, W.shape[0])))
+            dPb = ops.cast_bf16(as_f32(dpooled, (B, W.shape[0])))
             POOLb = save.get("ctxt.POOLb", (B, d), bf)
             ops.gemm(dPb, POOLb, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(W), accumulate=True)
             dL = torch.empty((B, d), device=s.device, dtype=f32)
@@ -424,7 +316,7 @@ class MultimodalDecoderTrainRuntime:
 
     def __init__(self, mod: nn.Module):
         self.mod = mod
-        self.s = _Stack(mod, mod.transformer_decoder.layer, "cmm")
+        self.s = ModuleStack(mod, mod.transformer_decoder.layer, "cmm")
         self.store = self.s.store
 
     def _forward(self, texts, images, save: Optional[Workspace], want_bf16: bool = False):
@@ -480,7 +372,7 @@ class MultimodalDecoderTrainRuntime:
         d, B, S = s.d, save.B, save.S
         M = B * S
         fln = self.mod.transformer_decoder.final_layer_norm
-        dOUT = _f32(dOUT, (M, d))
+        dOUT = as_f32(dOUT, (M, d))
         G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
         G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
         return (G.view(B, S, d).clone(), save.dENC.view(B, save.Si, save.dv))
@@ -601,53 +493,3 @@ def linear_f32(x: torch.Tensor, linear: nn.Linear) -> torch.Tensor:
 def linear_cross_entropy(hidden: torch.Tensor, linear: nn.Linear, labels: torch.Tensor, ignore_index: int) -> torch.Tensor:
     return LinearCrossEntropyFunction.apply(hidden.reshape(-1, hidden.shape[-1]), linear.weight, linear.bias, labels,
                                             ignore_index)
-
-
-class LayersTrainRuntime:
-    """A standalone pre-norm `TransformerEncoderLayer` or `TransformerEncoder` (modules/layers/transformer.py:31-259) called
-    on its own under autograd: hidden_states [B, S, d] in (differentiable), residual stream (and final LayerNorm) out."""
-
-    def __init__(self, owner: nn.Module, layers, final_ln: Optional[nn.Module]):
-        self.s = _Stack(owner, layers, "lyr")
-        self.store = self.s.store
-        self.final_ln = final_ln
-
-    def forward(self, data, diff):
-        (mask_u8,) = data
-        (x,) = diff
-        s = self.s
-        B, S, d = x.shape
-        self.store.refresh()
-        save = Workspace(s.device)
-        X0 = torch.empty((B * S, d), device=s.device, dtype=torch.float32)
-        X0.view(B, S, d).copy_(x)
-        scales = drop_path_scales(s.layers, B, s.device)
-        hidden: List[torch.Tensor] = []
-        XM, Y = s.stack.forward(X0, B, S, save, mask3=mask_u8, scales=scales, hidden=hidden)
-        XF, LAST = s.finish(XM, Y, B, S, self.final_ln, save, scales)
-        save.B, save.S = B, S
-        self.last_hidden = hidden + [XF.view(B, S, d)]
-        return ((LAST if LAST is not None else XF),), save
-
-    def backward(self, save, dOUT):
-        s = self.s
-        d, B, S = s.d, save.B, save.S
-        M = B * S
-        fln = self.final_ln
-        dOUT = _f32(dOUT, (M, d))
-        G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
-        G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
-        return (G.view(B, S, d).clone(),)
-
-
-def standalone_layers(owner: nn.Module, layers, final_ln, hidden_states: torch.Tensor, mask_u8):
-    """-> (output [B, S, d] with autograd history, hidden_states list) for a standalone layer / encoder call."""
-    ids = [(id(p), p.device) for p in owner.parameters()]
-    rt = getattr(owner, "_mmb_trt", None)
-    if rt is None or getattr(owner, "_mmb_trt_ids", None) != ids:
-        rt = LayersTrainRuntime(owner, layers, final_ln)
-        object.__setattr__(owner, "_mmb_trt", rt)
-        object.__setattr__(owner, "_mmb_trt_ids", ids)
-    (out,) = run(rt, (mask_u8,), (hidden_states.float(),))
-    hidden, rt.last_hidden = rt.last_hidden, None
-    return out.view(hidden_states.shape), hidden

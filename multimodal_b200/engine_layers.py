@@ -8,9 +8,10 @@ exposes — and tests — on their own are callable outside an encoder:
 
 They launch exactly the kernels the fused encoder schedules launch (wgmma GEMMs with bias / activation epilogues,
 tensor-core attention, the add+LayerNorm kernel); nothing is computed by PyTorch.  Pre-norm `TransformerEncoderLayer` /
-`TransformerEncoder` also train on their own (grad mode on: `engine_coca_train.LayersTrainRuntime`, the CLIP towers' fused
-forward / backward schedule); the other standalone modules compute forward values only, and asking them for an autograd
-graph raises instead of returning detached tensors.
+`TransformerEncoder` run on one runtime per module in both grad modes (`EncoderLayersRuntime` on `engine.ModuleStack`:
+the CLIP towers' fused forward / backward schedule, `infer` under torch.no_grad()); the other standalone modules,
+post-norm layers included, compute forward values only, and asking them for an autograd graph raises instead of
+returning detached tensors.
   modules/layers/multi_head_attention.py:83-180  MultiHeadAttentionWithCache (key / value cache, cross-attention)
   modules/layers/transformer.py:262-657          TransformerDecoderLayer (pre- and post-norm), TransformerDecoder
 
@@ -23,14 +24,15 @@ Autoregressive decoding (queries of at most 16 rows over a key / value cache) ru
 from __future__ import annotations
 
 import math
-from typing import Optional
+from typing import List, Optional
 
 import torch
 from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import Workspace, _Shadows, act_code, patch_embed_fwd, scaled
+from .engine import ModuleStack, Workspace, _Shadows, act_code, as_f32, patch_embed_fwd, run, scaled
+from .modules.layers.stochastic_depth import drop_path_scales
 
 
 def forward_only_guard(mod: nn.Module, what: str) -> None:
@@ -130,20 +132,85 @@ def mlp_forward(mod: nn.Module, x: torch.Tensor) -> torch.Tensor:
     return out.view(*x.shape[:-1], dout).to(x.dtype)
 
 
+class EncoderLayersRuntime:
+    """A standalone pre-norm `TransformerEncoderLayer` or `TransformerEncoder` (modules/layers/transformer.py:31-259) in
+    both grad modes: hidden_states [B, S, d] in, the residual stream after the last layer (and the final LayerNorm, if
+    any) out.  `forward(data, diff)` / `backward` run under autograd (engine.run), `infer` under torch.no_grad()."""
+
+    def __init__(self, owner: nn.Module, layers, final_ln: Optional[nn.Module]):
+        self.s = ModuleStack(owner, layers, "lyr")
+        self.store = self.s.store
+        self.final_ln = final_ln
+
+    def _forward(self, x: torch.Tensor, mask_u8, save: Optional[Workspace], hidden: Optional[List[torch.Tensor]]):
+        s = self.s
+        B, S, d = x.shape
+        self.store.refresh()
+        if save is None:
+            X0 = x.contiguous().float().view(B * S, d)      # only read
+        else:
+            X0 = torch.empty((B * S, d), device=s.device, dtype=torch.float32)
+            X0.view(B, S, d).copy_(x)    # the backward reads it: a copy the caller cannot change
+        scales = drop_path_scales(s.layers, B, s.device)   # training with drop_path_rate: once, for all layers
+        XM, Y = s.stack.forward(X0, B, S, save, mask3=mask_u8, scales=scales, hidden=hidden)
+        XF, LAST = s.finish(XM, Y, B, S, self.final_ln, save, scales)
+        if hidden is not None:
+            hidden.append(XF.view(B, S, d))
+        return LAST if LAST is not None else XF
+
+    def forward(self, data, diff):
+        """data: (uint8 [B, S, S] mask or None, the caller's list that receives hidden_states or None)."""
+        mask_u8, hidden = data
+        (x,) = diff
+        save = Workspace(self.s.device)
+        out = self._forward(x, mask_u8, save, hidden)
+        save.B, save.S = x.shape[:2]
+        return (out,), save
+
+    def infer(self, x: torch.Tensor, mask_u8: Optional[torch.Tensor], return_hidden_states: bool = False):
+        """-> (output [B, S, d], hidden_states or None), in x's dtype.  hidden_states[0] is x itself; the others are
+        fresh tensors, the last one before the final LayerNorm."""
+        hidden: Optional[List[torch.Tensor]] = [] if return_hidden_states else None
+        out = self._forward(x, mask_u8, None, hidden)
+        if hidden is not None:
+            hidden = [x] + [h.to(x.dtype) for h in hidden[1:]]
+        return out.view(x.shape).to(x.dtype), hidden
+
+    def backward(self, save, dOUT):
+        s = self.s
+        d, B, S = s.d, save.B, save.S
+        M = B * S
+        fln = self.final_ln
+        dOUT = as_f32(dOUT, (M, d))
+        G, Gb, done = s.start_backward(save, M, fln, dOUT if fln is not None else None, None if fln is not None else dOUT)
+        G = s.stack.backward(G, Gb, B, S, top_bias_done=done, save=save)
+        return (G.view(B, S, d).clone(),)
+
+
+def _pre_norm_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask: Optional[torch.Tensor], what: str,
+                      return_hidden_states: bool = False):
+    """A pre-norm TransformerEncoderLayer / TransformerEncoder on its EncoderLayersRuntime -> (output, hidden_states or
+    None).  With an autograd graph the output is fp32."""
+    B, S, _ = hidden_states.shape
+    if _wants_graph(mod, hidden_states):
+        hidden = [] if return_hidden_states else None
+        (out,) = run(mod._runtime(), (_bool_mask_u8(attention_mask, B, S, what), hidden), (hidden_states.float(),))
+        return out.view(hidden_states.shape), hidden
+    _cuda(hidden_states, what)
+    with torch.no_grad():
+        return mod._runtime().infer(hidden_states, _bool_mask_u8(attention_mask, B, S, what), return_hidden_states)
+
+
 def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
                           attention_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """TransformerEncoderLayer.forward (transformer.py:95-154), pre-norm (:95-111) and post-norm (:113-128).  With a
-    drop_path_rate in training, each branch is scaled per sample inside the residual add that follows it."""
-    from .modules.layers.stochastic_depth import drop_path_scales
-
+    """TransformerEncoderLayer.forward (transformer.py:95-154): pre-norm (:95-111) on its runtime, post-norm
+    (:113-128) forward-only.  With a drop_path_rate in training, each branch is scaled per sample inside the residual
+    add that follows it."""
+    if mod.norm_first:
+        return _pre_norm_forward(mod, hidden_states, attention_mask, "TransformerEncoderLayer")[0]
     if _wants_graph(mod, hidden_states):
-        if not mod.norm_first:
-            raise MMBError("standalone post-norm TransformerEncoderLayer has no backward schedule; call it under "
-                           "torch.no_grad()")
-        from .engine_coca_train import standalone_layers
-        B, S, _ = hidden_states.shape
-        return standalone_layers(mod, [mod], None, hidden_states,
-                                 _bool_mask_u8(attention_mask, B, S, "TransformerEncoderLayer"))[0]
+        raise MMBError("standalone post-norm TransformerEncoderLayer has no backward schedule; call it under "
+                       "torch.no_grad()")
     _cuda(hidden_states, "TransformerEncoderLayer")
     B, S, d = hidden_states.shape
     at, mlp = mod.attention, mod.feedforward.model
@@ -167,47 +234,29 @@ def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
     out = torch.empty((M, d), device=X.device, dtype=f32)
     scales = drop_path_scales([mod], B, X.device)
     s_attn, s_ff = scales[0] if scales is not None else (None, None)
-    if mod.norm_first:
-        ops.add_layernorm_fwd(X, None, None, LN, None, ln1.weight, ln1.bias, None, None, M, d, ln1.eps)
-        ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
-        ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
-        ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
-        XM = ws.get("l.XM", (M, d), f32)                       # x + attention(LN(x)); LN2 of it for the MLP
-        ops.add_layernorm_fwd(X, Y, XM, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
-                              **scaled(s_attn, S))
-        ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
-        ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
-        # out = XM + mlp: the add kernel with an identity-free LayerNorm is not needed — reuse add+LN writing only x_out
-        ops.add_layernorm_fwd(XM, Y, out, LN, None, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
-                              **scaled(s_ff, S))
-    else:
-        ops.cast_bf16(X.view(-1), LN.view(-1))                 # attention(x) on the raw input
-        ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
-        ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
-        ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
-        H1 = ws.get("l.H1", (M, d), f32)                       # LN1(x + attention(x)), fp32 + its bf16 operand copy
-        ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps,
-                              **scaled(s_attn, S))
-        ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
-        ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
-        ops.add_layernorm_fwd(H1, Y, None, None, out, ln2.weight, ln2.bias, None, None, M, d, ln2.eps,
-                              **scaled(s_ff, S))
+    ops.cast_bf16(X.view(-1), LN.view(-1))                 # attention(x) on the raw input
+    ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
+    ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
+    ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
+    H1 = ws.get("l.H1", (M, d), f32)                       # LN1(x + attention(x)), fp32 + its bf16 operand copy
+    ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps, **scaled(s_attn, S))
+    ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
+    ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
+    ops.add_layernorm_fwd(H1, Y, None, None, out, ln2.weight, ln2.bias, None, None, M, d, ln2.eps, **scaled(s_ff, S))
     return out.view(B, S, d).to(hidden_states.dtype)
 
 
 def encoder_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
                     return_hidden_states: bool = False):
-    """TransformerEncoder.forward (transformer.py:216-259): the layers (+ optional final LayerNorm)."""
+    """TransformerEncoder.forward (transformer.py:216-259): the layers (+ optional final LayerNorm); pre-norm on the
+    encoder's runtime, post-norm forward-only, one layer at a time."""
     from .modules.layers.transformer import TransformerOutput
 
+    if all(layer.norm_first for layer in mod.layer):
+        out, hidden = _pre_norm_forward(mod, hidden_states, attention_mask, "TransformerEncoder", return_hidden_states)
+        return TransformerOutput(last_hidden_state=out, hidden_states=hidden)
     if _wants_graph(mod, hidden_states):
-        if not all(layer.norm_first for layer in mod.layer):
-            raise MMBError("standalone post-norm TransformerEncoder has no backward schedule; call it under torch.no_grad()")
-        from .engine_coca_train import standalone_layers
-        B, S, _ = hidden_states.shape
-        out, hidden = standalone_layers(mod, mod.layer, mod.final_layer_norm, hidden_states,
-                                        _bool_mask_u8(attention_mask, B, S, "TransformerEncoder"))
-        return TransformerOutput(last_hidden_state=out, hidden_states=hidden if return_hidden_states else None)
+        raise MMBError("standalone post-norm TransformerEncoder has no backward schedule; call it under torch.no_grad()")
     _cuda(hidden_states, "TransformerEncoder")
     x = hidden_states
     all_hidden = [x] if return_hidden_states else None

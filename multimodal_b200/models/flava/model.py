@@ -149,7 +149,7 @@ class FLAVAModel(nn.Module):
         if torch.is_grad_enabled() and (out.last_hidden_state.requires_grad or wants_grad(linear)):
             return T.first_token_linear(out.last_hidden_state, linear)
         with torch.no_grad():
-            return encoder._runtime().ts.project_first_token(out.last_hidden_state, linear, key)
+            return encoder._runtime().project_first_token(out.last_hidden_state, linear, key)
 
     def _encode_data_to_embeddings(self, data: Optional[Tensor], selected_head_encoder: str, encoder_options: List[str],
                                    encode_callable: Callable[..., Any]) -> Any:
@@ -166,7 +166,7 @@ class FLAVAModel(nn.Module):
         enc, ip, tp = self.mm_encoder, self.image_to_mm_projection, self.text_to_mm_projection
         if wants_grad(enc, ip, tp) or (torch.is_grad_enabled() and
                                           (image_embedding.requires_grad or text_embedding.requires_grad)):
-            return T.encoder_output(enc._runtime(ip, tp), None, (image_embedding, text_embedding), enc.pooler)
+            return T.encoder_output(enc._runtime(ip, tp), (), (image_embedding, text_embedding), enc.pooler)
         with torch.no_grad():
             return enc._runtime(ip, tp).infer(image_embedding, text_embedding,
                                               want_attn=bool(getattr(enc, "output_attentions", False)))

@@ -98,7 +98,7 @@ class FLAVATransformerWithoutEmbeddings(_RuntimeOwner):
         from ... import engine_flava_train as T
         from ...engine import wants_grad
         if wants_grad(self) or (torch.is_grad_enabled() and hidden_states.requires_grad):
-            return T.encoder_output(self._runtime(), None, (hidden_states,), self.pooler)
+            return T.encoder_output(self._runtime(), (), (hidden_states,), self.pooler)
         with torch.no_grad():
             return self._runtime().infer(hidden_states, want_attn=bool(getattr(self, "output_attentions", False)))
 

@@ -40,9 +40,8 @@ class VisionTransformer(_RuntimeOwner):
             warnings.warn("image_patches_mask passed but use_image_masking in init was false. Ignoring.")
         from ...engine import run, wants_grad
         if wants_grad(self):   # training: forward keeps activations, the autograd node carries the explicit backward
-            rt = self._runtime()
-            (last,) = run(rt, (images, image_patches_mask), ())
-            hidden, rt.last_hidden = rt.last_hidden, None
+            hidden = []
+            (last,) = run(self._runtime(), (images, image_patches_mask, hidden), ())
             B, S, d = hidden[0].shape
             out = TransformerOutput(last_hidden_state=last.view(B, S, d), pooler_output=None, hidden_states=hidden,
                                     attentions=None)

@@ -2,7 +2,9 @@
 CoCa encoder returns) and the parameter containers `TransformerEncoderLayer` / `TransformerEncoder` (:31-259) and
 `TransformerDecoderLayer` / `TransformerDecoder` (:262-657) — same constructors, state-dict keys and creation order.
 The layers execute inside `engine.TransformerStack` (fused kernels), owned by VisionTransformer / CoCaTextDecoder /
-CoCaMultimodalDecoder; all four are also callable on their own (forward values, same kernels: `engine_layers.py`), the
+CoCaMultimodalDecoder; all four are also callable on their own (same kernels: `engine_layers.py`).  A pre-norm
+`TransformerEncoderLayer` / `TransformerEncoder` is then a runtime owner like the encoders: one runtime on its own
+`TransformerStack` serves torch.no_grad() and training.  Post-norm layers and the decoders compute forward values, the
 decoders with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive decoding.
 
 With `drop_path_rate` an encoder layer applies stochastic depth as the reference does: one shared
@@ -14,6 +16,8 @@ from typing import Callable, List, NamedTuple, Optional, Tuple
 
 import torch
 from torch import nn, Tensor
+
+from ...engine import _RuntimeOwner
 
 
 class TransformerOutput(NamedTuple):
@@ -30,7 +34,7 @@ def _no_dropout(dropout: float, what: str) -> None:
         raise NotImplementedError(f"{what}: dropout > 0 is not on the accelerated path (reference default is 0.0)")
 
 
-class TransformerEncoderLayer(nn.Module):
+class TransformerEncoderLayer(_RuntimeOwner):
     def __init__(self, d_model: int, n_head: int, dim_feedforward: int, dropout: float = 0.0,
                  activation: Callable[..., nn.Module] = nn.ReLU, layer_norm_eps: float = 1e-12, norm_first: bool = False,
                  drop_path_rate: Optional[float] = None) -> None:
@@ -53,13 +57,13 @@ class TransformerEncoderLayer(nn.Module):
         self.norm_first = norm_first
 
     def forward(self, hidden_states: Tensor, attention_mask: Optional[Tensor] = None) -> Tensor:
-        """Standalone forward (values only; inside VisionTransformer the layer runs in the fused TransformerStack)."""
+        """Standalone forward (inside VisionTransformer the layer runs in the owner's fused TransformerStack)."""
         from ...engine_layers import encoder_layer_forward
 
         return encoder_layer_forward(self, hidden_states, attention_mask)
 
 
-class TransformerEncoder(nn.Module):
+class TransformerEncoder(_RuntimeOwner):
     def __init__(self, n_layer: int, d_model: int, n_head: int, dim_feedforward: int, dropout: float = 0.0,
                  activation: Callable[..., nn.Module] = nn.ReLU, layer_norm_eps: float = 1e-12, norm_first: bool = False,
                  final_layer_norm_eps: Optional[float] = None, drop_path_rate: Optional[float] = None):
@@ -79,10 +83,24 @@ class TransformerEncoder(nn.Module):
 
     def forward(self, hidden_states: Tensor, attention_mask: Optional[Tensor] = None,
                 return_hidden_states: bool = False) -> TransformerOutput:
-        """Standalone forward (values only; inside VisionTransformer the stack runs in the fused TransformerStack)."""
+        """Standalone forward (inside VisionTransformer the stack runs in the owner's fused TransformerStack)."""
         from ...engine_layers import encoder_forward
 
         return encoder_forward(self, hidden_states, attention_mask, return_hidden_states)
+
+
+def _layer_runtime(mod):
+    from ...engine_layers import EncoderLayersRuntime
+    return EncoderLayersRuntime(mod, [mod], None)
+
+
+def _encoder_runtime(mod):
+    from ...engine_layers import EncoderLayersRuntime
+    return EncoderLayersRuntime(mod, mod.layer, mod.final_layer_norm)
+
+
+TransformerEncoderLayer._runtime_cls = staticmethod(_layer_runtime)
+TransformerEncoder._runtime_cls = staticmethod(_encoder_runtime)
 
 
 class TransformerDecoderLayer(nn.Module):

@@ -1,12 +1,13 @@
-"""The CLIP, FLAVA and CoCa modules compute the same forward values under torch.no_grad() and with grad mode on, bit
-for bit.
+"""The CLIP, FLAVA and CoCa modules and the standalone pre-norm encoder compute the same forward values under
+torch.no_grad() and with grad mode on, bit for bit.
 
 The inference and training runtimes launch the same kernels on the same operands (ops.self_attention picks the
 attention kernel for both); only the buffers that keep activations for the backward differ.  The cases are those of
-test_gpu_runtime_pinned.py, plus a CoCa vision tower at 400 tokens, inside the band (385-512 tokens, unmasked
-head_dim-64 self-attention) where the two modes once chose different attention kernels.  On an H100 the fused and the
-general forward give the same bits in that band, so this test would not notice that split coming back (it only cost
-speed); tests/test_attention_router_cpu.py is what guards the routing rule.
+test_gpu_runtime_pinned.py (the standalone pre-norm TransformerEncoder with its [B, S, S] mask), plus a CoCa vision
+tower at 400 tokens, inside the band (385-512 tokens, unmasked head_dim-64 self-attention) where the two modes once
+chose different attention kernels.  On an H100 the fused and the general forward give the same bits in that band, so
+this test would not notice that split coming back (it only cost speed); tests/test_attention_router_cpu.py is what
+guards the routing rule.
 """
 import pytest
 import torch
@@ -58,6 +59,9 @@ def _outputs(name, dev):
         assert v.last_hidden_state.shape[1] == 400
         return {"last_hidden_state": v.last_hidden_state,
                 **{f"hidden_states.{i}": h for i, h in enumerate(v.hidden_states)}}
+    if name == "standalone_encoder":
+        m, x, mask = P._standalone("encoder")
+        return P._standalone_outputs(m.to(dev), x, mask, dev)
     if name == "clip_small":
         m, image, text = P._clip_small()
         return P._clip_outputs(m.to(dev), image, text, dev)
@@ -66,7 +70,7 @@ def _outputs(name, dev):
 
 
 @pytest.mark.parametrize("name", ["flava_small", "flava_long", "flava_text512", "coca_small", "coca_parallel",
-                                  "coca_l14", "coca_vision_400", "clip_small"])
+                                  "coca_l14", "coca_vision_400", "clip_small", "standalone_encoder"])
 def test_no_grad_equals_grad_mode_forward(name):
     dev = torch.device("cuda:0")
     with torch.no_grad():

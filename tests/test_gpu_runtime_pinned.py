@@ -1,4 +1,5 @@
-"""Pins the CLIP, FLAVA and CoCa module forwards bit for bit, under torch.no_grad() and with grad mode on.
+"""Pins the CLIP, FLAVA and CoCa module forwards and the standalone pre-norm encoder layers bit for bit, under
+torch.no_grad() and with grad mode on.
 
 Every tensor the inference forwards return is hashed: hidden states, pooler outputs, projected embeddings, attention
 probabilities, multimodal logits, both CoCa losses and the CLIP towers' embeddings and text hidden state.  With grad
@@ -182,6 +183,38 @@ def _clip_small():
     return m.train(), image, text
 
 
+def _standalone(kind, drop=False):
+    """A standalone pre-norm TransformerEncoder (3 layers, final LayerNorm) or TransformerEncoderLayer at width 128
+    (head_dim 64) with perturbed weights, an input batch and a [B, S, S] bool mask; with `drop`, drop_path_rate 0.5."""
+    from multimodal_b200.modules.layers.transformer import TransformerEncoder, TransformerEncoderLayer
+
+    torch.manual_seed(0)
+    rate = 0.5 if drop else None
+    if kind == "layer":
+        m = TransformerEncoderLayer(128, 2, 256, activation=torch.nn.GELU, layer_norm_eps=1e-5, norm_first=True,
+                                    drop_path_rate=rate)
+    else:
+        m = TransformerEncoder(3, 128, 2, 256, activation=torch.nn.GELU, layer_norm_eps=1e-5, norm_first=True,
+                               final_layer_norm_eps=1e-5, drop_path_rate=rate)
+    g = torch.Generator().manual_seed(31)
+    with torch.no_grad():
+        for p in m.parameters():
+            p.add_(0.03 * torch.randn(p.shape, generator=g))
+    x = torch.randn(4, 20, 128, generator=g)
+    mask = torch.rand(4, 20, 20, generator=g) < 0.7
+    mask[:, :, 0] = True
+    return (m.train() if drop else m.eval()), x, mask
+
+
+def _standalone_outputs(m, x, mask, dev):
+    """Output and hidden states of one standalone call (the encoder with `return_hidden_states`)."""
+    x, mask = x.to(dev), (mask.to(dev) if mask is not None else None)
+    if not hasattr(m, "layer"):
+        return {"output": m(x, mask)}
+    o = m(x, mask, return_hidden_states=True)
+    return {"last_hidden_state": o.last_hidden_state, **{f"hidden_states.{i}": h for i, h in enumerate(o.hidden_states)}}
+
+
 def _clip_outputs(m, image, text, dev):
     """The embeddings of both CLIP towers."""
     return {"image.embeddings": m.encoder_a(image.to(dev)), "text.embeddings": m.encoder_b(text.to(dev))}
@@ -245,6 +278,17 @@ def _case(name, dev):
         m, images, texts = _coca_l14() if base == "coca_l14" else _coca(base)
         m = m.to(dev)
         return (_coca_inference if mode == "infer" else _coca_grad)(m, images, texts, dev)
+    if name.startswith("standalone_"):
+        base, mode = name.rsplit(".", 1)
+        m, x, mask = _standalone("layer" if base == "standalone_layer" else "encoder", drop=base == "standalone_drop")
+        m = m.to(dev)
+        if base != "standalone_encoder":
+            mask = None     # the fused attention kernels
+        torch.manual_seed(37)
+        with torch.set_grad_enabled(mode == "grad"):
+            res = _standalone_outputs(m, x, mask, dev)
+        assert res.get("output", res.get("last_hidden_state")).requires_grad == (mode == "grad")
+        return res
     if name == "text_decoder_no_cls.infer":
         m, ids = _text_decoder_no_cls()
         m = m.to(dev)
@@ -257,7 +301,8 @@ def _case(name, dev):
 CASES = ["flava_small.infer", "flava_small.grad", "flava_long.infer", "flava_long.grad", "flava_attentions.infer",
          "flava_text512.infer", "flava_text512.grad", "coca_small.infer", "coca_small.grad", "coca_parallel.infer",
          "coca_parallel.grad", "coca_l14.infer", "coca_l14.grad", "text_decoder_no_cls.infer", "coca_hd96.infer",
-         "coca_hd128.infer", "vit_drop.infer", "clip_small.infer", "clip_small.grad"]
+         "coca_hd128.infer", "vit_drop.infer", "clip_small.infer", "clip_small.grad", "standalone_encoder.infer",
+         "standalone_encoder.grad", "standalone_drop.infer", "standalone_layer.infer"]
 
 # {case: {output: sha256 of its bytes}}, recorded on an H100 80GB HBM3
 PINNED = {
@@ -473,6 +518,30 @@ PINNED = {
     'clip_small.grad': {
         'image.embeddings': '(6, 64) torch.float32 37cf4a55f7b872b5ac1e7d732d658d269390e051db61cb5693e2a7d23372f4c4',
         'text.embeddings': '(6, 64) torch.float32 f9b77915bf2430ad93236172cdc3d49aff5ca3a673eefda1c8df4c2da5f894e3',
+    },
+    'standalone_encoder.infer': {
+        'hidden_states.0': '(4, 20, 128) torch.float32 9d2d3d9fc40a1929827fccec26876dd39d07c3a57c7dc3367a68bddba21b09a2',
+        'hidden_states.1': '(4, 20, 128) torch.float32 44ecc096c17cf09b63301cddaeff103101db20a2146c81e966eda5574c73bf9f',
+        'hidden_states.2': '(4, 20, 128) torch.float32 91e73578053ab421bc58731fc4d4dd5dff9d227d7553eb2a4d8d3af344f0ec83',
+        'hidden_states.3': '(4, 20, 128) torch.float32 ce8e54f33464f33d98c4d6d2fa1a47086ee65972330266092856198d79179d56',
+        'last_hidden_state': '(4, 20, 128) torch.float32 ef4ad8177bf3f469852fb8bfda2d335f634c60d76c3fe94c16ab764a0f8c109d',
+    },
+    'standalone_encoder.grad': {
+        'hidden_states.0': '(4, 20, 128) torch.float32 9d2d3d9fc40a1929827fccec26876dd39d07c3a57c7dc3367a68bddba21b09a2',
+        'hidden_states.1': '(4, 20, 128) torch.float32 44ecc096c17cf09b63301cddaeff103101db20a2146c81e966eda5574c73bf9f',
+        'hidden_states.2': '(4, 20, 128) torch.float32 91e73578053ab421bc58731fc4d4dd5dff9d227d7553eb2a4d8d3af344f0ec83',
+        'hidden_states.3': '(4, 20, 128) torch.float32 ce8e54f33464f33d98c4d6d2fa1a47086ee65972330266092856198d79179d56',
+        'last_hidden_state': '(4, 20, 128) torch.float32 ef4ad8177bf3f469852fb8bfda2d335f634c60d76c3fe94c16ab764a0f8c109d',
+    },
+    'standalone_drop.infer': {
+        'hidden_states.0': '(4, 20, 128) torch.float32 9d2d3d9fc40a1929827fccec26876dd39d07c3a57c7dc3367a68bddba21b09a2',
+        'hidden_states.1': '(4, 20, 128) torch.float32 831be8cd17d14c2a10ec1fc0fb037335fa7edd667894cddaf44a2987f38474c3',
+        'hidden_states.2': '(4, 20, 128) torch.float32 b22710c0b864a6a69bfd6a084477f604a431b22ceb83b350ba689d0402031f89',
+        'hidden_states.3': '(4, 20, 128) torch.float32 580b39fd455652233940b0f84b80a462ca3b76e53687a7adbdf708b73b8104ce',
+        'last_hidden_state': '(4, 20, 128) torch.float32 bc0a74b24f291f7f5fc16bda0108db7132132b82256d907203a0f33847d415b7',
+    },
+    'standalone_layer.infer': {
+        'output': '(4, 20, 128) torch.float32 c4306e38ee00eb9866b496cc9a428796cb5822d58bade6a7f14f0abdfd768594',
     },
 }
 

@@ -1,6 +1,6 @@
-"""One runtime per CLIP / FLAVA / CoCa module serves both grad modes; these tests check, WITHOUT a GPU, that its
-torch.no_grad() entry point (no save Workspace, scratch shared by the layers) and its training forward (activations
-saved per call) compute the same bits, with the kernels swapped for their torch emulation (tests/emu_ops.py, with the
+"""One runtime per CLIP / FLAVA / CoCa module and per standalone pre-norm encoder serves both grad modes; these tests
+check, WITHOUT a GPU, that its torch.no_grad() entry point (no save Workspace, scratch shared by the layers) and its
+training forward (activations saved per call) compute the same bits, with the kernels swapped for their torch emulation (tests/emu_ops.py, with the
 stochastic-depth variants of tests/emu_drop_path_ops.py).  The same property on the kernels proper:
 tests/test_gpu_grad_mode_invariance.py."""
 import pytest
@@ -53,6 +53,25 @@ def test_no_grad_forward_equals_training_forward_with_drop_path(emu, name):
         out = vit(images)
         return {"last_hidden_state": out.last_hidden_state,
                 **{f"hidden_states.{i}": h for i, h in enumerate(out.hidden_states)}}
+
+    _assert_grad_modes_agree(outputs)
+
+
+@pytest.mark.parametrize("kind,masked,drop", [("encoder", False, False), ("encoder", True, False),
+                                               ("encoder", False, True), ("encoder", True, True),
+                                               ("layer", False, False), ("layer", True, False)])
+def test_standalone_no_grad_forward_equals_training_forward(emu, monkeypatch, kind, masked, drop):
+    """A standalone pre-norm TransformerEncoder (final LayerNorm, return_hidden_states) or TransformerEncoderLayer, with
+    and without a [B, S, S] bool mask; with drop_path_rate in train() mode both grad modes draw the same factors under
+    the same seed.  The CUDA-input check of the no_grad call is lifted for the emulated kernels."""
+    from multimodal_b200 import engine_layers
+
+    monkeypatch.setattr(engine_layers, "_cuda", lambda t, what: None)
+    m, x, mask = P._standalone(kind, drop=drop)
+
+    def outputs():
+        torch.manual_seed(37)
+        return P._standalone_outputs(m, x, mask if masked else None, CPU)
 
     _assert_grad_modes_agree(outputs)
 
