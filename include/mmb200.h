@@ -39,14 +39,15 @@ int mmb_version(void);
  *           `x @ self.projection` in models/clip/image_encoder.py:112, Linear in text_encoder.py:130.
  * colsum (optional, EPI_BF16 / EPI_BF16_DACT): colsum[n] += sum_m of the bf16-rounded D0[m,n] — the bias gradient of
  *           the Linear whose input-gradient this GEMM produces (linear1.bias from the FC2 dgrad), fused into the
- *           epilogue's copy-out so the tensor is not re-read by a column-sum pass. */
+ *           epilogue's copy-out so the tensor is not re-read by a column-sum pass.
+ * accumulate is accepted with EPI_F32 only, bias with every epilogue but EPI_BF16_DACT; either elsewhere: MMB_ERR_ARG. */
 int mmb_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb, int b_mn_major,
                   void* D0, long long ldd0, void* D1, long long ldd1, int M, int N, int K, int epilogue, int act,
                   float alpha, const float* bias, const void* aux, long long ld_aux, int splits, int accumulate,
                   float* colsum, void* stream);
 
 /* Test / A-B hook (process-wide): force the kernel variant mmb_gemm_bf16 dispatches to.
- *   cta2: -1 = automatic (size heuristic), 0 = one CTA per 128x128 tile, 1 = 2-CTA clusters (256x128 tiles, the B tile
+ *   cta2: -1 = automatic (size heuristic), 0 = one CTA per 128x256 tile, 1 = 2-CTA clusters (256x256 tiles, the B tile
  *   multicast to both CTAs); epilogue_warps: 0 or 8 (the two consumer warpgroups run every epilogue).  Returns
  *   MMB_ERR_ARG on other values.
  * No reference counterpart: it exists so the parity tests can drive both kernels over every operand / epilogue case. */

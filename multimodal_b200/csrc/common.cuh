@@ -292,7 +292,10 @@ __device__ __forceinline__ float tanh_approx(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// sigmoid(1.702 x) = 0.5 + 0.5 tanh(0.851 x): ONE MUFU op (tanh.approx, rel. error 2^-11 < bf16 output rounding).
+// sigmoid(1.702 x) = 0.5 + 0.5 tanh(0.851 x): ONE MUFU op (tanh.approx, relative error <= 2^-10.987 in t).  The
+// result's error is an absolute one, <= |x| / 2 * 2^-10.987: measured over every bf16 input on an H100 it stays below
+// the bf16 output rounding (0.023 of it) for x > -4; where 1 + t cancels (x <= -4) it grows up to the whole
+// value (0 at x = -9.44, where tanh.approx returns -1; |x sigmoid(1.702 x)| is 1e-6 there).
 __device__ __forceinline__ float quick_gelu(float x) {
   const float t = tanh_approx(0.851f * x), h = 0.5f * x;
   return fmaf(h, t, h);

@@ -653,6 +653,9 @@ static int gemm_dispatch(const void* A, long long lda, int a_mn_major, const voi
   if ((epilogue == EPI_CE_STATS || epilogue == EPI_CE_GRAD) && (!ce || a_mn_major || b_mn_major)) return MMB_ERR_ARG;
   if ((lda & 7) || (ldb & 7)) return MMB_ERR_ARG;
   if (epilogue != EPI_CE_STATS && (epilogue == EPI_F32 ? (N & 3) : (N & 7))) return MMB_ERR_ARG;   // CE_STATS writes no tensor
+  // only the fp32 epilogue adds into D0, and EPI_BF16_DACT takes no bias: refuse what the kernel would ignore
+  if (accumulate && epilogue != EPI_F32) return MMB_ERR_ARG;
+  if (bias && epilogue == EPI_BF16_DACT) return MMB_ERR_ARG;
   // 2-CTA clusters (256x256 tiles, B multicast) for everything large enough to fill the SM pairs at least once
   const long long big_tiles = (long long)((M + 2 * BLOCK_M - 1) / (2 * BLOCK_M)) * ((N + BLOCK_N - 1) / BLOCK_N);
   const bool cta2 = g_force_cta2 == 1 ||

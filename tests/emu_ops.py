@@ -33,6 +33,8 @@ def gemm(A, B, *, a_mn=False, b_mn=False, epilogue=EPI_BF16, out=None, out2=None
     assert Af.shape[1] == Bf.shape[1], (Af.shape, Bf.shape)
     acc = alpha * (Af @ Bf.t())
     M, N = acc.shape
+    assert not (accumulate and epilogue != EPI_F32) and not (bias is not None and epilogue == EPI_BF16_DACT)
+    assert colsum is None or epilogue in (EPI_BF16, EPI_BF16_DACT)
     if bias is not None:
         assert bias.dtype == F32 and bias.numel() == N
         acc = acc + bias.detach().view(1, N)
@@ -43,9 +45,10 @@ def gemm(A, B, *, a_mn=False, b_mn=False, epilogue=EPI_BF16, out=None, out2=None
     if epilogue == EPI_F32:
         out.copy_(out + acc if accumulate else acc)
         return out
-    assert not accumulate
     if epilogue == EPI_BF16:
         out.copy_(acc.to(BF))
+        if colsum is not None:
+            colsum.add_(out.float().sum(0))
         return out
     if epilogue == EPI_BF16_ACT:
         if out2 is None:

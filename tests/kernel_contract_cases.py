@@ -165,10 +165,17 @@ class _Out:
         self.rec[name] = Rec("bound", got, total.clone(), r)
 
 
-def compare_recs(name, a: Rec, b: Rec, slack=0.0):
+def compare_recs(name, a: Rec, b: Rec, slack=0.0, where=None):
     """Holds two implementations' results of the same check against each other under the output's class.  slack widens
-    a bound where the output sums another compared output that may legitimately differ (gsum over g_bf16)."""
+    a bound where the output sums another compared output that may legitimately differ (gsum over g_bf16, the GEMM's
+    colsum over D0); where (bf16 class) restricts the comparison to the elements formed from identical inputs (the
+    GEMM's act(D0) where the two D0 agree: each implementation met the contract on its own D0 everywhere)."""
     assert a.kind == b.kind
+    if where is not None:
+        assert a.kind == "bf16"
+        err = a.param[1]
+        a = Rec("bf16", a.got[where], (a.param[0], None if err is None else err[where]))
+        b = Rec("bf16", b.got[where])
     if a.kind == "exact":
         assert_exact(name, a.got, b.got)
     elif a.kind == "bf16":
@@ -185,7 +192,9 @@ def compare_recs(name, a: Rec, b: Rec, slack=0.0):
 # (P rounded to bf16 in rows that one key dominates), and attention_probs 0.24, so those stay derived.
 TIGHTENED = {
     "sum_scale.out": 0.01,                   # measured 0.0027 (kernel and emulation: the final rounding only)
-    "gemm.D": 0.04,                          # EPI_F32 accumulate: 0.013 kernel, 0.012 emulation
+    "gemm.D": 0.42,                          # EPI_F32, every case: 0.139 kernel, 0.141 emulation
+    "gemm.D_acc": 0.6,                       # EPI_F32 D += result (TMA reduce-add, split-K, direct): 0.142 / 0.197
+    "gemm.colsum": 0.33,                     # 0.111 / 0.110
     "colsum_bf16.out": 0.11,                 # 0.036 / 0.036
     "ce_labels.accum": 0.11,                 # 0.036 / 0.036
     "layernorm_bwd.gsum": 0.28,              # 0.091 / 0.091
@@ -207,6 +216,10 @@ TIGHTENED = {
     "linear_cross_entropy.row_loss": 0.15,   # 0.048 / 0.048
     "linear_cross_entropy.accum": 0.1,       # 0.033 / 0.024
 }
+# The GEMM epilogue's QuickGELU (common.cuh quick_gelu: x / 2 (1 + tanh.approx(0.851 x))), measured in fp32 on an H100
+# 80GB HBM3 over every bf16 input against float64, as a multiple of the bf16 output rounding 2^-8 |ref|: 0.0037 for
+# x > -1, 0.023 for -4 < x <= -1, and up to 256 for x <= -4 (the result is 0 where tanh.approx returns -1, e.g.
+# x = -9.4375).  The derived bound _act_fwd_epi_err, absolute in |x| |t| 2^-10.987, holds everywhere (largest share 0.96).
 
 
 # ---- special values --------------------------------------------------------------------------------------------------
@@ -768,6 +781,37 @@ def _act_grad64(x64, kind):
     return _phi_cdf(x64) + x64 * torch.exp(-0.5 * x64 * x64) / math.sqrt(2 * math.pi)
 
 
+TANH_APPROX = 2.0 ** -10.987   # maximum relative error of tanh.approx.f32 (PTX ISA)
+
+
+def _quick_gelu_tanh(x64):
+    """u = 0.851 x, t = tanh(u) and the absolute error of the kernels' t = tanh.approx(fl(0.851f x)) (common.cuh
+    quick_gelu / quick_gelu_grad): the approximation's TANH_APPROX |t| plus u's rounding (2 U |u|: the constant and the
+    product) carried through dt / du = 1 - t^2."""
+    u = 0.851 * x64
+    t = torch.tanh(u)
+    return u, t, TANH_APPROX * t.abs() + 2 * U * u.abs() * (1 - t * t)
+
+
+def _act_fwd_epi_err(x64, kind):
+    """Absolute error of the GEMM epilogue's act(x) in fp32 (common.cuh act_fn).  QuickGELU = fmaf(h, t, h), h = x / 2:
+    |h| times t's error plus the fmaf's rounding; GELU-erf as check_act_fwd."""
+    if kind == 0:
+        _, _, et = _quick_gelu_tanh(x64)
+        return 0.5 * x64.abs() * et + U * _act64(x64, 0).abs()
+    return 4 * U * _act64(x64, 1).abs() + 8 * U * x64.abs()
+
+
+def _act_grad_err(x64, kind):
+    """Absolute error of the kernels' act'(x) in fp32 (common.cuh act_grad).  QuickGELU': 0.5 (1 + t + u (1 - t^2)),
+    whose derivative in t is 0.5 (1 - 2 u t), plus the roundings of the three fmaf; GELU-erf': Phi(x) = 0.5 (1 + erf)
+    carries an absolute error of a few ulp of 1, exp of -x^2/2 a relative one ~ x^2 u."""
+    if kind == 0:
+        u, t, et = _quick_gelu_tanh(x64)
+        return 0.5 * (1 - 2 * u * t).abs() * et + 8 * U * (1 + u.abs())
+    return 8 * U + (8 + x64 * x64) * U * (x64 * torch.exp(-0.5 * x64 * x64)).abs()
+
+
 def _act_input(case, n):
     x = torch.randn(n, generator=_gen(case)) * 3
     return _with_specials(x, ACT_SPECIALS)
@@ -828,15 +872,8 @@ def check_act_bwd(impl, device, case):
     dx = torch.empty(n, dtype=BF, device=device)
     impl.act_bwd(dy.to(device, copy=True), pre.to(device, copy=True), dx, kind)
     x64, dy64 = d64(pre), d64(dy)
-    if kind == 0:
-        # tanh.approx (relative error 2^-11) inside 0.5 (1 + t + u (1 - t^2)), u = 0.851 x
-        u = 0.851 * x64
-        t = torch.tanh(u)
-        err = dy64.abs() * (0.5 * (1 - 2 * u * t).abs() * 2.0 ** -11 * t.abs() + 8 * U * (1 + u.abs()))
-    else:
-        # Phi(x) = 0.5 (1 + erf) carries an absolute error of a few ulp of 1; exp of -x^2/2 a relative one ~ x^2 u
-        err = dy64.abs() * (8 * U + (8 + x64 * x64) * U * (x64 * torch.exp(-0.5 * x64 * x64)).abs())
-    o.bf16("dx", dx, dy64 * _act_grad64(x64, kind), case.get("min_equal", 0.99), err=err)
+    o.bf16("dx", dx, dy64 * _act_grad64(x64, kind), case.get("min_equal", 0.99),
+           err=dy64.abs() * _act_grad_err(x64, kind))
     return o.rec
 
 
@@ -1075,23 +1112,135 @@ def check_ce_labels_bwd(impl, device, case):
     return o.rec
 
 
-# ---- GEMM: a small case each, so the emulation meets the kernel --------------------------------------------------------
+# ---- GEMM: every instantiation gemm_launch dispatches, its fused epilogues, tile boundaries and operand pitches ----------
+# A case names the epilogue ("epi": bf16 / act / dact / f32), the operand layouts (a_mn, b_mn), the activation (act:
+# 0 QuickGELU, 1 GELU-erf), alpha, bias, colsum, split-K (splits), "pad" extra columns on every pitch and, for fp32,
+# the output's first column "col0" in its buffer (1: a base off 16 bytes, written with direct stores).
+# Operands: A scaled by 3 / sqrt(K) (pre-activations of a few units, where the activations bend), bf16 before the
+# float64 products are formed (_gemm64), stored at pitches rounded up to 8 elements past extent + pad with the padding
+# NaN: a read of it poisons the result.  Outputs are [M, N] views one row into [M + 2, ld] buffers of a sentinel bit
+# pattern: every element outside [M, N] must come back unchanged.
+# Bounds (S = the split count the dispatch forms):
+#   acc     the fp32 accumulation and the fmaf that applies alpha and bias, (K + S + 3) U (|alpha| sum|a||b| + |bias|);
+#   D0      bf16 (EPI_BF16, the ACT pre-activation): within 1 bf16 ulp of bf16(alpha A B^T + bias), err = acc;
+#   D1      act(D0) of the implementation's own stored bf16 D0 (mmb200.h: D1 = bf16(act(D0))), err = _act_fwd_epi_err;
+#   DACT    alpha acc act'(aux): err = (acc + U |alpha acc|) |act'| + |alpha acc| _act_grad_err;
+#   colsum  colsum0 + sum_m of the stored D0: k U sum|terms| with k = 2 (rows per thread) + 3 (shuffle levels) +
+#           8 (warps) + ceil(P / 8) + 8 + 1 (reduce_partials over P = ceil(M / 128) row blocks);
+#   fp32    D = alpha acc + bias within acc, and D_acc = C0 + alpha acc + bias within acc + (K + S + 3) U |C0|.
+_SENT_BF16 = 0x4B39
+_SENT_F32 = 0x4B39A5C3
+_EPI = {"bf16": 0, "act": 1, "dact": 2, "f32": 3}
+
+
+def _ld8(n):
+    return _cdiv(n, 8) * 8
+
+
+def _nan_padded(x, ld):
+    """x [rows, cols] bf16 stored in a [rows, ld] buffer whose padding columns are NaN."""
+    buf = torch.full((x.shape[0], ld), NAN, dtype=BF)
+    buf[:, :x.shape[1]] = x
+    return buf
+
+
+def _gemm_splits(K, splits, epi):
+    """The split count gemm_dispatch forms: clamped to [1, k-blocks], one for bf16 epilogues, then whole k-block runs."""
+    kb = _cdiv(K, 64)
+    s = 1 if epi != "f32" else min(max(splits, 1), kb)
+    return _cdiv(kb, _cdiv(kb, s))
+
+
+def _sentinel_out(M, N, ld, col0, dtype, device, inner=None):
+    """The [M, N] view at row 1, column col0 of a [M + 2, ld] buffer filled with the sentinel (inner: its values)."""
+    if dtype == BF:
+        buf = torch.full((M + 2, ld), _SENT_BF16, dtype=torch.int16).view(BF)
+    else:
+        buf = torch.full((M + 2, ld), _SENT_F32, dtype=torch.int32).view(F32)
+    if inner is not None:
+        buf[1:M + 1, col0:col0 + N] = inner
+    buf = buf.to(device, copy=True)
+    return buf, buf[1:M + 1, col0:col0 + N]
+
+
+def _check_outside(o, name, buf, M, N, col0):
+    got = buf.detach().cpu()
+    keep = torch.ones(got.shape, dtype=torch.bool)
+    keep[1:M + 1, col0:col0 + N] = False
+    want = _SENT_BF16 if got.dtype == BF else _SENT_F32
+    o.exact(name, _bits(got)[keep], torch.full((int(keep.sum()),), want, dtype=_bits(got).dtype))
+
+
 def check_gemm(impl, device, case):
     o = _Out("gemm")
     g = _gen(case)
     M, N, K = case["M"], case["N"], case["K"]
-    A, Bm = torch.randn(M, K, generator=g).to(BF), torch.randn(N, K, generator=g).to(BF)
+    epi, act, a_mn, b_mn = case["epi"], case.get("act", 0), case.get("a_mn", 0), case.get("b_mn", 0)
+    alpha, pad, col0 = case.get("alpha", 1.0), case.get("pad", 0), case.get("col0", 0)
+    S = _gemm_splits(K, case.get("splits", 1), epi)
+    use_bias = case.get("bias", epi != "dact")
+    use_colsum = case.get("colsum", epi in ("bf16", "dact"))
+    A = (torch.randn(M, K, generator=g) * (3 / math.sqrt(K))).to(BF)
+    Bm = torch.randn(N, K, generator=g).to(BF)
     bias = torch.randn(N, generator=g)
-    ref = d64(A) @ d64(Bm).t()
-    mag = d64(A).abs() @ d64(Bm).abs().t()
-    if case["epi"] == "f32":
+    As = _nan_padded(A.t() if a_mn else A, _ld8((M if a_mn else K) + pad))
+    Bs = _nan_padded(Bm.t() if b_mn else Bm, _ld8((N if b_mn else K) + pad))
+    Ad = As.to(device, copy=True)[:, :(M if a_mn else K)]
+    Bd = Bs.to(device, copy=True)[:, :(N if b_mn else K)]
+    tod = lambda t: t.to(device, copy=True)  # noqa: E731
+    acc, mag = _gemm64(A, Bm)
+    mag = mag / ((K + 3) * U)
+    b64 = d64(bias) if use_bias else torch.zeros(N, dtype=F64)
+    ref = alpha * acc + b64
+    e_acc = (K + S + 3) * U * (abs(alpha) * mag + b64.abs())
+    kw = dict(a_mn=bool(a_mn), b_mn=bool(b_mn), epilogue=_EPI[epi], alpha=alpha, act=act, splits=case.get("splits", 1),
+              bias=tod(bias) if use_bias else None)
+    ld = (_ld8 if epi != "f32" else lambda n: _cdiv(n, 4) * 4)(col0 + N + pad)
+
+    if epi == "f32":
         C0 = torch.randn(M, N, generator=g)
-        C = C0.to(device, copy=True)
-        impl.gemm(A.to(device, copy=True), Bm.to(device, copy=True), epilogue=3, out=C, accumulate=True)
-        o.bound("D", C, ref + d64(C0), (K + 3) * U * (mag + d64(C0).abs()))
+        buf, D = _sentinel_out(M, N, ld, col0, F32, device)
+        buf_acc, D_acc = _sentinel_out(M, N, ld, col0, F32, device, inner=C0)
+        with _gemm_mode(impl, case):
+            impl.gemm(Ad, Bd, out=D, **kw)
+            impl.gemm(Ad, Bd, out=D_acc, accumulate=True, **kw)
+        o.bound("D", D, ref, e_acc)
+        o.bound("D_acc", D_acc, ref + d64(C0), e_acc + (K + S + 3) * U * d64(C0).abs())
+        _check_outside(o, "D_outside", buf, M, N, col0)
+        _check_outside(o, "D_acc_outside", buf_acc, M, N, col0)
+        return o.rec
+
+    cs0 = torch.randn(N, generator=g)
+    cs = tod(cs0) if use_colsum else None
+    buf0, D0 = _sentinel_out(M, N, ld, 0, BF, device)
+    if epi == "act":
+        buf1, D1 = _sentinel_out(M, N, ld, 0, BF, device)
+        with _gemm_mode(impl, case):
+            impl.gemm(Ad, Bd, out=D0, out2=D1, **kw)
+    elif epi == "dact":
+        aux = (torch.randn(M, N, generator=g) * 2).to(BF)
+        auxd = tod(_nan_padded(aux, _ld8(N + pad)))[:, :N]
+        with _gemm_mode(impl, case):
+            impl.gemm(Ad, Bd, out=D0, aux=auxd, colsum=cs, **kw)
     else:
-        D = impl.gemm(A.to(device, copy=True), Bm.to(device, copy=True), bias=bias.to(device, copy=True))
-        o.bf16("D", D, ref + d64(bias), err=(K + 3) * U * (mag + d64(bias).abs()))
+        with _gemm_mode(impl, case):
+            impl.gemm(Ad, Bd, out=D0, colsum=cs, **kw)
+
+    if epi == "dact":
+        x64 = d64(aux)
+        gr = _act_grad64(x64, act)
+        o.bf16("D0", D0, ref * gr, err=(e_acc + U * ref.abs()) * gr.abs() + ref.abs() * _act_grad_err(x64, act))
+    else:
+        o.bf16("D0", D0, ref, err=e_acc)
+    _check_outside(o, "D0_outside", buf0, M, N, 0)
+    if epi == "act":
+        pre = d64(D0)
+        o.bf16("D1", D1, _act64(pre, act), err=_act_fwd_epi_err(pre, act))
+        _check_outside(o, "D1_outside", buf1, M, N, 0)
+    if use_colsum:
+        terms = d64(D0)
+        k = 2 + 3 + 8 + _cdiv(_cdiv(M, 128), 8) + 8 + 1
+        o.bound("colsum", cs, d64(cs0) + terms.sum(0), k * U * (terms.abs().sum(0) + d64(cs0).abs()))
     return o.rec
 
 
@@ -2127,6 +2276,99 @@ _LINEAR_CE = _both_modes([
     {"M": 1000, "V": 1001, "K": 768, "n_ignored": 100, "gpu": True},
 ])
 
+# The ten (a_mn, b_mn, epilogue, act) instantiations gemm_launch dispatches, split-K on the two wgrad layouts.
+GEMM_KINDS = [
+    {"epi": "bf16"}, {"epi": "act", "act": 0}, {"epi": "act", "act": 1}, {"epi": "f32"},
+    {"epi": "bf16", "b_mn": 1}, {"epi": "dact", "b_mn": 1, "act": 0}, {"epi": "dact", "b_mn": 1, "act": 1},
+    {"epi": "f32", "b_mn": 1}, {"epi": "f32", "a_mn": 1, "b_mn": 1, "splits": 3}, {"epi": "f32", "a_mn": 1, "splits": 2},
+]
+
+
+def _gemm_kind_key(c):
+    return c.get("a_mn", 0), c.get("b_mn", 0), _EPI[c["epi"]], c.get("act", 0) if c["epi"] in ("act", "dact") else 0
+
+
+def _gc(M, N, K, kind, **kw):
+    return {"M": M, "N": N, "K": K, **GEMM_KINDS[kind], **kw}
+
+
+# Edges, each in both variants: M below 64 (the second consumer warpgroup has no rows) and on both sides of 64, 128 and
+# 256, M <= 128 in a cluster (the peer CTA has no rows), N = 8 and one 8-column chunk past 64 / 256, fp32 N = 4 mod 8,
+# K = 8, 64, 65 and tails shorter than one k-block, alpha 1 / 0.125 / -0.5 with and without bias, NaN-padded operand
+# pitches, fp32 outputs off 16 bytes (direct stores, also under split-K).
+_GEMM_EDGES = [
+    _gc(40, 264, 72, 0, alpha=0.125, pad=8),
+    _gc(65, 72, 65, 1, alpha=-0.5),
+    _gc(127, 8, 8, 2, pad=16),
+    _gc(129, 260, 200, 3, alpha=-0.5, col0=1, pad=4),
+    _gc(100, 520, 64, 4, bias=False, pad=8),
+    _gc(257, 136, 136, 5, alpha=0.125, pad=8),
+    _gc(64, 264, 72, 6, alpha=-0.5),
+    _gc(255, 68, 8, 7, bias=False, pad=4),
+    _gc(136, 12, 392, 8, alpha=0.125, pad=8),
+    _gc(264, 200, 136, 9, col0=1),
+    _gc(63, 328, 65, 0, bias=False, colsum=True, alpha=-0.5),
+    _gc(128, 72, 64, 1, bias=False, pad=8),
+    _gc(256, 264, 130, 5, alpha=-0.5, pad=8),
+    _gc(48, 260, 200, 8, alpha=-0.5, splits=4),
+    _gc(300, 516, 200, 3, bias=False, col0=1),       # an fp32 column slice: base 4 bytes past a 16-byte boundary
+]
+# Persistent loops: every CTA (cluster) of a 132-SM H100 runs >= 3 tiles, and N = 1032 (five 256-column tiles, the
+# last 8 columns wide) puts a partial-N tile after full ones in the same CTA (test_gemm_cases_sit_where_they_say).
+_GEMM_PERSIST = [_gc(3400, 1032, 392, i, splits=3, alpha=0.125, persist=True, gpu=True) if GEMM_KINDS[i].get("a_mn")
+                 else _gc(10200, 1032, 72, i, alpha=0.125, persist=True, gpu=True) for i in range(10)]
+# GPU-sized shapes at the epilogue settings the fused layers use (bf16: alpha 0.5 with bias and column sums, and alpha 1
+# without either; act and dact at alpha 0.125; fp32 with bias): M and N across the 128 / 256 tile boundaries with K
+# tails for every operand layout, several tiles per CTA, and (_GEMM_WIDE) every instantiation at M and N one 8-row /
+# 8-column step either side of a 256 multiple (an MN-major A keeps M a multiple of 8).
+_LEGACY_EPI = {"bf16": {"alpha": 0.5}, "act": {"alpha": 0.125}, "dact": {"alpha": 0.125}, "f32": {}}
+
+
+def _legacy(M, N, K, a_mn, b_mn, epi, act, splits):
+    kind = {"epi": ["bf16", "act", "dact", "f32"][epi], "a_mn": a_mn, "b_mn": b_mn}
+    if epi in (1, 2):
+        kind["act"] = act
+    if epi == 3:
+        kind["splits"] = splits
+    return {"M": M, "N": N, "K": K, **kind, **_LEGACY_EPI[kind["epi"]], "gpu": True}
+
+
+_GEMM_PARITY = [
+    # M, N, K, a_mn, b_mn, epi, act, splits   (epi: 0 bf16, 1 bf16 + act (two outputs), 2 bf16 x act'(aux), 3 fp32)
+    (128, 256, 64, 0, 0, 3, 0, 1), (1000, 768, 200, 0, 0, 3, 0, 1), (1000, 768, 328, 0, 0, 0, 0, 1),
+    (512, 1024, 256, 0, 0, 1, 0, 1), (1000, 712, 264, 0, 0, 1, 1, 1),
+    (1000, 768, 264, 0, 1, 0, 0, 1), (640, 512, 512, 0, 1, 2, 0, 1), (1000, 776, 192, 0, 1, 2, 1, 1),
+    (768, 768, 4096, 1, 1, 3, 0, 4), (1000, 520, 1000, 1, 1, 3, 0, 3), (520, 768, 1000, 1, 0, 3, 0, 2),
+    (300, 4, 512, 0, 0, 3, 0, 1), (8, 512, 768, 0, 1, 3, 0, 1),
+    (5000, 2304, 768, 0, 0, 0, 0, 1), (5000, 3072, 768, 0, 0, 1, 0, 1), (5000, 3072, 768, 0, 1, 2, 0, 1),
+    (2304, 768, 5000, 1, 1, 3, 0, 5),
+    (129, 136, 72, 0, 0, 0, 0, 1), (257, 200, 136, 0, 0, 1, 1, 1), (300, 264, 648, 0, 1, 2, 1, 1),
+    (384, 392, 320, 1, 0, 3, 0, 2), (640, 136, 2048, 1, 1, 3, 0, 7), (96, 1160, 64, 0, 1, 0, 0, 1),
+    (2000, 4104, 512, 0, 0, 1, 0, 1), (1500, 1032, 256, 0, 1, 2, 0, 1), (16, 8, 16, 0, 0, 3, 0, 1),
+]
+_GEMM_WIDE = [(M if not k[0] else {255: 248, 257: 264, 4097: 4104}.get(M, M), N, K) + k
+                     for M, N, K in [(255, 520, 136), (257, 264, 200), (4097, 776, 72), (1000, 1032, 584)]
+                     for k in [(0, 0, 0, 0, 1), (0, 0, 1, 0, 1), (0, 0, 1, 1, 1), (0, 0, 3, 0, 1), (0, 1, 0, 0, 1),
+                               (0, 1, 2, 0, 1), (0, 1, 2, 1, 1), (0, 1, 3, 0, 1), (1, 1, 3, 0, 3), (1, 0, 3, 0, 2)]]
+# the ViT-B/16 image tower's GEMMs at the benchmark's N and K, M cut from 100 864 tokens to 2048 rows (the FC1 wgrad:
+# its contraction over the tokens cut to 8192)
+_GEMM_TOWER = [
+    (2048, 2304, 768, 0, 0, 0, 0, 1),    # QKV projection
+    (2048, 3072, 768, 0, 0, 1, 0, 1),    # FC1 + QuickGELU
+    (2048, 768, 3072, 0, 0, 0, 0, 1),    # FC2
+    (2048, 768, 3072, 0, 1, 0, 0, 1),    # FC1 dgrad
+    (2048, 3072, 768, 0, 1, 2, 0, 1),    # FC2 dgrad x QuickGELU'
+    (768, 3072, 8192, 1, 1, 3, 0, 5),    # FC1 wgrad, split-K
+]
+_GEMM = (
+    [{"M": 128, "N": 256, "K": 192, "epi": "bf16"}, {"M": 64, "N": 128, "K": 128, "epi": "f32"}]
+    + _both_modes(_GEMM_EDGES + _GEMM_PERSIST + [_legacy(*c) for c in _GEMM_PARITY + _GEMM_WIDE + _GEMM_TOWER]
+                  + [dict(_legacy(*c), alpha=1.0, bias=False, colsum=False) for c in _GEMM_PARITY if c[5] == 0])
+    # the automatic choice: 1-CTA tiles below M = 512 or with fewer 256 x 256 tiles than SM pairs, clusters above
+    + [_gc(511, 4104, 72, 1, gpu=True), _gc(1024, 4104, 72, 1, gpu=True), _gc(512, 520, 1000, 8, splits=40, gpu=True),
+       _gc(1024, 264, 136, 6, alpha=-0.5, pad=8)]
+)
+
 # ---- cases -----------------------------------------------------------------------------------------------------------------
 _WIDTHS = [128 * nv for nv in range(1, 9)]
 
@@ -2217,7 +2459,7 @@ CASES = {
     "ce_labels_bwd": [{"M": 6, "V": 49408, "stride": 2, "n_ignored": 2, "gscale": True}, {"M": 5, "V": 97, "stride": 1},
                       {"M": 4, "V": 49408, "stride": 3, "n_ignored": 4},
                       {"M": 300, "V": 49408, "stride": 2, "n_ignored": 50, "gpu": True}],
-    "gemm": [{"M": 128, "N": 256, "K": 192, "epi": "bf16"}, {"M": 64, "N": 128, "K": 128, "epi": "f32"}],
+    "gemm": _GEMM,
     "attention_fwd": _PACKED,
     "attention_fwd_kmask": _KMASKED,
     "attention_bwd": _PACKED,
@@ -2237,7 +2479,10 @@ CASES = {
 # Kernels whose results DESIGN.md §4 documents as run-to-run bit-exact (no floating-point atomics).
 DETERMINISTIC = ["layernorm_bwd", "vit_embed_ln_bwd", "batch_sum", "colsum_bf16", "text_embed_bwd", "ce_labels",
                  "sum_scale", "contrastive_ce_stats", "contrastive_ce_grad", "gemm_ce_stats", "ce_stats_reduce",
-                 "gemm_ce_grad", "linear_cross_entropy"]
+                 "gemm_ce_grad", "linear_cross_entropy", "gemm"]
+# The ops on the GEMM kernel, whose two variants (one CTA per 128 x 256 tile, 2-CTA clusters) run the same wgmma
+# sequence per 128-row block and differ only in the tile origin and the B multicast: bit-identical results.
+GEMM_FAMILY = ["gemm", "gemm_ce_stats", "gemm_ce_grad", "linear_cross_entropy"]
 
 CHECKS = {op: globals()["check_" + op] for op in CASES}
 

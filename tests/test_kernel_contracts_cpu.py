@@ -284,7 +284,77 @@ def _linear_ce_counts_ignored(hidden, weight, labels, ignore_index, accum, row_l
     accum[1] += (labels == ignore_index).sum()
 
 
+def _gemm_k(A, kw):
+    return A.shape[0] if kw.get("a_mn") else A.shape[1]
+
+
+def _gemm_bias_every_split(A, B, **kw):
+    out = emu_ops.gemm(A, B, **kw)
+    if kw["epilogue"] == emu_ops.EPI_F32 and kw.get("bias") is not None:
+        out += (KC._gemm_splits(_gemm_k(A, kw), kw.get("splits", 1), "f32") - 1) * kw["bias"]
+    return out
+
+
+def _gemm_act_of_fp32_pre(A, B, **kw):
+    res = emu_ops.gemm(A, B, **kw)
+    if kw["epilogue"] == emu_ops.EPI_BF16_ACT:
+        pre = emu_ops.gemm(A, B, **dict(kw, epilogue=emu_ops.EPI_F32, out=None, out2=None))
+        res[1].copy_(emu_ops._act(pre, kw.get("act", 0)).to(torch.bfloat16))
+    return res
+
+
+def _gemm_colsum_unrounded(A, B, *, colsum=None, **kw):
+    res = emu_ops.gemm(A, B, **kw)
+    if colsum is not None:
+        pre = emu_ops.gemm(A, B, **dict(kw, epilogue=emu_ops.EPI_F32, out=None, aux=None))
+        if kw["epilogue"] == emu_ops.EPI_BF16_DACT:
+            pre = pre * emu_ops._act_grad(kw["aux"].float(), kw.get("act", 0))
+        colsum.add_(pre.sum(0))
+    return res
+
+
+def _gemm_colsum_assigns(A, B, *, colsum=None, **kw):
+    if colsum is not None:
+        colsum.zero_()
+    return emu_ops.gemm(A, B, colsum=colsum, **kw)
+
+
+def _gemm_drops_partial_k_block(A, B, **kw):
+    k0 = _gemm_k(A, kw) // 64 * 64
+    A = A[:k0] if kw.get("a_mn") else A[:, :k0]
+    B = B[:k0] if kw.get("b_mn") else B[:, :k0]
+    return emu_ops.gemm(A, B, **kw)
+
+
+def _gemm_dact_ignores_alpha(A, B, **kw):
+    if kw["epilogue"] == emu_ops.EPI_BF16_DACT:
+        kw["alpha"] = 1.0
+    return emu_ops.gemm(A, B, **kw)
+
+
+def _gemm_splitk_ignores_accumulate(A, B, **kw):
+    if kw["epilogue"] == emu_ops.EPI_F32 and KC._gemm_splits(_gemm_k(A, kw), kw.get("splits", 1), "f32") > 1:
+        kw["accumulate"] = False
+    return emu_ops.gemm(A, B, **kw)
+
+
+def _gemm_writes_row_padding(A, B, *, out=None, **kw):
+    res = emu_ops.gemm(A, B, out=out, **kw)
+    if out is not None and out.stride(0) > out.shape[1]:
+        rows = torch.as_strided(out, (out.shape[0], out.stride(0)), out.stride(), out.storage_offset())
+        rows[:, out.shape[1]:] = 0
+    return res
+
+
 MUTANTS = {
+    "gemm adds the bias in every split": ("gemm", "gemm", _gemm_bias_every_split),
+    "gemm applies the activation to the fp32 pre-activation": ("gemm", "gemm", _gemm_act_of_fp32_pre),
+    "gemm column sums over the unrounded output": ("gemm", "gemm", _gemm_colsum_unrounded),
+    "gemm column sums assigned instead of accumulated": ("gemm", "gemm", _gemm_colsum_assigns),
+    "gemm drops the last partial k-block": ("gemm", "gemm", _gemm_drops_partial_k_block),
+    "gemm act' epilogue ignores alpha": ("gemm", "gemm", _gemm_dact_ignores_alpha),
+    "split-K gemm ignores accumulate": ("gemm", "gemm", _gemm_splitk_ignores_accumulate),
+    "gemm writes the padding columns between N and ld": ("gemm", "gemm", _gemm_writes_row_padding),
     "cast truncates instead of rounding": ("cast_bf16", "cast_bf16", _truncating_cast_bf16),
     "LayerNorm backward skips the last row": ("layernorm_bwd", "layernorm_bwd", _ln_bwd_skips_last_row),
     "rows_per_group ignored": ("add_layernorm_fwd", "add_layernorm_fwd", _ln_fwd_ignores_rows_per_group),
@@ -361,6 +431,47 @@ def test_attention_cases_sit_where_they_say():
     assert set(KC._STREAMED.values()) == {0, 1}
     for c in KC.CASES["attention_fwd_decode"]:
         assert lib.mmb_attention_decode_splits(c["B"], c["H"], c["Skv"]) == c.get("splits", 1), c
+
+
+def test_gemm_cases_sit_where_they_say():
+    """The persistent-loop GEMM cases give every CTA (2-CTA cluster) of a 132-SM H100 at least 3 tiles, and some CTA
+    a partial-N tile right after a full one (tile t runs on unit t mod units, n_blk = t mod n_tiles within a split);
+    together they cover every instantiation in both variants."""
+    seen = set()
+    for c in KC.CASES["gemm"]:
+        if not c.get("persist"):
+            continue
+        clu = c["gemm_mode"] == 1
+        units = KC.H100_SMS // 2 if clu else KC.H100_SMS
+        m_tiles, n_tiles = KC._cdiv(c["M"], 256 if clu else 128), KC._cdiv(c["N"], 256)
+        tiles = m_tiles * n_tiles * KC._gemm_splits(c["K"], c.get("splits", 1), c["epi"])
+        assert tiles // units >= 3, c
+        assert c["N"] % 256 and n_tiles > 1, c
+        n_blk = lambda t: t % (m_tiles * n_tiles) % n_tiles  # noqa: E731
+        assert any(n_blk(t) < n_tiles - 1 and n_blk(t + units) == n_tiles - 1 for t in range(tiles - units)), c
+        seen.add((KC._gemm_kind_key(c), c["gemm_mode"]))
+    assert seen == {(KC._gemm_kind_key(k), m) for k in KC.GEMM_KINDS for m in (0, 1)}
+
+
+def test_gemm_cases_cover_every_instantiation_on_the_cpu():
+    """The CPU cases reach every instantiation, so each emulation mutant meets the epilogue it breaks."""
+    cpu = {KC._gemm_kind_key(c) for c in KC.CASES["gemm"] if not c.get("gpu")}
+    assert cpu == {KC._gemm_kind_key(k) for k in KC.GEMM_KINDS}
+
+
+@pytest.mark.parametrize("epilogue,accumulate,bias", [(0, 1, False), (1, 1, False), (2, 1, False), (2, 0, True)],
+                         ids=["bf16_accumulate", "act_accumulate", "dact_accumulate", "dact_bias"])
+def test_gemm_refuses_accumulate_and_bias_its_epilogue_would_ignore(epilogue, accumulate, bias):
+    """mmb_gemm_bf16 returns MMB_ERR_ARG before touching any pointer: only EPI_F32 adds into D0, and
+    EPI_BF16_DACT has no bias term (D0 = bf16(alpha acc act'(aux)))."""
+    from multimodal_b200 import _lib
+
+    null = ctypes.c_void_p(0)
+    host = (ctypes.c_float * 64)()        # a real address that the refused call never reads
+    b = ctypes.cast(host, ctypes.c_void_p) if bias else null
+    rc = _lib.lib().mmb_gemm_bf16(null, 8, 0, null, 8, int(epilogue == 2), null, 8, null, 8, 8, 8, 8, epilogue, 0,
+                                  ctypes.c_float(1.0), b, null, 8, 1, accumulate, null, null)
+    assert rc == -22, rc     # MMB_ERR_ARG
 
 
 # ---- zero-size calls ---------------------------------------------------------------------------------------------------
