@@ -23,10 +23,11 @@ extern "C" {
 /* GEMM epilogues (mmb_gemm_bf16) */
 #define MMB_EPI_BF16 0      /* D0 = bf16(alpha*acc + bias)                                   */
 #define MMB_EPI_BF16_ACT 1  /* D0 = bf16(pre = alpha*acc + bias), D1 = bf16(act(D0))         */
-#define MMB_EPI_BF16_DACT 2 /* D0 = bf16(alpha*acc * act'(aux))                              */
+#define MMB_EPI_BF16_DACT 2 /* D0 = bf16(alpha*acc * act'(aux)); ReLU: aux > 0 ? alpha*acc : +0 */
 #define MMB_EPI_F32 3       /* D0 = fp32(alpha*acc + bias) (+ D0 when accumulate); split-K summed in a fixed order */
 #define MMB_ACT_QUICK_GELU 0 /* torchmultimodal/modules/layers/activation.py:12-25 ("SiLU")  */
 #define MMB_ACT_GELU_ERF 1   /* nn.GELU(), torchmultimodal/modules/layers/mlp.py             */
+#define MMB_ACT_RELU 2       /* nn.ReLU(), the default of MLP and the transformer layers      */
 
 int mmb_version(void);
 
@@ -181,7 +182,8 @@ int mmb_anyprecision_adamw_step(float* p, float* g, void* m, int m_dtype, void* 
                                 void* stream);
 int mmb_memset_async(void* p, int value, long long bytes, void* stream);
 /* Standalone activation, fp32: kind MMB_ACT_QUICK_GELU = x*sigmoid(1.702x) (modules/layers/activation.py:24-25),
- * MMB_ACT_GELU_ERF = nn.GELU().  (Inside the encoders the activation is a GEMM epilogue.) */
+ * MMB_ACT_GELU_ERF = nn.GELU(), MMB_ACT_RELU = max(x, 0) (exact).  (Inside the encoders the activation is a GEMM
+ * epilogue.) */
 int mmb_act_fwd(const float* x, float* y, long long n, int kind, void* stream);
 
 /* ---- attention --------------------------------------------------------------------------------------------- */
@@ -279,7 +281,8 @@ int mmb_scatter_rows_idx_add(const float* src, const long long* idx, float* dst,
 int mmb_ce_labels_bwd(const float* logits, long long ld, const long long* labels, long long label_stride,
                       long long ignore_index, int M, int V, const float* accum, float grad_scale,
                       const float* grad_scale_dev, void* dlogits_bf16, long long ldd, void* stream);
-/* dx = bf16(dy * act'(pre)), bf16 tensors of n elements; kind = ACT_QUICK_GELU (0) / ACT_GELU_ERF (1): the activation
+/* dx = bf16(dy * act'(pre)), bf16 tensors of n elements; kind = ACT_QUICK_GELU (0) / ACT_GELU_ERF (1) / ACT_RELU (2,
+ * dx = pre > 0 ? dy : +0 exactly): the activation
  * backward outside a GEMM epilogue (MaskedPredictionHead transform, modules/losses/flava.py:174-180 under autograd). */
 int mmb_act_bwd(const void* dy_bf16, const void* pre_bf16, void* dx_bf16, long long n, int kind, void* stream);
 

@@ -313,8 +313,17 @@ __device__ __forceinline__ float gelu_erf_grad(float x) {
   return 0.5f * (1.f + erff(x * 0.70710678118654752f)) + x * 0.3989422804014327f * ex2_approx(-0.7213475204444817f * x * x);
 }
 template <int ACT>
-__device__ __forceinline__ float act_fn(float x) { return ACT == 0 ? quick_gelu(x) : gelu_erf(x); }
+__device__ __forceinline__ float act_fn(float x) {
+  if constexpr (ACT == 2) return fmaxf(x, 0.f);   // nn.ReLU (the reference default of MLP and the transformer layers)
+  else return ACT == 0 ? quick_gelu(x) : gelu_erf(x);
+}
 template <int ACT>
 __device__ __forceinline__ float act_grad(float x) { return ACT == 0 ? quick_gelu_grad(x) : gelu_erf_grad(x); }
+// g * act'(pre).  ReLU selects instead of multiplying by 0 / 1, so the result is g or +0 exactly (no -0, no NaN * 0)
+template <int ACT>
+__device__ __forceinline__ float act_dgrad(float g, float pre) {
+  if constexpr (ACT == 2) return pre > 0.f ? g : 0.f;
+  else return g * act_grad<ACT>(pre);
+}
 
 }  // namespace mmb

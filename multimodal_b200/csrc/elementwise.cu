@@ -915,6 +915,11 @@ __global__ void act_fwd_kernel(const float* __restrict__ x, float* __restrict__ 
     y[i] = kind == ACT_QUICK_GELU ? v / (1.f + __expf(-1.702f * v)) : 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
   }
 }
+// nn.ReLU() called on its own, exact: a kernel of its own so that the GELU kinds' kernel stays as it is
+__global__ void relu_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    y[i] = fmaxf(x[i], 0.f);
+}
 
 }  // namespace mmb
 
@@ -1202,7 +1207,8 @@ extern "C" int mmb_anyprecision_adamw_step(float* p, float* g, void* m, int m_dt
 
 extern "C" int mmb_act_fwd(const float* x, float* y, long long n, int kind, void* stream) {
   if (n <= 0) return MMB_OK;
-  if (kind != ACT_QUICK_GELU && kind != ACT_GELU_ERF) return MMB_ERR_ARG;
-  act_fwd_kernel<<<grid_for(n, 256), 256, 0, ST(stream)>>>(x, y, n, kind);
+  if (kind == ACT_RELU) relu_fwd_kernel<<<grid_for(n, 256), 256, 0, ST(stream)>>>(x, y, n);
+  else if (kind == ACT_QUICK_GELU || kind == ACT_GELU_ERF) act_fwd_kernel<<<grid_for(n, 256), 256, 0, ST(stream)>>>(x, y, n, kind);
+  else return MMB_ERR_ARG;
   return LAUNCH_RC();
 }

@@ -262,10 +262,10 @@ __global__ void act_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_
   const long long n2 = n >> 1;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n2; i += (long long)gridDim.x * blockDim.x) {
     const uint32_t a = reinterpret_cast<const uint32_t*>(dy)[i], b = reinterpret_cast<const uint32_t*>(pre)[i];
-    reinterpret_cast<uint32_t*>(dx)[i] = pack_bf16x2(bf16_lo(a) * act_grad<ACT>(bf16_lo(b)), bf16_hi(a) * act_grad<ACT>(bf16_hi(b)));
+    reinterpret_cast<uint32_t*>(dx)[i] = pack_bf16x2(act_dgrad<ACT>(bf16_lo(a), bf16_lo(b)), act_dgrad<ACT>(bf16_hi(a), bf16_hi(b)));
   }
   if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0)
-    dx[n - 1] = __float2bfloat16(__bfloat162float(dy[n - 1]) * act_grad<ACT>(__bfloat162float(pre[n - 1])));
+    dx[n - 1] = __float2bfloat16(act_dgrad<ACT>(__bfloat162float(dy[n - 1]), __bfloat162float(pre[n - 1])));
 }
 
 }  // namespace mmb
@@ -346,6 +346,7 @@ extern "C" int mmb_act_bwd(const void* dy_bf16, const void* pre_bf16, void* dx_b
   const __nv_bfloat16 *dy = (const __nv_bfloat16*)dy_bf16, *pre = (const __nv_bfloat16*)pre_bf16;
   if (kind == ACT_QUICK_GELU) act_bwd_kernel<0><<<grid_cap(n / 2 + 1, 256), 256, 0, ST(stream)>>>(dy, pre, (__nv_bfloat16*)dx_bf16, n);
   else if (kind == ACT_GELU_ERF) act_bwd_kernel<1><<<grid_cap(n / 2 + 1, 256), 256, 0, ST(stream)>>>(dy, pre, (__nv_bfloat16*)dx_bf16, n);
+  else if (kind == ACT_RELU) act_bwd_kernel<2><<<grid_cap(n / 2 + 1, 256), 256, 0, ST(stream)>>>(dy, pre, (__nv_bfloat16*)dx_bf16, n);
   else return MMB_ERR_ARG;
   return LAUNCH_RC();
 }

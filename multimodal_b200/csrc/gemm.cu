@@ -414,8 +414,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 }
                 if (EPI == EPI_BF16_DACT) {
                   const uint32_t av = *sp;   // pre-activation, loaded into this very slot by TMA
-                  f0 *= act_grad<ACT>(bf16_lo(av));
-                  f1 *= act_grad<ACT>(bf16_hi(av));
+                  f0 = act_dgrad<ACT>(f0, bf16_lo(av));
+                  f1 = act_dgrad<ACT>(f1, bf16_hi(av));
                 }
                 uint32_t o = pack_bf16x2(f0, f1);
                 // the activation is applied to the bf16-ROUNDED pre-activation: exactly what the backward (which only
@@ -750,10 +750,12 @@ static int gemm_launch(int a_mn_major, int b_mn_major, int epilogue, int act, bo
   MMB_CASE(0, 0, EPI_BF16, -1)
   MMB_CASE(0, 0, EPI_BF16_ACT, ACT_QUICK_GELU)
   MMB_CASE(0, 0, EPI_BF16_ACT, ACT_GELU_ERF)
+  MMB_CASE(0, 0, EPI_BF16_ACT, ACT_RELU)
   MMB_CASE(0, 0, EPI_F32, -1)
   MMB_CASE(0, 1, EPI_BF16, -1)
   MMB_CASE(0, 1, EPI_BF16_DACT, ACT_QUICK_GELU)
   MMB_CASE(0, 1, EPI_BF16_DACT, ACT_GELU_ERF)
+  MMB_CASE(0, 1, EPI_BF16_DACT, ACT_RELU)
   MMB_CASE(0, 1, EPI_F32, -1)
   MMB_CASE(1, 1, EPI_F32, -1)
   MMB_CASE(1, 0, EPI_F32, -1)

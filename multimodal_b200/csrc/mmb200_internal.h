@@ -19,6 +19,7 @@
 
 #define ACT_QUICK_GELU 0
 #define ACT_GELU_ERF 1
+#define ACT_RELU 2
 
 namespace mmb {
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, bool is_f32, uint64_t inner, uint64_t outer,

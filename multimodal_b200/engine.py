@@ -255,7 +255,9 @@ def act_code(act: nn.Module) -> int:
         return ops.ACT_GELU_ERF
     if isinstance(act, SiLU):
         return ops.ACT_QUICK_GELU
-    raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU / SiLU)")
+    if isinstance(act, nn.ReLU):
+        return ops.ACT_RELU
+    raise MMBError(f"unsupported MLP activation {type(act).__name__} on the accelerated path (nn.GELU / SiLU / nn.ReLU)")
 
 
 def scaled(scale: Optional[torch.Tensor], rows_per_scale: int) -> dict:

@@ -7,11 +7,11 @@ exposes — and tests — on their own are callable outside an encoder:
   modules/layers/mlp.py:13-66                    MLP ([Linear, activation, Linear] form)
 
 They launch exactly the kernels the fused encoder schedules launch (wgmma GEMMs with bias / activation epilogues,
-tensor-core attention, the add+LayerNorm kernel); nothing is computed by PyTorch.  Pre-norm `TransformerEncoderLayer` /
-`TransformerEncoder` run on one runtime per module in both grad modes (`EncoderLayersRuntime` on `engine.ModuleStack`:
-the CLIP towers' fused forward / backward schedule, `infer` under torch.no_grad()); the other standalone modules,
-post-norm layers included, compute forward values only, and asking them for an autograd graph raises instead of
-returning detached tensors.
+tensor-core attention, the add+LayerNorm kernel); nothing is computed by PyTorch.  `TransformerEncoderLayer` /
+`TransformerEncoder` run on one runtime per module in both grad modes, `infer` under torch.no_grad(): pre-norm layers on
+`EncoderLayersRuntime` (`engine.ModuleStack`: the CLIP towers' fused forward / backward schedule), post-norm layers (the
+reference default) on `PostNormLayersRuntime`, a schedule of their own.  The other standalone modules compute forward
+values only, and asking them for an autograd graph raises instead of returning detached tensors.
   modules/layers/multi_head_attention.py:83-180  MultiHeadAttentionWithCache (key / value cache, cross-attention)
   modules/layers/transformer.py:262-657          TransformerDecoderLayer (pre- and post-norm), TransformerDecoder
 
@@ -31,7 +31,7 @@ from torch import nn
 
 from . import ops
 from ._lib import MMBError
-from .engine import ModuleStack, Workspace, _Shadows, act_code, as_f32, patch_embed_fwd, run, scaled
+from .engine import ModuleStack, ParamStore, Workspace, _Shadows, act_code, as_f32, patch_embed_fwd, run, scaled
 from .modules.layers.stochastic_depth import drop_path_scales
 
 
@@ -187,10 +187,178 @@ class EncoderLayersRuntime:
         return (G.view(B, S, d).clone(),)
 
 
-def _pre_norm_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask: Optional[torch.Tensor], what: str,
-                      return_hidden_states: bool = False):
-    """A pre-norm TransformerEncoderLayer / TransformerEncoder on its EncoderLayersRuntime -> (output, hidden_states or
-    None).  With an autograd graph the output is fp32."""
+class PostNormLayersRuntime:
+    """A standalone post-norm `TransformerEncoderLayer` or `TransformerEncoder` (modules/layers/transformer.py:113-128,
+    216-259) in both grad modes, with the same interface as EncoderLayersRuntime.  Per layer, x1 = LN1(x + s_a Attn(x))
+    and out = LN2(x1 + s_f FF(x1)) (s_a / s_f: stochastic-depth factors, 1 without drop path), then the optional final
+    LayerNorm.  Its own schedule, not TransformerStack's: there each LayerNorm feeds a branch, here it closes one.
+
+    The backward runs the LayerNorm backward on the fp32 gradient of its output (no residual gradient comes in: the
+    residual stream is the normalised one), and the FC1 / QKV input gradients are fp32 GEMMs that accumulate into the
+    gradient that left that LayerNorm, which forms dx1 = dS2 + W1^T dPRE and dx = dS1 + Wqkv^T dQKV in place."""
+
+    def __init__(self, owner: nn.Module, layers, final_ln: Optional[nn.Module]):
+        self.layers = list(layers)
+        self.final_ln = final_ln
+        self.store = ParamStore(list(owner.parameters()))
+        self.device = self.store.device
+        self.ws = Workspace(self.device)
+        l0 = self.layers[0]
+        self.d = l0.attention_layernorm.normalized_shape[0]
+        self.H = l0.attention.num_heads
+        self.hd = self.d // self.H
+        if self.d % self.H or self.hd not in (64, 96, 128):
+            raise MMBError(f"TransformerEncoderLayer: head_dim {self.d / self.H:g} is not supported by the attention "
+                           "kernels")
+        mlp = l0.feedforward.model
+        self.ff = mlp[0].weight.shape[0]
+        self.act = act_code(mlp[1])
+
+    def _forward(self, x: torch.Tensor, mask_u8, save: Optional[Workspace], hidden: Optional[List[torch.Tensor]]):
+        """-> the output fp32 [B*S, d].  hidden: receives each layer's output fp32 [B, S, d] (fresh tensors).  A bf16 x
+        without `save` rounds each layer's output to bf16 before the next layer reads it, as the layer-at-a-time call
+        does when each layer returns in its input's dtype."""
+        st, d, H, hd, ff = self.store, self.d, self.H, self.hd, self.ff
+        B, S, _ = x.shape
+        M = B * S
+        bf, f32 = torch.bfloat16, torch.float32
+        if save is not None and hd != 64:
+            raise MMBError(f"training needs head_dim 64 in the layer stacks (got {hd}); call it under torch.no_grad()")
+        st.refresh()
+        if save is None:
+            buf = lambda name, l, shape, dt: self.ws.get(f"pn.{name}", shape, dt)  # noqa: E731
+        else:
+            buf = lambda name, l, shape, dt: save.get(f"pn.{name}.{l}", shape, dt)  # noqa: E731
+        round_bf16 = save is None and x.dtype == bf
+        scales = drop_path_scales(self.layers, B, self.device)   # training with drop_path_rate: once, for all layers
+        if save is not None:
+            save.mask, save.B, save.S, save.scales = mask_u8, B, S, scales
+        X = x.contiguous().float().view(M, d)      # only read: the residual add of the first layer
+        Xb = buf("Xb", 0, (M, d), bf)
+        ops.cast_bf16(X.view(-1), Xb.view(-1))
+        QKV0, O0 = self.ws.get("pn.QKV", (M, 3 * d), bf), self.ws.get("pn.O", (M, d), bf)
+        Y = self.ws.get("pn.Y", (M, d), bf)
+        for l, layer in enumerate(self.layers):
+            at, mlp = layer.attention, layer.feedforward.model
+            ln1, ln2 = layer.attention_layernorm, layer.feedforward_layernorm
+            s_a, s_f = scales[l] if scales is not None else (None, None)
+            keep = save is not None
+            QKV = buf("QKV", l, (M, 3 * d), bf) if keep else QKV0
+            O = buf("O", l, (M, d), bf) if keep else O0
+            LSE = buf("LSE", l, (B * H * S,), f32)
+            S1 = buf("S1", l, (M, d), f32) if keep else None          # x + s_a Attn(x): LN1's input
+            X1 = buf("X1", l, (M, d), f32)                             # LN1's output, fp32 + its bf16 operand copy
+            X1b = buf("X1b", l, (M, d), bf)
+            PRE, HACT = buf("PRE", l, (M, ff), bf), buf("HACT", l, (M, ff), bf)
+            S2 = buf("S2", l, (M, d), f32) if keep else None          # x1 + s_f FF(x1): LN2's input
+            m1, r1, m2, r2 = ((buf(n, l, (M,), f32) for n in ("m1", "r1", "m2", "r2")) if keep else (None,) * 4)
+            last = l == len(self.layers) - 1
+            OUT = (torch.empty((M, d), device=self.device, dtype=f32) if hidden is not None or last
+                   else self.ws.get(f"pn.X{l % 2}", (M, d), f32))
+            OUTb = buf("Xb", l + 1, (M, d), bf) if not last or round_bf16 else None   # the next QKV GEMM's operand
+            ops.gemm(Xb, st.shadow(at.input_proj.weight), bias=at.input_proj.bias, out=QKV)
+            ops.self_attention(QKV, O, LSE, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
+            ops.gemm(O, st.shadow(at.output_proj.weight), bias=at.output_proj.bias, out=Y)
+            ops.add_layernorm_fwd(X, Y, S1, X1b, X1, ln1.weight, ln1.bias, m1, r1, M, d, ln1.eps, **scaled(s_a, S))
+            ops.gemm(X1b, st.shadow(mlp[0].weight), bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT,
+                     act=self.act)
+            ops.gemm(HACT, st.shadow(mlp[-1].weight), bias=mlp[-1].bias, out=Y)
+            ops.add_layernorm_fwd(X1, Y, S2, OUTb, OUT, ln2.weight, ln2.bias, m2, r2, M, d, ln2.eps, **scaled(s_f, S))
+            if round_bf16:
+                ops.cast_f32(OUTb, OUT)
+            if hidden is not None:
+                hidden.append(OUT.view(B, S, d))
+            X, Xb = OUT, OUTb
+        fln = self.final_ln
+        if save is not None:
+            save.XF = X
+        if fln is None:
+            return X
+        LAST = torch.empty((M, d), device=self.device, dtype=f32)
+        stats = save if save is not None else self.ws
+        ops.add_layernorm_fwd(X, None, None, None, LAST, fln.weight, fln.bias, stats.get("pn.mF", (M,), f32),
+                              stats.get("pn.rF", (M,), f32), M, d, fln.eps)
+        return LAST
+
+    def forward(self, data, diff):
+        """data: (uint8 [B, S, S] mask or None, the caller's list that receives hidden_states or None)."""
+        mask_u8, hidden = data
+        (x,) = diff
+        save = Workspace(self.device)
+        if hidden is not None:
+            hidden.append(x)
+        out = self._forward(x, mask_u8, save, hidden)
+        return (out.view(x.shape),), save
+
+    def infer(self, x: torch.Tensor, mask_u8: Optional[torch.Tensor], return_hidden_states: bool = False):
+        """-> (output [B, S, d], hidden_states or None), in x's dtype.  hidden_states: x itself, then each layer's
+        output (the last one before the final LayerNorm)."""
+        hidden: Optional[List[torch.Tensor]] = [] if return_hidden_states else None
+        out = self._forward(x, mask_u8, None, hidden)
+        if hidden is not None:
+            hidden = [x] + [h.to(x.dtype) for h in hidden]
+        return out.view(x.shape).to(x.dtype), hidden
+
+    def backward(self, save, dOUT):
+        st, d, H, hd, ff = self.store, self.d, self.H, self.hd, self.ff
+        B, S, mask_u8 = save.B, save.S, save.mask
+        M = B * S
+        bf, f32 = torch.bfloat16, torch.float32
+        sp = ops.wgrad_splits
+        scales = save.scales
+        G = as_f32(dOUT, (M, d))                 # the gradient of the current layer's output, read only
+        GA, GB = self.ws.get("pn.GA", (M, d), f32), self.ws.get("pn.GB", (M, d), f32)   # dS1 / dx, dS2 / dx1
+        Gb = self.ws.get("pn.Gb", (M, d), bf)
+        T1, T3 = self.ws.get("pn.T1", (M, d), bf), self.ws.get("pn.T3", (M, 3 * d), bf)
+        fln = self.final_ln
+        if fln is not None:
+            ops.layernorm_bwd(save.XF, None, G, save.get("pn.mF", (M,), f32), save.get("pn.rF", (M,), f32), fln.weight,
+                              None, GA, None, st.grad(fln.weight), st.grad(fln.bias), M, d)
+            G = GA
+        for l in range(len(self.layers) - 1, -1, -1):
+            layer = self.layers[l]
+            at, mlp = layer.attention, layer.feedforward.model
+            ln1, ln2 = layer.attention_layernorm, layer.feedforward_layernorm
+            s_a, s_f = scales[l] if scales is not None else (None, None)
+            g = lambda n, shape, dt: save.get(f"pn.{n}.{l}", shape, dt)  # noqa: E731
+            Xb, QKV, O = g("Xb", (M, d), bf), g("QKV", (M, 3 * d), bf), g("O", (M, d), bf)
+            LSE = g("LSE", (B * H * S,), f32)
+            S1, X1b, S2 = g("S1", (M, d), f32), g("X1b", (M, d), bf), g("S2", (M, d), f32)
+            PRE, HACT = g("PRE", (M, ff), bf), g("HACT", (M, ff), bf)
+            m1, r1, m2, r2 = (g(n, (M,), f32) for n in ("m1", "r1", "m2", "r2"))
+            w1, w2 = mlp[0].weight, mlp[-1].weight
+            dS2, dS1 = GB, GA   # G (GA below the top layer) is dead once LN2's backward has read it
+            # ---- LN2:  dS2 = dLN2/dS2 (fp32), Gb = bf16(s_f dS2) enters the feed-forward branch ----
+            ops.layernorm_bwd(S2, None, G, m2, r2, ln2.weight, None, dS2, Gb, st.grad(ln2.weight), st.grad(ln2.bias),
+                              M, d, gsum=st.grad(mlp[-1].bias), **scaled(s_f, S))
+            ops.gemm(Gb, HACT, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(w2), splits=sp(d, ff, M),
+                     accumulate=True)
+            dPRE = HACT   # the activation output is dead once its wgrad has been issued (same stream)
+            ops.gemm(Gb, st.shadow(w2), b_mn=True, epilogue=ops.EPI_BF16_DACT, aux=PRE, out=dPRE, act=self.act,
+                     colsum=st.grad(mlp[0].bias))
+            ops.gemm(dPRE, X1b, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(w1), splits=sp(ff, d, M),
+                     accumulate=True)
+            ops.gemm(dPRE, st.shadow(w1), b_mn=True, epilogue=ops.EPI_F32, out=dS2, accumulate=True)   # dx1
+            # ---- LN1:  dS1 = dLN1/dS1, Gb = bf16(s_a dS1) enters the attention branch ----
+            ops.layernorm_bwd(S1, None, dS2, m1, r1, ln1.weight, None, dS1, Gb, st.grad(ln1.weight), st.grad(ln1.bias),
+                              M, d, gsum=st.grad(at.output_proj.bias), **scaled(s_a, S))
+            ops.gemm(Gb, O, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(at.output_proj.weight),
+                     splits=sp(d, d, M), accumulate=True)
+            ops.gemm(Gb, st.shadow(at.output_proj.weight), b_mn=True, out=T1)   # dO
+            ops.self_attention(QKV, O, LSE, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8, dout=T1, dqkv=T3)
+            ops.gemm(T3, Xb, a_mn=True, b_mn=True, epilogue=ops.EPI_F32, out=st.grad(at.input_proj.weight),
+                     splits=sp(3 * d, d, M), accumulate=True)
+            ops.colsum_bf16(T3, st.grad(at.input_proj.bias), M, 3 * d, 3 * d)
+            ops.gemm(T3, st.shadow(at.input_proj.weight), b_mn=True, epilogue=ops.EPI_F32, out=dS1, accumulate=True)
+            G = dS1   # dx: the gradient of the layer below's output
+        return (G.view(B, S, d).clone(),)
+
+
+def _runtime_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask: Optional[torch.Tensor], what: str,
+                     return_hidden_states: bool = False):
+    """A TransformerEncoderLayer / TransformerEncoder on its runtime (EncoderLayersRuntime for pre-norm layers,
+    PostNormLayersRuntime for post-norm ones) -> (output, hidden_states or None).  With an autograd graph the output
+    is fp32."""
     B, S, _ = hidden_states.shape
     if _wants_graph(mod, hidden_states):
         hidden = [] if return_hidden_states else None
@@ -203,71 +371,20 @@ def _pre_norm_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mas
 
 def encoder_layer_forward(mod: nn.Module, hidden_states: torch.Tensor,
                           attention_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """TransformerEncoderLayer.forward (transformer.py:95-154): pre-norm (:95-111) on its runtime, post-norm
-    (:113-128) forward-only.  With a drop_path_rate in training, each branch is scaled per sample inside the residual
-    add that follows it."""
-    if mod.norm_first:
-        return _pre_norm_forward(mod, hidden_states, attention_mask, "TransformerEncoderLayer")[0]
-    if _wants_graph(mod, hidden_states):
-        raise MMBError("standalone post-norm TransformerEncoderLayer has no backward schedule; call it under "
-                       "torch.no_grad()")
-    _cuda(hidden_states, "TransformerEncoderLayer")
-    B, S, d = hidden_states.shape
-    at, mlp = mod.attention, mod.feedforward.model
-    H = at.num_heads
-    hd = d // H
-    if d % H or hd not in (64, 96, 128):
-        raise MMBError(f"TransformerEncoderLayer: head_dim {d / H:g} is not supported by the attention kernels")
-    rt = _rt(mod, hidden_states.device)
-    ws, sh = rt.ws, rt.sh
-    M = B * S
-    bf, f32 = torch.bfloat16, torch.float32
-    act = act_code(mlp[1])
-    ff = mlp[0].weight.shape[0]
-    mask_u8 = _bool_mask_u8(attention_mask, B, S, "TransformerEncoderLayer")
-    X = hidden_states.contiguous().float().view(M, d)
-    LN, QKV, O = ws.get("l.LN", (M, d), bf), ws.get("l.QKV", (M, 3 * d), bf), ws.get("l.O", (M, d), bf)
-    Y, PRE, HACT = ws.get("l.Y", (M, d), bf), ws.get("l.PRE", (M, ff), bf), ws.get("l.HACT", (M, ff), bf)
-    ln1, ln2 = mod.attention_layernorm, mod.feedforward_layernorm
-    wqkv, wo = sh.get("wqkv", [at.input_proj.weight]), sh.get("wo", [at.output_proj.weight])
-    w1, w2 = sh.get("w1", [mlp[0].weight]), sh.get("w2", [mlp[-1].weight])
-    out = torch.empty((M, d), device=X.device, dtype=f32)
-    scales = drop_path_scales([mod], B, X.device)
-    s_attn, s_ff = scales[0] if scales is not None else (None, None)
-    ops.cast_bf16(X.view(-1), LN.view(-1))                 # attention(x) on the raw input
-    ops.gemm(LN, wqkv, bias=at.input_proj.bias, out=QKV)
-    ops.self_attention(QKV, O, None, B, S, H, hd, False, 1.0 / math.sqrt(hd), mask=mask_u8)
-    ops.gemm(O, wo, bias=at.output_proj.bias, out=Y)
-    H1 = ws.get("l.H1", (M, d), f32)                       # LN1(x + attention(x)), fp32 + its bf16 operand copy
-    ops.add_layernorm_fwd(X, Y, None, LN, H1, ln1.weight, ln1.bias, None, None, M, d, ln1.eps, **scaled(s_attn, S))
-    ops.gemm(LN, w1, bias=mlp[0].bias, epilogue=ops.EPI_BF16_ACT, out=PRE, out2=HACT, act=act)
-    ops.gemm(HACT, w2, bias=mlp[-1].bias, out=Y)
-    ops.add_layernorm_fwd(H1, Y, None, None, out, ln2.weight, ln2.bias, None, None, M, d, ln2.eps, **scaled(s_ff, S))
-    return out.view(B, S, d).to(hidden_states.dtype)
+    """TransformerEncoderLayer.forward (transformer.py:95-154), pre-norm (:95-111) or post-norm (:113-128), on the
+    layer's runtime.  With a drop_path_rate in training, each branch is scaled per sample inside the residual add that
+    follows it."""
+    return _runtime_forward(mod, hidden_states, attention_mask, "TransformerEncoderLayer")[0]
 
 
 def encoder_forward(mod: nn.Module, hidden_states: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
                     return_hidden_states: bool = False):
-    """TransformerEncoder.forward (transformer.py:216-259): the layers (+ optional final LayerNorm); pre-norm on the
-    encoder's runtime, post-norm forward-only, one layer at a time."""
+    """TransformerEncoder.forward (transformer.py:216-259): the layers (+ optional final LayerNorm) on the encoder's
+    runtime."""
     from .modules.layers.transformer import TransformerOutput
 
-    if all(layer.norm_first for layer in mod.layer):
-        out, hidden = _pre_norm_forward(mod, hidden_states, attention_mask, "TransformerEncoder", return_hidden_states)
-        return TransformerOutput(last_hidden_state=out, hidden_states=hidden)
-    if _wants_graph(mod, hidden_states):
-        raise MMBError("standalone post-norm TransformerEncoder has no backward schedule; call it under torch.no_grad()")
-    _cuda(hidden_states, "TransformerEncoder")
-    x = hidden_states
-    all_hidden = [x] if return_hidden_states else None
-    with torch.no_grad():
-        for layer in mod.layer:
-            x = encoder_layer_forward(layer, x, attention_mask)
-            if return_hidden_states:
-                all_hidden.append(x)
-        if mod.final_layer_norm is not None:
-            x = mod.final_layer_norm(x)
-    return TransformerOutput(last_hidden_state=x, hidden_states=all_hidden)
+    out, hidden = _runtime_forward(mod, hidden_states, attention_mask, "TransformerEncoder", return_hidden_states)
+    return TransformerOutput(last_hidden_state=out, hidden_states=hidden)
 
 
 def patch_embeddings_forward(mod: nn.Module, image: torch.Tensor, image_patches_mask: Optional[torch.Tensor] = None):

@@ -2,10 +2,11 @@
 CoCa encoder returns) and the parameter containers `TransformerEncoderLayer` / `TransformerEncoder` (:31-259) and
 `TransformerDecoderLayer` / `TransformerDecoder` (:262-657) — same constructors, state-dict keys and creation order.
 The layers execute inside `engine.TransformerStack` (fused kernels), owned by VisionTransformer / CoCaTextDecoder /
-CoCaMultimodalDecoder; all four are also callable on their own (same kernels: `engine_layers.py`).  A pre-norm
-`TransformerEncoderLayer` / `TransformerEncoder` is then a runtime owner like the encoders: one runtime on its own
-`TransformerStack` serves torch.no_grad() and training.  Post-norm layers and the decoders compute forward values, the
-decoders with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive decoding.
+CoCaMultimodalDecoder; all four are also callable on their own (same kernels: `engine_layers.py`).  A
+`TransformerEncoderLayer` / `TransformerEncoder` is then a runtime owner like the encoders: one runtime serves
+torch.no_grad() and training (pre-norm: its own `TransformerStack`; post-norm: `PostNormLayersRuntime`).  The decoders
+compute forward values, with the reference's key / value cache (`past_key_values` / `use_cache`) for autoregressive
+decoding.
 
 With `drop_path_rate` an encoder layer applies stochastic depth as the reference does: one shared
 `StochasticDepth(p, "row")` (modules/layers/stochastic_depth.py) is both `attention_dropout` and `feedforward_dropout`,
@@ -89,14 +90,22 @@ class TransformerEncoder(_RuntimeOwner):
         return encoder_forward(self, hidden_states, attention_mask, return_hidden_states)
 
 
+def _layers_runtime(owner, layers, final_ln):
+    from ...engine_layers import EncoderLayersRuntime, PostNormLayersRuntime
+    from ..._lib import MMBError
+
+    kinds = {layer.norm_first for layer in layers}
+    if len(kinds) != 1:
+        raise MMBError("TransformerEncoder: layers that mix pre-norm and post-norm are not on the accelerated path")
+    return (EncoderLayersRuntime if kinds.pop() else PostNormLayersRuntime)(owner, layers, final_ln)
+
+
 def _layer_runtime(mod):
-    from ...engine_layers import EncoderLayersRuntime
-    return EncoderLayersRuntime(mod, [mod], None)
+    return _layers_runtime(mod, [mod], None)
 
 
 def _encoder_runtime(mod):
-    from ...engine_layers import EncoderLayersRuntime
-    return EncoderLayersRuntime(mod, mod.layer, mod.final_layer_norm)
+    return _layers_runtime(mod, mod.layer, mod.final_layer_norm)
 
 
 TransformerEncoderLayer._runtime_cls = staticmethod(_layer_runtime)

@@ -15,7 +15,7 @@ from . import _lib
 from ._lib import MMBError
 
 EPI_BF16, EPI_BF16_ACT, EPI_BF16_DACT, EPI_F32 = 0, 1, 2, 3
-ACT_QUICK_GELU, ACT_GELU_ERF = 0, 1
+ACT_QUICK_GELU, ACT_GELU_ERF, ACT_RELU = 0, 1, 2
 
 _NULL = ctypes.c_void_p(0)
 
